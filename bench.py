@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py - sequences/sec of one biGRU train step on N B200s (BASELINE.json metric).
+"""bench.py - sequences/sec of one biGRU train step on N H100s (BASELINE.json metric).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--precision bf16|fp32]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--precision bf16|fp32] [--dump-outputs DIR]
   N>1: python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N
 
 A "step" is the body of the reference training loop (biGRU_model.py:198-210): zero_grad -> forward ->
@@ -11,7 +11,9 @@ bidirectional, 3 classes; weak scaling (per-GPU batch fixed, global batch = 512*
 The headline (`value`, `e2e`, `roofline`) is measured on the precision that meets north_star's tolerance (logits <= 1e-4
 rel of the reference's torch.nn.GRU path): "bf16x3", the fp32-class tensor-core path = BASELINE.json configs[1].  The
 pure-bf16 tensor-core path (configs[2], logits ~3e-3) is measured in the same run and reported under `variants`.
-Rank 0 prints ONE JSON line.  `--impl reference` times the reference's CPU implementation of the same
+Rank 0 prints ONE JSON line.  `--dump-outputs DIR` writes what the headline arm's last timed step returned (loss, logits)
+and the parameters that step left behind as DIR/<name>.npy, so that two builds can be compared output for output on the
+same seeded inputs.  `--impl reference` times the reference's CPU implementation of the same
 step (the oracle port: torch.nn.GRU on the host cores, as biGRU_model.py:54-56/:102 call it).
 """
 import argparse
@@ -45,7 +47,7 @@ def flops_train_per_seq(T, F, H, L, C, D=2):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -165,9 +167,9 @@ def run_reference(args):
     _emit(line)
 
 
-CONFIG_OF = {"bf16x3": "configs[1] (fused-gate tensor-core kernels at fp32 tolerance: split bf16x3 operands, fp32 accumulate)",
-             "fp32": "configs[1] (fp32 FFMA parity path)", "bf16": "configs[2] (bf16 tcgen05 gate GEMM)"}
-CONFIG_OF_C4 = {"bf16": "configs[4] (long sequence, hidden 512: 8-CTA-cluster persistent scans, bf16 tcgen05)",
+CONFIG_OF = {"bf16x3": "configs[1] (tensor-core kernels at fp32 tolerance: split bf16x3 operands, fp32 accumulate)",
+             "fp32": "configs[1] (fp32 FFMA parity path)", "bf16": "configs[2] (bf16 tensor-core GEMMs and scans)"}
+CONFIG_OF_C4 = {"bf16": "configs[4] (long sequence, hidden 512: 8-CTA-cluster persistent scans, bf16 tensor cores)",
                 "fp32": "configs[4] (long sequence, hidden 512, fp32 FFMA path)"}
 
 
@@ -183,7 +185,7 @@ def workload_config(n_gpus, precision, cpu=False, batch=None):
             "n_features": W["n_features"], "hidden": W["hidden"], "layers": W["layers"], "bidirectional": True,
             "classes": W["classes"], "loss": "CrossEntropyLoss", "optimizer": "Adam(lr=1e-3)+clip_grad_norm_(50)",
             "parallelism": "cpu" if cpu else f"dp{n_gpus}", "precision": precision,
-            "l2": "rotating input batches + >1 GB of activation traffic per step (>> 126 MB L2)"}
+            "l2": "rotating input batches + >1 GB of activation traffic per step (>> 50 MB L2)"}
 
 
 def main():
@@ -197,6 +199,8 @@ def main():
     ap.add_argument("--no-variants", action="store_true", help="skip the secondary precision (bf16) measurement")
     ap.add_argument("--config", default="c1", choices=["c1", "c4"],
                     help="c1: BASELINE.json configs[1] (the headline metric); c4: configs[4] long sequence (B256 T1024 F128 H512)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's loss, logits and updated parameters as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     global WORK, METRIC
     if args.config == "c4":
@@ -214,7 +218,7 @@ def main():
     from financial_market_data_analysis_b200.prefetch import DevicePrefetcher
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device; the B200 path has no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py: no CUDA device; the CUDA path has no CPU fallback (use --impl reference for the CPU arm)")
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -280,21 +284,28 @@ def main():
             ms = max_over_ranks(ms, dev)
         return ms, launches
 
-    def measure(prec, steps, warmup, with_e2e=True, with_roofline=True, clocks=False):
+    def measure(prec, steps, warmup, with_e2e=True, with_roofline=True, clocks=False, dump_dir=None):
         """value (device-resident inputs), e2e (pinned host inputs, H2D + loss D2H inside the timed region) and the live
         per-kernel-class roofline of one precision."""
         model = make_model(prec)
         out = {"precision": prec, "workload": (CONFIG_OF_C4 if args.config == "c4" else CONFIG_OF).get(prec)}
 
+        last = {}
+
         def step_resident(i):
             x, t = resident[i % NBUF]
-            model.train_step(x, t)
+            last["loss"], last["logits"] = model.train_step(x, t)
 
         sampler = ClockSampler(local)
         if clocks and rank == 0:
             sampler.start()
             time.sleep(0.3)
         ms, launches = timed(step_resident, steps, warmup)
+        if dump_dir is not None and rank == 0:
+            # the last timed step's results, before any later arm steps the model again (graph replays reuse the buffers)
+            out["_dump"] = {"loss": last["loss"].detach().float().reshape(1).cpu().numpy(),
+                            "logits": last["logits"].detach().float().cpu().numpy(),
+                            "params": model.flat_parameters().detach().float().cpu().numpy()}
         if clocks:
             out["clocks"] = sampler.stop() if rank == 0 else None
         ms_step = ms / steps
@@ -393,9 +404,9 @@ def main():
                     peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
                 except Exception:
                     pass
-                tf_peak = peaks.get("bf16_tflops_sustained") or 1400.0     # kernel timed inside a long step
-                hbm_peak = peaks.get("hbm_gbs") or 6650.0
-                src = "measured (MEASURED_PEAKS.json)" if peaks else "fallback (B200_PROFILING.md)"
+                tf_peak = peaks.get("bf16_tflops_sustained") or 989.0      # H100 SXM data sheet: dense bf16, 700 W
+                hbm_peak = peaks.get("hbm_gbs") or 3350.0                  # H100 SXM data sheet: HBM3
+                src = "measured (MEASURED_PEAKS.json)" if peaks else "H100 SXM data sheet (not reached; a power-limited card runs lower)"
                 if rows:
                     top = rows[0]
                     if top["flops"] > 0:
@@ -411,14 +422,6 @@ def main():
                     if prec == "bf16x3":
                         rl["note"] = ("achieved = ALGORITHMIC FLOPs (SURVEY 8(d): 2*3H*H per row-step, 2*M*N*K per GEMM) over measured time, against "
                                       "the bf16 peak; the fp32-class products issue 4x (recurrence) / 3x (GEMMs) that many bf16 tensor FLOPs")
-                    try:        # DRAM traffic of the dominant kernel from the committed ncu --set full capture (per launch)
-                        tr = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-                        ent = tr.get(prec, {}).get(top["name"])
-                        if ent:
-                            rl["traffic"] = ent["dram_bytes_per_launch"]
-                            rl["traffic_source"] = ent["source"]
-                    except Exception:
-                        pass
                     step_flops = flops_train_per_seq(T, F, H, L, C) * B
                     rl["step_model_tflops"] = step_flops / (ms_step * 1e-3) / 1e12
                     rl["step_frac_of_gemm_roofline"] = rl["step_model_tflops"] / tf_peak
@@ -428,8 +431,13 @@ def main():
         out["_model"] = model
         return out
 
-    head = measure(precision, args.steps, args.warmup, clocks=True)
+    head = measure(precision, args.steps, args.warmup, clocks=True, dump_dir=args.dump_outputs)
     model = head.pop("_model")
+    if "_dump" in head:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in head.pop("_dump").items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), arr.astype(np.float32))
 
     # ---- end to end THROUGH THE LOADER (SURVEY 8(f) N1): a host chunk -> device -> zero-copy windows ----------------
     e2e_windows = None
@@ -466,7 +474,7 @@ def main():
         e2e_windows = {"value": B * world / (ms_w / args.steps * 1e-3), "unit": "sequences/s", "ms_per_step": ms_w / args.steps,
                        "h2d_bytes_per_step": n_rows * (F + 1) * 4, "d2h_bytes_per_step": 4,
                        "how": "host chunk (B+T-1 rows x F + targets, pinned) -> device copy inside the timed region -> BiGRU.train_step_windows: the "
-                              "windowed collation, min-max normalisation and the cast are fused into the first kernel (no x[B,T,F] anywhere); "
+                              "windows are collated and min-max normalised on the device into x[B,T,F] (one gather kernel), then the step; "
                               "every step's loss is read back to the host through a pinned ring"}
     except Exception as e:                                      # the extra arm must never break the bench line
         e2e_windows = {"error": str(e)[:200]}
@@ -494,8 +502,7 @@ def main():
             with torch.no_grad():
                 want = ref(xs)
             parity = {"what": "max |logit - oracle logit| / max |oracle logit| on %d sequences of the benchmark shape (eval mode); "
-                              "the full-batch figures with gradients are in profiles/r02_parity_c%s.json (tests/test_gpu_parity.py)"
-                              % (xs.shape[0], "1" if args.config == "c1" else "4"),
+                              "the full-batch figures with gradients come from tests/test_gpu_parity.py" % xs.shape[0],
                       "tolerance": 1e-4 if args.config == "c1" else 3e-2}
             for prec in [precision] + list(variants):
                 m2 = pkg.BiGRU(H, F, C, L, 50, 0.0, False, True, precision=prec)

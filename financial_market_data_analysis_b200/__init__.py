@@ -1,4 +1,4 @@
-"""financial_market_data_analysis_b200 - B200-native (sm_100a) implementation of the one hot path of
+"""financial_market_data_analysis_b200 - H100-native (sm_90a) implementation of the one hot path of
 radoslawkrolikowski/financial-market-data-analysis: the bidirectional-GRU classifier
 (biGRU_model.py) and the windowed collation that feeds it (sql_pytorch_dataloader.py).
 

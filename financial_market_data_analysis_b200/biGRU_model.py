@@ -1,4 +1,4 @@
-"""B200-native drop-in for the reference's ``biGRU_model`` module.
+"""H100-native drop-in for the reference's ``biGRU_model`` module.
 
 ``BiGRU`` keeps the class surface of /root/reference/biGRU_model.py:8-286 - constructor
 argument order (:32-33), attribute names (:39-47), submodule names ``dropout`` /
@@ -6,7 +6,7 @@ argument order (:32-33), attribute names (:39-47), submodule names ``dropout`` /
 ``forward(input_seq, hidden=None)`` (:63), ``add_loss_fn`` / ``add_optimizer`` / ``add_device``
 (:141-159), ``train_model`` (:162) and ``evaluate_model`` (:227) with the same return tuples -
 but every floating-point operation of forward/backward, the loss, gradient clipping and the
-Adam update run in hand-written sm_100a CUDA kernels behind the C ABI of
+Adam update run in hand-written sm_90a CUDA kernels behind the C ABI of
 ``libbigru_b200.so`` (include/bigru_b200.h).  PyTorch only owns device memory, streams and the
 process group.  There is no CPU path: parameters must live on a CUDA device.
 """
@@ -202,10 +202,10 @@ class BiGRU(nn.Module):
     output_size, n_layers=1, clip=50, dropout=0.2, spatial_dropout=True, bidirectional=True.
     Extra keyword ``precision``:
       "fp32"    FFMA kernels, exact transcendental functions; any shape (the exact path),
-      "bf16x3"  fp32-class on tcgen05 tensor cores (every operand a (hi, lo) bf16 pair, fp32 accumulation / state /
+      "bf16x3"  fp32-class on tensor cores (every operand a (hi, lo) bf16 pair, fp32 accumulation / state /
                 gradients): meets the reference's 1e-4 logits tolerance; H in {128, 256} (other batch sizes than whole 32-row tiles
                 run zero-padded, any feature count),
-      "bf16"    single bf16 operands on tcgen05, fp32 accumulation and state (fastest, ~3e-3 on logits); H in {128, 256, 512},
+      "bf16"    single bf16 operands on tensor cores, fp32 accumulation and state (fastest, ~3e-3 on logits); H in {128, 256, 512},
       "auto"    "bf16x3" for hidden sizes up to 256 (smaller models run zero-padded to 128 / 256 hidden units), "fp32" beyond.
     Default: $BIGRU_B200_PRECISION or "auto" (the reference tolerance at tensor-core speed wherever the kernels apply).
     """
@@ -410,7 +410,7 @@ class BiGRU(nn.Module):
             self._flatten()
         dev = self._flat.device
         if dev.type != "cuda":
-            raise RuntimeError("BiGRU (B200-native) has no CPU path: move the model to a CUDA device with .cuda() first")
+            raise RuntimeError("BiGRU (H100-native) has no CPU path: move the model to a CUDA device with .cuda() first")
         if input_seq.dim() != 3 or input_seq.shape[2] != self.n_features:
             raise ValueError(f"input_seq must be [batch, seq_len, {self.n_features}], got {tuple(input_seq.shape)}")
         x = input_seq.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
@@ -597,7 +597,7 @@ class BiGRU(nn.Module):
         gradients are gathered only after the whole backward)."""
         if self._dp_world <= 1 or self.n_layers < 2 or "pflat" in st or self.resolved_precision() == "fp32":
             return 0
-        if os.environ.get("BIGRU_B200_DP_OVERLAP", "0") != "1":      # opt-in: measured no faster (two collectives cost more than the overlap wins)
+        if os.environ.get("BIGRU_B200_DP_OVERLAP", "0") != "1":      # opt-in: two collectives per step instead of one
             return 0
         per_dir0 = 3 * self.hidden_size * (self.n_features + self.hidden_size + 2)
         return self.n_directions * per_dir0

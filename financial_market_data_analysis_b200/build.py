@@ -1,4 +1,4 @@
-"""Builds libbigru_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds libbigru_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libbigru_b200.so")
 SOURCES = ["api.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v"]
 
 

@@ -1,8 +1,7 @@
 // api.cu - extern "C" entry points of libbigru_b200.so (see include/bigru_b200.h).
 #include "common.cuh"
 #include "kernels_f32.cuh"
-#include "path_bf16.cuh"
-#include "path_x3.cuh"
+#include "tc_hopper.cuh"
 #include "features.cuh"
 #include "infer_small.cuh"
 
@@ -29,8 +28,8 @@ extern "C" int bigru_device_check(int dev) {
     }
     cudaDeviceProp p;
     CUDA_TRY(cudaGetDeviceProperties(&p, dev));
-    if (p.major != 10) {
-        bigru_set_error("device %d is sm_%d%d; libbigru_b200 is built for sm_100a only", dev, p.major, p.minor);
+    if (p.major != 9 || p.minor != 0) {
+        bigru_set_error("device %d is sm_%d%d; libbigru_b200 is built for sm_90a (H100) only", dev, p.major, p.minor);
         return BIGRU_ERR_DEVICE;
     }
     return BIGRU_OK;
@@ -44,7 +43,7 @@ struct StashF32 {       // kept forward -> backward
     int64_t cat, arg, total;
 };
 struct ScratchF32 {
-    int64_t gi, gh, dgi, dgh, dYa, dYb, dhc, dcat, total;
+    int64_t gi, gh, dgi, dgh, dYa, dYb, dhc, dcat, csum, tcw, total;
 };
 static StashF32 stash_layout(const bigru_plan& p) {
     StashF32 s{};
@@ -73,8 +72,49 @@ static ScratchF32 scratch_layout(const bigru_plan& p) {
     s.dYb = o; o += BT * wide;
     s.dhc = o; o += (int64_t)p.D * p.B * p.H;
     s.dcat = o; o += (int64_t)p.B * 3 * p.H;
+    s.csum = o; o += (int64_t)COLSUM_MAX_CHUNKS * (3 * p.H > p.C ? 3 * p.H : p.C);   // colsum_launch partials
+    s.tcw = o;                                                                           // packed bf16 operands of tc_gemm_launch
+    if (p.prec != BIGRU_PREC_FP32) {
+        const int64_t H3 = 3LL * p.H, B = p.B, C = p.C, D = p.D;
+        int64_t need = 0;
+        for (int l = 0; l < p.L; ++l) {
+            const int64_t I = p.in_size(l);
+            const int64_t e[4] = {tc_gemm_ws_elems(BT, H3, I, D, p.prec),        // projection
+                                  tc_gemm_ws_elems(H3, I, BT, 1, p.prec),        // dW_ih
+                                  tc_gemm_ws_elems(BT, I, H3, 1, p.prec),        // dX
+                                  tc_gemm_ws_elems(H3, p.H, BT, 1, p.prec)};     // dW_hh
+            for (int64_t v : e) need = need > v ? need : v;
+        }
+        const int64_t h[4] = {tc_gemm_ws_elems(B, C, H3, 1, p.prec), tc_gemm_ws_elems(B, H3, C, 1, p.prec),
+                              tc_gemm_ws_elems(C, H3, B, 1, p.prec), tc_gemm_ws_elems(H3, p.H, B, 1, p.prec)};   // head, w0
+        for (int64_t v : h) need = need > v ? need : v;
+        o += (need + 1) / 2;
+    }
     s.total = o;
     return s;
+}
+
+// Shapes the tensor-core scans take: 64-unit slices per CTA (clusters of H/64), 16-row batch tiles.  bf16x3 needs hi/lo
+// weight pairs, which fit the 227 KB of shared memory per block up to H = 256; bf16 goes to H = 512.  The batch multiples
+// are those the Python mirror pads to.
+static int tc_plan_check(const bigru_plan& p) {
+    if (p.prec == BIGRU_PREC_BF16X3 && ((p.H != 128 && p.H != 256) || p.B % 32 != 0)) {
+        bigru_set_error("BIGRU_PREC_BF16X3 supports hidden_size 128 or 256 and batch %% 32 == 0 (got H=%d B=%d; the Python mirror pads "
+                        "other batch sizes with zero rows); use BIGRU_PREC_FP32 for other shapes", p.H, p.B);
+        return BIGRU_ERR_UNSUPPORTED;
+    }
+    if (p.prec == BIGRU_PREC_BF16 && !(((p.H == 128 || p.H == 256) && p.B % 16 == 0) || (p.H == 512 && p.B % 32 == 0))) {
+        bigru_set_error("BIGRU_PREC_BF16 supports hidden_size 128 or 256 with batch %% 16 == 0 and hidden_size 512 with batch %% 32 == 0 "
+                        "(got H=%d B=%d; the Python mirror pads other batch sizes with zero rows); use BIGRU_PREC_FP32 for other shapes", p.H, p.B);
+        return BIGRU_ERR_UNSUPPORTED;
+    }
+    return BIGRU_OK;
+}
+
+// GEMMs of a plan: FFMA on the fp32 path, tensor cores (bf16 or split bf16x3 operands) on the others
+static int plan_gemm(const bigru_plan& p, const GemmArgs& g, int cls, float* scratch, cudaStream_t st) {
+    return p.prec == BIGRU_PREC_FP32 ? sgemm_launch(g, st)
+                                     : tc_gemm_launch(g, p.prec, cls, reinterpret_cast<htc::bf16_t*>(scratch + scratch_layout(p).tcw), st);
 }
 
 extern "C" int bigru_plan_create(int B, int T, int F, int H, int L, int C, int bidirectional, int precision,
@@ -92,18 +132,12 @@ extern "C" int bigru_plan_create(int B, int T, int F, int H, int L, int C, int b
     if (!p) { bigru_set_error("plan_create: out of host memory"); return BIGRU_ERR_ARG; }
     p->B = B; p->T = T; p->F = F; p->H = H; p->L = L; p->C = C; p->D = bidirectional ? 2 : 1; p->prec = precision;
     p->nparams = p->off_linb() + C;
-    if (precision == BIGRU_PREC_BF16) {
-        int rc = bf16_plan_check(*p);
+    if (precision != BIGRU_PREC_FP32) {
+        int rc = tc_plan_check(*p);
         if (rc != BIGRU_OK) { delete p; return rc; }
-        bf16_workspace(*p, &p->stash_bytes, &p->scratch_bytes);
-    } else if (precision == BIGRU_PREC_BF16X3) {
-        int rc = x3_plan_check(*p);
-        if (rc != BIGRU_OK) { delete p; return rc; }
-        x3_workspace(*p, &p->stash_bytes, &p->scratch_bytes);
-    } else {
-        p->stash_bytes = (size_t)stash_layout(*p).total * sizeof(float);
-        p->scratch_bytes = (size_t)scratch_layout(*p).total * sizeof(float);
     }
+    p->stash_bytes = (size_t)stash_layout(*p).total * sizeof(float);
+    p->scratch_bytes = (size_t)scratch_layout(*p).total * sizeof(float);
     *out = p;
     return BIGRU_OK;
 }
@@ -142,20 +176,22 @@ extern "C" int bigru_workspace_bytes(const bigru_plan* p, size_t* stash_bytes, s
 // where the head keeps argmax_t of the pooled output (int32 [B][H]) inside the stash of the last forward
 extern "C" int bigru_stash_argmax_offset(const bigru_plan* p, size_t* byte_offset) {
     if (!p || !byte_offset) { bigru_set_error("stash_argmax_offset: null argument"); return BIGRU_ERR_ARG; }
-    if (p->prec == BIGRU_PREC_BF16) *byte_offset = bf16_layout(*p).arg;
-    else if (p->prec == BIGRU_PREC_BF16X3) *byte_offset = x3_layout(*p).arg;
-    else *byte_offset = (size_t)stash_layout(*p).arg * sizeof(float);
+    *byte_offset = (size_t)stash_layout(*p).arg * sizeof(float);
     return BIGRU_OK;
 }
 
 static inline unsigned nblk(int64_t n, int bs) { return (unsigned)cdiv64(n, bs); }
 
 // ------------------------------------------------------------------------------------------
-// fp32 forward
+// forward (all precisions share the layout; the recurrence and the GEMMs run on tensor cores except at fp32)
 // ------------------------------------------------------------------------------------------
-static int forward_f32(const bigru_plan& p, const float* params, const float* x, const float* h0, float drop,
-                       int spatial, int training, uint64_t seed, float* stash, float* scratch, float* logits,
-                       float* hn, cudaStream_t st) {
+static int forward_plan(const bigru_plan& p, const float* params, const float* x, const float* h0, float drop,
+                        int spatial, int training, uint64_t seed, float* stash, float* scratch, float* logits,
+                        float* hn, cudaStream_t st) {
+    if (p.prec == BIGRU_PREC_BF16 && h0) {
+        bigru_set_error("BIGRU_PREC_BF16: an initial hidden state is not supported; use BIGRU_PREC_FP32 or BIGRU_PREC_BF16X3");
+        return BIGRU_ERR_UNSUPPORTED;
+    }
     const StashF32 S = stash_layout(p);
     const ScratchF32 W = scratch_layout(p);
     const int B = p.B, T = p.T, H = p.H, D = p.D;
@@ -167,18 +203,23 @@ static int forward_f32(const bigru_plan& p, const float* params, const float* x,
         if (do_drop && (l == 0 || p.L > 1)) {
             // l == 0: input dropout (elementwise or per-channel); l > 0: nn.GRU inter-layer dropout
             float* xd = stash + S.X[l];
-            KLAUNCH(KC_MISC, 0.0, 0.0, st, dropout_kernel<<<148 * 8, 256, 0, st>>>(inp, xd, BT * I, T, I, l == 0 ? spatial : 0, drop, seed, (uint32_t)l));
+            KLAUNCH(KC_MISC, 0.0, 0.0, st, dropout_kernel<<<132 * 8, 256, 0, st>>>(inp, xd, BT * I, T, I, l == 0 ? spatial : 0, drop, seed, (uint32_t)l));
             inp = xd;
         }
         // gi[d] = X W_ih[d]^T + b_ih[d]   for both directions
         GemmArgs g = gemm_args(inp, params + p.off_wih(l, 0), scratch + W.gi, (int)BT, 3 * H, I, I, 1, I, 1, 3 * H);
         g.bias = params + p.off_bih(l, 0);
         g.batch = D; g.zA = 0; g.zB = p.ld_block(l); g.zBias = p.ld_block(l); g.zC = BT * 3 * H;
-        TRY(sgemm_launch(g, st));
+        TRY(plan_gemm(p, g, KC_TC_GEMM, scratch, st));
         float* Y = stash + S.Y[l];
         float* G = stash + S.G[l];
         const float* h0l = h0 ? h0 + (int64_t)l * D * B * H : nullptr;
         float* hnl = hn ? hn + (int64_t)l * D * B * H : nullptr;
+        if (p.prec != BIGRU_PREC_FP32) {
+            TRY(tc_scan_fwd(p, l, scratch + W.gi, params + p.off_whh(l, 0), params + p.off_bhh(l, 0), h0l, Y, G, hnl, st));
+            inp = Y;
+            continue;
+        }
         for (int s = 0; s < T; ++s) {
             // gh[d] = h_prev[d] W_hh[d]^T + b_hh[d];  h_prev rows live in Y (or h0 at s == 0)
             const float* hp; int64_t sam, zA;
@@ -208,49 +249,62 @@ static int forward_f32(const bigru_plan& p, const float* params, const float* x,
     KLAUNCH(KC_HEAD, 0.0, 0.0, st, head_pool_kernel<<<nblk((int64_t)B * H, 128), 128, 0, st>>>(Ytop, stash + S.cat, (int*)(stash + S.arg), B, T, H, D));
     GemmArgs lin = gemm_args(stash + S.cat, params + p.off_linw(), logits, B, p.C, 3 * H, 3 * H, 1, 3 * H, 1, p.C);
     lin.bias = params + p.off_linb();
-    TRY(sgemm_launch(lin, st));
+    TRY(plan_gemm(p, lin, KC_HEAD, scratch, st));
     return BIGRU_OK;
 }
 
 // ------------------------------------------------------------------------------------------
-// fp32 backward
+// backward of layers layer_from .. layer_to (descending); the head when layer_from is the top layer.  The upstream
+// gradient of layer l lives in dYa when L-1-l is even, else in dYb, so a split call picks up where the first left off.
 // ------------------------------------------------------------------------------------------
-static int backward_f32(const bigru_plan& p, const float* params, const float* x, const float* h0, float drop,
-                        int spatial, int training, uint64_t seed, const float* stash, float* scratch,
-                        const float* dlogits, float* grads, float* dx, float* dh0, cudaStream_t st) {
+static int backward_plan(const bigru_plan& p, const float* params, const float* x, const float* h0, float drop,
+                         int spatial, int training, uint64_t seed, const float* stash, float* scratch,
+                         const float* dlogits, float* grads, float* dx, float* dh0, cudaStream_t st,
+                         int layer_from, int layer_to) {
+    if (p.prec == BIGRU_PREC_BF16 && (h0 || dh0)) {
+        bigru_set_error("BIGRU_PREC_BF16: initial hidden state / its gradient are not supported");
+        return BIGRU_ERR_UNSUPPORTED;
+    }
     const StashF32 S = stash_layout(p);
     const ScratchF32 W = scratch_layout(p);
     const int B = p.B, T = p.T, H = p.H, D = p.D, C = p.C;
     const int64_t BT = (int64_t)B * T;
     const bool do_drop = training && drop > 0.f;
-    CUDA_TRY(cudaMemsetAsync(grads, 0, sizeof(float) * p.nparams, st));
-    // head: dcat = dlogits lin_w ; dlin_w = dlogits^T cat ; dlin_b = colsum(dlogits)
-    GemmArgs a = gemm_args(dlogits, params + p.off_linw(), scratch + W.dcat, B, 3 * H, C, C, 1, 1, 3 * H, 3 * H);
-    TRY(sgemm_launch(a, st));
-    GemmArgs w = gemm_args(dlogits, stash + S.cat, grads + p.off_linw(), C, 3 * H, B, 1, C, 1, 3 * H, 3 * H);
-    TRY(sgemm_launch(w, st));
-    TRY(colsum_launch(dlogits, grads + p.off_linb(), B, C, C, 1, 0, 0, st));
-    float* dY = scratch + W.dYa;
-    float* dYnext = scratch + W.dYb;
     float* dhc = scratch + W.dhc;
-    KLAUNCH(KC_HEAD, 0.0, 0.0, st, head_bwd_dy_kernel<<<nblk(BT * H, 256), 256, 0, st>>>(scratch + W.dcat, (const int*)(stash + S.arg), dY, dhc, B, T, H, D));
-    for (int l = p.L - 1; l >= 0; --l) {
+    if (layer_from == p.L - 1) {
+        CUDA_TRY(cudaMemsetAsync(grads, 0, sizeof(float) * p.nparams, st));
+        // head: dcat = dlogits lin_w ; dlin_w = dlogits^T cat ; dlin_b = colsum(dlogits)
+        GemmArgs a = gemm_args(dlogits, params + p.off_linw(), scratch + W.dcat, B, 3 * H, C, C, 1, 1, 3 * H, 3 * H);
+        TRY(plan_gemm(p, a, KC_HEAD, scratch, st));
+        GemmArgs w = gemm_args(dlogits, stash + S.cat, grads + p.off_linw(), C, 3 * H, B, 1, C, 1, 3 * H, 3 * H);
+        TRY(plan_gemm(p, w, KC_HEAD, scratch, st));
+        TRY(colsum_launch(dlogits, grads + p.off_linb(), B, C, C, 1, 0, 0, scratch + W.csum, st));
+        KLAUNCH(KC_HEAD, 0.0, 0.0, st, head_bwd_dy_kernel<<<nblk(BT * H, 256), 256, 0, st>>>(scratch + W.dcat, (const int*)(stash + S.arg), scratch + W.dYa, dhc, B, T, H, D));
+    }
+    for (int l = layer_from; l >= layer_to; --l) {
         const int I = (int)p.in_size(l);
+        const bool even = (p.L - 1 - l) % 2 == 0;
+        float* dY = scratch + (even ? W.dYa : W.dYb);
+        float* dYnext = scratch + (even ? W.dYb : W.dYa);
         const float* Y = stash + S.Y[l];
         const float* G = stash + S.G[l];
         const float* h0l = h0 ? h0 + (int64_t)l * D * B * H : nullptr;
         float* dgi = scratch + W.dgi;
         float* dgh = scratch + W.dgh;
         if (l != p.L - 1) CUDA_TRY(cudaMemsetAsync(dhc, 0, sizeof(float) * D * B * H, st));
-        for (int s = 0; s < T; ++s) {
-            KLAUNCH(KC_GATES_BWD, 0.0, 0.0, st, gru_gates_bwd_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(G, Y, h0l, dY, dhc, dgi, dgh, B, T, H, D, s));
-            // dhc[d] += dgh_t[d] W_hh[d]   (rows t: dir0 -> T-1-s, dir1 -> s)
-            const int t0 = T - 1 - s, t1 = s;
-            GemmArgs r = gemm_args(dgh + (int64_t)t0 * 3 * H, params + p.off_whh(l, 0), dhc, B, H, 3 * H,
-                                   (int64_t)T * 3 * H, 1, 1, H, H);
-            r.beta = 1; r.batch = D;
-            r.zA = BT * 3 * H + (int64_t)(t1 - t0) * 3 * H; r.zB = p.ld_block(l); r.zC = (int64_t)B * H;
-            TRY(sgemm_launch(r, st));
+        if (p.prec != BIGRU_PREC_FP32) {
+            TRY(tc_scan_bwd(p, l, G, Y, h0l, dY, dhc, dgi, dgh, params + p.off_whh(l, 0), st));
+        } else {
+            for (int s = 0; s < T; ++s) {
+                KLAUNCH(KC_GATES_BWD, 0.0, 0.0, st, gru_gates_bwd_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(G, Y, h0l, dY, dhc, dgi, dgh, B, T, H, D, s));
+                // dhc[d] += dgh_t[d] W_hh[d]   (rows t: dir0 -> T-1-s, dir1 -> s)
+                const int t0 = T - 1 - s, t1 = s;
+                GemmArgs r = gemm_args(dgh + (int64_t)t0 * 3 * H, params + p.off_whh(l, 0), dhc, B, H, 3 * H,
+                                       (int64_t)T * 3 * H, 1, 1, H, H);
+                r.beta = 1; r.batch = D;
+                r.zA = BT * 3 * H + (int64_t)(t1 - t0) * 3 * H; r.zB = p.ld_block(l); r.zC = (int64_t)B * H;
+                TRY(sgemm_launch(r, st));
+            }
         }
         if (dh0) CUDA_TRY(cudaMemcpyAsync(dh0 + (int64_t)l * D * B * H, dhc, sizeof(float) * D * B * H,
                                           cudaMemcpyDeviceToDevice, st));
@@ -264,24 +318,24 @@ static int backward_f32(const bigru_plan& p, const float* params, const float* x
             // dW_ih = dgi^T X
             GemmArgs wi = gemm_args(dgi_d, inp, grads + p.off_wih(l, d), 3 * H, I, (int)BT, 1, 3 * H, 1, I, I);
             wi.splitk = splitk;
-            TRY(sgemm_launch(wi, st));
+            TRY(plan_gemm(p, wi, KC_TC_GEMM_DWIH, scratch, st));
             // dW_hh = dgh^T H_prev ; H_prev(b,t) = Y[b,t-1] (dir 0) / Y[b,t+1] (dir 1), h0 at the first step
             if (T > 1) {
                 const float* hp = Y + (int64_t)d * H + (d == 0 ? -(int64_t)D * H : (int64_t)D * H);
                 GemmArgs wh = gemm_args(dgh_d, hp, grads + p.off_whh(l, d), 3 * H, H, (int)BT, 1, 3 * H, 1,
                                         (int64_t)D * H, H);
                 wh.splitk = splitk; wh.mask_period = T; wh.mask_skip = d == 0 ? 0 : T - 1;
-                TRY(sgemm_launch(wh, st));
+                TRY(plan_gemm(p, wh, KC_TC_GEMM_DWHH, scratch, st));
             }
             if (h0l) {
                 const int tf = d == 0 ? 0 : T - 1;
                 GemmArgs w0 = gemm_args(dgh_d + (int64_t)tf * 3 * H, h0l + (int64_t)d * B * H, grads + p.off_whh(l, d),
                                         3 * H, H, B, 1, (int64_t)T * 3 * H, 1, H, H);
                 w0.splitk = 2;       // forces the atomic-accumulate epilogue onto the existing sums
-                TRY(sgemm_launch(w0, st));
+                TRY(plan_gemm(p, w0, KC_TC_GEMM_DWHH, scratch, st));
             }
-            TRY(colsum_launch(dgi_d, grads + p.off_bih(l, d), BT, 3 * H, 3 * H, 1, 0, 0, st));
-            TRY(colsum_launch(dgh_d, grads + p.off_bhh(l, d), BT, 3 * H, 3 * H, 1, 0, 0, st));
+            TRY(colsum_launch(dgi_d, grads + p.off_bih(l, d), BT, 3 * H, 3 * H, 1, 0, 0, scratch + W.csum, st));
+            TRY(colsum_launch(dgh_d, grads + p.off_bhh(l, d), BT, 3 * H, 3 * H, 1, 0, 0, scratch + W.csum, st));
         }
         // dX = sum_d dgi[d] W_ih[d]
         float* dxo = l == 0 ? dx : dYnext;
@@ -290,14 +344,13 @@ static int backward_f32(const bigru_plan& p, const float* params, const float* x
                 GemmArgs gx = gemm_args(dgi + (int64_t)d * BT * 3 * H, params + p.off_wih(l, d), dxo, (int)BT, I, 3 * H,
                                         3 * H, 1, 1, I, I);
                 gx.beta = d;
-                TRY(sgemm_launch(gx, st));
+                TRY(plan_gemm(p, gx, KC_TC_GEMM_DX, scratch, st));
             }
             if (do_drop && (l == 0 || p.L > 1)) {
                 // d(dropout): same mask, in place.  dropout_kernel(in=dxo) multiplies by mask/(1-p)
-                KLAUNCH(KC_MISC, 0.0, 0.0, st, dropout_kernel<<<148 * 8, 256, 0, st>>>(dxo, dxo, BT * I, T, I, l == 0 ? spatial : 0, drop, seed, (uint32_t)l));
+                KLAUNCH(KC_MISC, 0.0, 0.0, st, dropout_kernel<<<132 * 8, 256, 0, st>>>(dxo, dxo, BT * I, T, I, l == 0 ? spatial : 0, drop, seed, (uint32_t)l));
             }
         }
-        float* tmp = dY; dY = dYnext; dYnext = tmp;
     }
     return BIGRU_OK;
 }
@@ -313,15 +366,8 @@ extern "C" int bigru_forward(const bigru_plan* plan, const float* d_params, cons
         return BIGRU_ERR_ARG;
     }
     if (dropout_p < 0.f || dropout_p >= 1.f) { bigru_set_error("forward: dropout_p must be in [0,1)"); return BIGRU_ERR_ARG; }
-    cudaStream_t st = (cudaStream_t)stream;
-    if (plan->prec == BIGRU_PREC_BF16)
-        return forward_bf16(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, d_stash, d_scratch,
-                            d_logits, d_hn, st);
-    if (plan->prec == BIGRU_PREC_BF16X3)
-        return forward_x3(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, d_stash, d_scratch,
-                          d_logits, d_hn, st);
-    return forward_f32(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, (float*)d_stash,
-                       (float*)d_scratch, d_logits, d_hn, st);
+    return forward_plan(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, (float*)d_stash,
+                        (float*)d_scratch, d_logits, d_hn, (cudaStream_t)stream);
 }
 
 extern "C" int bigru_backward(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
@@ -332,15 +378,8 @@ extern "C" int bigru_backward(const bigru_plan* plan, const float* d_params, con
         bigru_set_error("backward: null argument");
         return BIGRU_ERR_ARG;
     }
-    cudaStream_t st = (cudaStream_t)stream;
-    if (plan->prec == BIGRU_PREC_BF16)
-        return backward_bf16(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, d_stash, d_scratch,
-                             d_dlogits, d_grads, d_dx, d_dh0, st);
-    if (plan->prec == BIGRU_PREC_BF16X3)
-        return backward_x3(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, d_stash, d_scratch,
-                           d_dlogits, d_grads, d_dx, d_dh0, st);
-    return backward_f32(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, (const float*)d_stash,
-                        (float*)d_scratch, d_dlogits, d_grads, d_dx, d_dh0, st);
+    return backward_plan(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, (const float*)d_stash,
+                         (float*)d_scratch, d_dlogits, d_grads, d_dx, d_dh0, (cudaStream_t)stream, plan->L - 1, 0);
 }
 
 extern "C" int bigru_backward_layers(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
@@ -355,15 +394,12 @@ extern "C" int bigru_backward_layers(const bigru_plan* plan, const float* d_para
         bigru_set_error("backward_layers: bad layer range %d..%d for %d layers", layer_from, layer_to, plan->L);
         return BIGRU_ERR_ARG;
     }
-    cudaStream_t st = (cudaStream_t)stream;
-    if (plan->prec == BIGRU_PREC_BF16)
-        return backward_bf16(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, d_stash, d_scratch,
-                             d_dlogits, d_grads, d_dx, d_dh0, st, layer_from, layer_to);
-    if (plan->prec == BIGRU_PREC_BF16X3)
-        return backward_x3(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, d_stash, d_scratch,
-                           d_dlogits, d_grads, d_dx, d_dh0, st, layer_from, layer_to);
-    bigru_set_error("backward_layers: the fp32 path runs its layers in one call (bigru_backward)");
-    return BIGRU_ERR_UNSUPPORTED;
+    if (plan->prec == BIGRU_PREC_FP32) {
+        bigru_set_error("backward_layers: the fp32 path runs its layers in one call (bigru_backward)");
+        return BIGRU_ERR_UNSUPPORTED;
+    }
+    return backward_plan(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, (const float*)d_stash,
+                         (float*)d_scratch, d_dlogits, d_grads, d_dx, d_dh0, (cudaStream_t)stream, layer_from, layer_to);
 }
 
 extern "C" int bigru_forward_windows(const bigru_plan* plan, const float* d_params, const float* d_src, const float* d_xmin,
@@ -380,18 +416,11 @@ extern "C" int bigru_forward_windows(const bigru_plan* plan, const float* d_para
         return BIGRU_ERR_ARG;
     }
     if (dropout_p < 0.f || dropout_p >= 1.f) { bigru_set_error("forward_windows: dropout_p must be in [0,1)"); return BIGRU_ERR_ARG; }
-    cudaStream_t st = (cudaStream_t)stream;
-    if (plan->prec == BIGRU_PREC_BF16)
-        return forward_bf16(*plan, d_params, nullptr, nullptr, dropout_p, spatial, training, seed, d_stash, d_scratch,
-                            d_logits, d_hn, st, WindowSrc{d_src, d_xmin, d_xmax, start});
-    if (plan->prec == BIGRU_PREC_BF16X3)
-        return forward_x3(*plan, d_params, nullptr, nullptr, dropout_p, spatial, training, seed, d_stash, d_scratch,
-                          d_logits, d_hn, st, WindowSrc{d_src, d_xmin, d_xmax, start});
-    // fp32 path: collate into the stash slot of the layer-0 input, then the ordinary forward
+    // collate into the stash slot of the layer-0 input (the backward reads it there), then the ordinary forward
     float* xw = (float*)d_stash + stash_layout(*plan).X[0];
     TRY(bigru_window_gather_norm(d_src, d_xmin, d_xmax, start, N, plan->B, plan->T, plan->F, xw, stream));
-    return forward_f32(*plan, d_params, xw, nullptr, dropout_p, spatial, training, seed, (float*)d_stash,
-                       (float*)d_scratch, d_logits, d_hn, st);
+    return forward_plan(*plan, d_params, xw, nullptr, dropout_p, spatial, training, seed, (float*)d_stash,
+                        (float*)d_scratch, d_logits, d_hn, (cudaStream_t)stream);
 }
 
 extern "C" int bigru_chunk_minmax(const float* d_table, int64_t N, int F, int64_t row_lo, int64_t row_hi, float* d_min,
@@ -446,7 +475,7 @@ extern "C" int bigru_window_features(const float* d_close, const float* d_high, 
     if (smem > 48 * 1024)        // per-device opt-in, set on every call (no process-wide cache: a second GPU would miss it)
         CUDA_TRY(fast ? cudaFuncSetAttribute(window_features_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
                       : cudaFuncSetAttribute(window_features_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const unsigned blocks = (unsigned)std::min<int64_t>((n + FEAT_TR - 1) / FEAT_TR, 148 * 8);
+    const unsigned blocks = (unsigned)std::min<int64_t>((n + FEAT_TR - 1) / FEAT_TR, 132 * 8);
     if (fast)
         KLAUNCH(KC_GATHER, 0.0, 4.0 * n * (5 + cfg.n_out + 4), (cudaStream_t)stream,
                 window_features_kernel<true><<<blocks, FEAT_TR, smem, (cudaStream_t)stream>>>(d_close, d_high, d_low, d_volume, d_delta, n, cfg,
@@ -496,7 +525,7 @@ extern "C" int bigru_loss(int kind, const float* d_logits, const void* d_target,
 extern "C" int bigru_sqnorm(const float* d_g, int64_t n, float* d_out, void* stream) {
     if (!d_g || !d_out || n < 0) { bigru_set_error("sqnorm: bad argument"); return BIGRU_ERR_ARG; }
     if (n == 0) return BIGRU_OK;
-    const unsigned blocks = (unsigned)min((int64_t)148 * 4, cdiv64(n, 256));
+    const unsigned blocks = (unsigned)min((int64_t)132 * 4, cdiv64(n, 256));
     KLAUNCH(KC_OPTIM, 0.0, 0.0, (cudaStream_t)stream, sqnorm_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d_g, n, d_out));
     return BIGRU_OK;
 }
@@ -509,7 +538,7 @@ extern "C" int bigru_clip_adam_step(float* d_params, float* d_grads, float* d_m,
         return BIGRU_ERR_ARG;
     }
     const double bc1 = 1.0 - pow((double)b1, step), bc2 = 1.0 - pow((double)b2, step);
-    const unsigned blocks = (unsigned)min((int64_t)148 * 8, cdiv64(n, 256));
+    const unsigned blocks = (unsigned)min((int64_t)132 * 8, cdiv64(n, 256));
     KLAUNCH(KC_OPTIM, 0.0, 0.0, (cudaStream_t)stream, clip_adam_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d_params, d_grads, d_m, d_v, n, d_sqnorm, clip, lr, b1,
                                                                 b2, eps, (float)bc1, (float)sqrt(bc2), grad_scale));
     return BIGRU_OK;
@@ -528,7 +557,7 @@ extern "C" int bigru_clip_adam_step_dev(float* d_params, float* d_grads, float* 
         bigru_set_error("clip_adam_step_dev: bad argument");
         return BIGRU_ERR_ARG;
     }
-    const unsigned blocks = (unsigned)min((int64_t)148 * 8, cdiv64(n, 256));
+    const unsigned blocks = (unsigned)min((int64_t)132 * 8, cdiv64(n, 256));
     KLAUNCH(KC_OPTIM, 0.0, 0.0, (cudaStream_t)stream, clip_adam_dev_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d_params, d_grads, d_m, d_v, n, d_sqnorm, clip,
                                                                     lr, b1, b2, eps, d_step, grad_scale));
     return BIGRU_OK;
@@ -546,7 +575,7 @@ extern "C" int bigru_window_gather_norm(const float* d_src, const float* d_xmin,
     const bool vec = F % 4 == 0 && ((uintptr_t)d_src % 16 == 0) && ((uintptr_t)d_out % 16 == 0) &&
                      (!d_xmin || (((uintptr_t)d_xmin % 16 == 0) && ((uintptr_t)d_xmax % 16 == 0)));
     const int64_t total = (int64_t)B * T * (vec ? F / 4 : F);
-    const unsigned blocks = (unsigned)min((int64_t)148 * 16, cdiv64(total, 256));
+    const unsigned blocks = (unsigned)min((int64_t)132 * 16, cdiv64(total, 256));
     // algorithmic bytes: write B*T*F floats, read the (B+T-1)*F source rows once (SURVEY.md 8(d))
     const double bytes = 4.0 * ((double)B * T * F + (double)(B + T - 1) * F);
     if (vec) KLAUNCH(KC_GATHER, 0.0, bytes, st, window_gather_kernel<4><<<blocks, 256, 0, st>>>(d_src, d_xmin, d_xmax, start, B, T, F, d_out));

@@ -1,4 +1,4 @@
-// common.cuh - shared declarations for libbigru_b200.so (sm_100a only).
+// common.cuh - shared declarations for libbigru_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>

@@ -1,6 +1,6 @@
 // kernels_f32.cuh - the fp32 (FFMA) path: strided SGEMM, GRU gate math forward/backward,
 // pooling head, losses, clip+Adam, window gather, dropout.  This is the parity path
-// (BIGRU_PREC_FP32); the bf16 tcgen05 path reuses the pointwise pieces.
+// (BIGRU_PREC_FP32); the tensor-core precisions reuse the layout, head, loss and optimiser kernels.
 #pragma once
 #include "common.cuh"
 
@@ -110,7 +110,7 @@ static int sgemm_launch(const GemmArgs& g, cudaStream_t st) {
     if (g.M <= 0 || g.N <= 0 || g.K <= 0) return BIGRU_OK;
     ProfScope ps(KC_SGEMM, 2.0 * g.M * g.N * (double)g.K * g.batch, 0.0, st);
     const int64_t big_tiles = cdiv64(g.M, 128) * cdiv64(g.N, 128) * g.batch * g.splitk;
-    const bool big = big_tiles >= 96 && g.M >= 64 && g.N >= 64;   // enough 128x128 tiles to fill 148 SMs
+    const bool big = big_tiles >= 132 && g.M >= 64 && g.N >= 64;  // enough 128x128 tiles to fill 132 SMs
     if (big) {
         dim3 grid((g.N + 127) / 128, (g.M + 127) / 128, g.batch * g.splitk);
         sgemm_kernel<128, 128, 16, 8, 8><<<grid, 256, 0, st>>>(g);
@@ -122,9 +122,12 @@ static int sgemm_launch(const GemmArgs& g, cudaStream_t st) {
     return BIGRU_OK;
 }
 
-// column sums: out[z][c] += sum_r A[z][r*ld + c]   (out pre-zeroed)
-__global__ void colsum_kernel(const float* __restrict__ A, float* __restrict__ out, int64_t rows, int cols,
-                              int64_t ld, int64_t zA, int64_t zOut, int rows_per_block) {
+// column sums: out[z][c] += sum_r A[z][r*ld + c], in a fixed order so that a gradient is the same from run to run (a step
+// replayed from a CUDA graph matches plain launches bit for bit): block (x, y, z) sums its row chunk into ws, then
+// colsum_finish_kernel adds the chunks in chunk order.  ws holds COLSUM_MAX_CHUNKS * cols * batch floats.
+constexpr int COLSUM_MAX_CHUNKS = 64;
+__global__ void colsum_kernel(const float* __restrict__ A, float* __restrict__ ws, int64_t rows, int cols,
+                              int64_t ld, int64_t zA, int rows_per_block) {
     __shared__ float sm[8][33];
     const float* a = A + blockIdx.z * zA;
     const int c = blockIdx.x * 32 + threadIdx.x;
@@ -139,15 +142,27 @@ __global__ void colsum_kernel(const float* __restrict__ A, float* __restrict__ o
         float t = 0.f;
 #pragma unroll
         for (int i = 0; i < 8; ++i) t += sm[i][threadIdx.x];
-        atomicAdd(out + blockIdx.z * zOut + c, t);
+        ws[((int64_t)blockIdx.z * gridDim.y + blockIdx.y) * cols + c] = t;
     }
 }
+__global__ void colsum_finish_kernel(const float* __restrict__ ws, float* __restrict__ out, int nchunks, int cols, int batch,
+                                     int64_t zOut) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (int64_t)cols * batch) return;
+    const int c = i % cols, z = i / cols;
+    float t = 0.f;
+    for (int k = 0; k < nchunks; ++k) t += ws[((int64_t)z * nchunks + k) * cols + c];
+    out[z * zOut + c] += t;
+}
 static int colsum_launch(const float* A, float* out, int64_t rows, int cols, int64_t ld, int batch, int64_t zA,
-                         int64_t zOut, cudaStream_t st) {
+                         int64_t zOut, float* ws, cudaStream_t st) {
     ProfScope ps(KC_MISC, 0.0, 4.0 * rows * cols * batch, st);
-    int rpb = (int)max((int64_t)256, cdiv64(rows, 64));
-    dim3 grid((cols + 31) / 32, (unsigned)cdiv64(rows, rpb), batch);
-    colsum_kernel<<<grid, dim3(32, 8), 0, st>>>(A, out, rows, cols, ld, zA, zOut, rpb);
+    const int rpb = (int)max((int64_t)256, cdiv64(rows, COLSUM_MAX_CHUNKS));
+    const int nchunks = (int)cdiv64(rows, rpb);
+    dim3 grid((cols + 31) / 32, nchunks, batch);
+    colsum_kernel<<<grid, dim3(32, 8), 0, st>>>(A, ws, rows, cols, ld, zA, rpb);
+    LAUNCH_CHECK();
+    colsum_finish_kernel<<<(unsigned)cdiv64((int64_t)cols * batch, 256), 256, 0, st>>>(ws, out, nchunks, cols, batch, zOut);
     LAUNCH_CHECK();
     return BIGRU_OK;
 }

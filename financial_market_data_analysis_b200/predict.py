@@ -1,4 +1,4 @@
-"""The model side of the reference's live predictor (``predict.py``) on the B200 path (SURVEY.md 8(f) N5).
+"""The model side of the reference's live predictor (``predict.py``) on the H100 path (SURVEY.md 8(f) N5).
 
 ``predict.py`` builds ``BiGRU(hidden_size=8, n_features, output_size=4, n_layers=1, clip=50, dropout=0.2,
 spatial_dropout=False, bidirectional=True)`` (``:73-88``), loads ``model_params.pt`` (``:104``) and the pickled

@@ -1,7 +1,7 @@
 """Host -> device input pipeline for the training loop: batches that live in (pinned) host memory are copied to the
 GPU on a side stream one step ahead of their use, so the H2D transfer of step i+1 overlaps the kernels of step i.
 The reference feeds CPU tensors from a DataLoader straight into the model (biGRU_model.py:189-200); this is the
-B200 counterpart for callers that keep their batches on the host."""
+H100 counterpart for callers that keep their batches on the host."""
 from __future__ import annotations
 
 import torch

@@ -1,4 +1,4 @@
-"""B200-native drop-in for the reference's ``sql_pytorch_dataloader`` module.
+"""H100-native drop-in for the reference's ``sql_pytorch_dataloader`` module.
 
 Same public names and constructor signatures as /root/reference/sql_pytorch_dataloader.py
 (``window_indices`` :8, ``MySQLChunkLoader`` :21, ``MySQLBatchLoader`` :162, ``TrainValTestSplit`` :251).
@@ -190,7 +190,7 @@ class MySQLBatchLoader(Dataset):
 
         if device is None:
             if not torch.cuda.is_available():
-                raise RuntimeError("MySQLBatchLoader (B200-native) keeps the chunk in HBM and collates with a CUDA "
+                raise RuntimeError("MySQLBatchLoader (H100-native) keeps the chunk in HBM and collates with a CUDA "
                                    "kernel; no CUDA device is available and there is no CPU fallback")
             device = torch.device("cuda", torch.cuda.current_device())
         self.device = torch.device(device)
@@ -216,7 +216,7 @@ class MySQLBatchLoader(Dataset):
             device = x_rows.device if x_rows.is_cuda else torch.device("cuda", torch.cuda.current_device())
         self.device = torch.device(device)
         if self.device.type != "cuda":
-            raise RuntimeError("MySQLBatchLoader (B200-native) keeps the chunk in HBM; there is no CPU fallback")
+            raise RuntimeError("MySQLBatchLoader (H100-native) keeps the chunk in HBM; there is no CPU fallback")
         self.window = int(window)
         self.x_raw = x_rows.to(self.device, torch.float32).contiguous()
         self.y = y_rows.to(self.device, torch.float32).contiguous()

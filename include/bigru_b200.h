@@ -1,4 +1,4 @@
-/* bigru_b200.h - C ABI of libbigru_b200.so: the B200 (sm_100a) biGRU hot path.
+/* bigru_b200.h - C ABI of libbigru_b200.so: the H100 (sm_90a) biGRU hot path.
  *
  * The reference (radoslawkrolikowski/financial-market-data-analysis) has no FFI layer of its
  * own: its hot path is the Python class surface of biGRU_model.py / sql_pytorch_dataloader.py,
@@ -34,14 +34,14 @@ extern "C" {
 #define BIGRU_OK               0
 #define BIGRU_ERR_ARG         -1   /* bad shape / null pointer / unsupported combination */
 #define BIGRU_ERR_CUDA        -2   /* a CUDA runtime call failed (message has the reason) */
-#define BIGRU_ERR_DEVICE      -3   /* no sm_100-class device */
+#define BIGRU_ERR_DEVICE      -3   /* no sm_90 (H100) device */
 #define BIGRU_ERR_UNSUPPORTED -4   /* shape not supported by the requested precision path */
 
 #define BIGRU_PREC_FP32 0          /* fp32 FFMA path: exact, any shape (<=1e-4 rel on logits) */
-#define BIGRU_PREC_BF16 1          /* bf16 operands on tcgen05 tensor cores, fp32 accumulate/state.
+#define BIGRU_PREC_BF16 1          /* bf16 operands on tensor cores, fp32 accumulate/state.
                                       hidden_size 128 or 256 with batch % 16 == 0, hidden_size 512 with batch % 32 == 0
                                       (BASELINE.json configs[4]); no initial hidden state */
-#define BIGRU_PREC_BF16X3 2        /* fp32-class on tensor cores: (hi, lo) bf16 operand pairs, 3-4 products per term,
+#define BIGRU_PREC_BF16X3 2        /* fp32-class on tensor cores: (hi, lo) bf16 operand pairs, 3 products per term,
                                       fp32 accumulate / gate math / stash; meets the 1e-4 logit tolerance at tensor-core speed.
                                       hidden_size 128 or 256, batch % 32 == 0.
                                       Both tensor-core paths take any n_features (the layer-0 operands are stored with the

@@ -1,5 +1,5 @@
 """GPU parity tests: the CUDA path (through the C ABI) against the oracle and the golden fixtures.
-Run on the B200 box:  python -m pytest tests -m gpu -x -q"""
+Run on an H100:  python -m pytest tests -m gpu -x -q"""
 import json
 import os
 
@@ -195,7 +195,7 @@ SWEEP = [  # B, T, F, H, L, C, bidir, h0
     (64, 2, 16, 256, 2, 2, True, True),
     (32, 300, 8, 256, 1, 2, True, False),     # many steps: barrier phase bookkeeping of the ping-pong scans far beyond the ring depths
     (32, 1, 16, 512, 1, 2, True, False),
-    (64, 6, 24, 512, 2, 3, True, False),      # hidden 512 (bf16 path: 8-CTA clusters, tc_scan_w.cuh), two batch tiles
+    (64, 6, 24, 512, 2, 3, True, False),      # hidden 512 (bf16 path: 8-CTA clusters, tc_hopper.cuh), two batch tiles
     (40, 3, 128, 512, 1, 2, False, False),
 ]
 
@@ -611,7 +611,7 @@ def test_model_on_a_device_that_is_not_current():
 
 def test_long_sequence_config_reduced():
     """BASELINE config 4 (B256,T1024,F128,H512,L2) at reduced batch/length on the exact FFMA path (logits <= 1e-4 rel of the
-    torch.nn.GRU CPU path); the bf16x3 path must refuse H = 512 loudly (its split weights do not fit tensor memory)."""
+    torch.nn.GRU CPU path); the bf16x3 path must refuse H = 512 loudly (its split weights do not fit an H100 block's shared memory)."""
     B, T, F, H, L, C = 16, 256, 128, 512, 2, 3
     torch.manual_seed(0)
     ref = bo.OracleBiGRU(H, F, C, L, 50, 0.0, False, True)
@@ -634,7 +634,7 @@ def test_long_sequence_config_reduced():
 
 def test_long_sequence_config_on_tensor_cores():
     """BASELINE configs[4] at its FULL sequence length, feature count and hidden size (T1024, F128, H512, L2, bidirectional) on the
-    persistent 8-CTA-cluster tensor-core kernels (precision="bf16", tc_scan_w.cuh), batch 64 so that the torch.nn.GRU CPU
+    persistent 8-CTA-cluster tensor-core kernels (precision="bf16", tc_hopper.cuh), batch 64 so that the torch.nn.GRU CPU
     oracle (forward + autograd) finishes in about a minute: logits and every gradient against the oracle at the bf16 path's
     tolerances, the training step against the exact FFMA path's loss."""
     if "bf16" not in precisions():

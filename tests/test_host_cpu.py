@@ -292,7 +292,7 @@ def test_next_row_entry_points_refuse_the_cpu(pkg):
 def test_drop_in_import_route(tmp_path):
     """INTEGRATION.md: with the package directory itself on sys.path the reference's own import lines
     (`from biGRU_model import BiGRU`, predict.py:16; `from sql_pytorch_dataloader import ...`, the notebook) resolve
-    to the B200 implementation - checked in a fresh interpreter started outside the repo."""
+    to the H100 implementation - checked in a fresh interpreter started outside the repo."""
     import subprocess
     code = (
         "import sys; sys.path.insert(0, %r)\n"

@@ -1,5 +1,5 @@
 """Train-step time of the reference's OWN model shapes (notebook: F=108, H=32, window 30, batch 2; predict.py: H=8, window 5) on
-the exact FFMA path vs precision="auto" (zero-padded onto the fp32-class tensor-core kernels).  GPU box: python tools/small_shapes_bench.py"""
+the exact FFMA path vs precision="auto" (zero-padded onto the fp32-class tensor-core kernels).  Usage: python tools/small_shapes_bench.py [OUT.json]"""
 import json, os, sys, time
 import torch, torch.nn as nn
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -27,4 +27,5 @@ for name, (B, T, F, H, L, C, drop) in {"notebook (B2 T30 F108 H32 L2, dropout 0.
         row[prec + "_runs_as"] = m.resolved_precision(B) + (f" (hidden {m.plan_hidden(B)})" if m.plan_hidden(B) != H else "")
     out.append(row)
     print(row)
-json.dump(out, open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out", "r02_small_shapes.json"), "w"), indent=1)
+if len(sys.argv) > 1:                  # optional output path for the rows as JSON
+    json.dump(out, open(sys.argv[1], "w"), indent=1)
