@@ -13,6 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libbigru_b200.so")
 
 PREC_FP32, PREC_BF16, PREC_BF16X3 = 0, 1, 2
+SQNORM_WS = 528                     # BIGRU_SQNORM_WS: floats of scratch bigru_sqnorm needs
 LOSS_CE, LOSS_BCE, LOSS_MLSM = 0, 1, 2
 ERR_ARG, ERR_CUDA, ERR_DEVICE, ERR_UNSUPPORTED = -1, -2, -3, -4
 
@@ -33,7 +34,7 @@ SIGNATURES = {
     "bigru_backward": (_i, [_vp, _vp, _vp, _vp, _f, _i, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_backward_layers": (_i, [_vp, _vp, _vp, _vp, _f, _i, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     "bigru_loss": (_i, [_i, _vp, _vp, _vp, _vp, _i, _i, _d, _vp, _vp, _vp]),
-    "bigru_sqnorm": (_i, [_vp, _i64, _vp, _vp]),
+    "bigru_sqnorm": (_i, [_vp, _i64, _vp, _vp, _vp]),
     "bigru_clip_adam_step": (_i, [_vp, _vp, _vp, _vp, _i64, _vp, _f, _f, _f, _f, _f, _i, _f, _vp]),
     "bigru_adam_tick": (_i, [_vp, _vp, _vp]),
     "bigru_clip_adam_step_dev": (_i, [_vp, _vp, _vp, _vp, _i64, _vp, _f, _f, _f, _f, _f, _vp, _f, _vp]),

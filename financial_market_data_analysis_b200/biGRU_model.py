@@ -517,7 +517,8 @@ class BiGRU(nn.Module):
             st = self._adam = {"m": torch.zeros_like(self._flat), "v": torch.zeros_like(self._flat), "step": 0,
                                "dstep": torch.zeros(1, device=dev, dtype=torch.int32),
                                "gext": gext, "grad": gext[:P], "loss": gext[P:P + 1],
-                               "scal": torch.zeros(2, device=dev, dtype=torch.float32)}
+                               "scal": torch.zeros(2, device=dev, dtype=torch.float32),
+                               "sqws": torch.empty(_lib.SQNORM_WS, device=dev, dtype=torch.float32)}
             pm = self._pad_map(dev)
             if pm is not None:                                # zero-padded hidden units (plan_hidden): the plan's own parameter / gradient vectors
                 st["pflat"] = torch.zeros(pm[1], device=dev, dtype=torch.float32)
@@ -620,7 +621,7 @@ class BiGRU(nn.Module):
         """clip_grad_norm_(clip) + Adam on the flat buffers; the step counter is incremented on the device."""
         sq = st["scal"][1:2]
         _lib.check(lib.bigru_adam_tick(_lib.ptr(st["dstep"]), _lib.ptr(sq), s), "bigru_adam_tick")
-        _lib.check(lib.bigru_sqnorm(_lib.ptr(st["grad"]), st["grad"].numel(), _lib.ptr(sq), s), "bigru_sqnorm")
+        _lib.check(lib.bigru_sqnorm(_lib.ptr(st["grad"]), st["grad"].numel(), _lib.ptr(sq), _lib.ptr(st["sqws"]), s), "bigru_sqnorm")
         b1, b2 = g["betas"]
         _lib.check(lib.bigru_clip_adam_step_dev(_lib.ptr(self._flat), _lib.ptr(st["grad"]), _lib.ptr(st["m"]),
                                                 _lib.ptr(st["v"]), self._flat.numel(), _lib.ptr(sq), float(self.clip),

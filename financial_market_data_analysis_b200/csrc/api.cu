@@ -38,13 +38,21 @@ extern "C" int bigru_device_check(int dev) {
 // ------------------------------------------------------------------------------------------
 // workspace carve-up (fp32 path).  Offsets in floats.
 // ------------------------------------------------------------------------------------------
+// Tensor-core precisions add bf16 planes of the GEMM operands (hi, and lo at bf16x3; see tc_hopper.cuh) in their
+// producers' layouts.  Plane offsets are rounded to 64 floats: TMA needs 16-byte aligned bases.
 struct StashF32 {       // kept forward -> backward
     int64_t Y[16], G[16], X[16];   // per layer: output [B*T*D*H], gates [D][B*T][4H], dropped input [B*T*I_l]
+    int64_t YP[16], XP[16];        // per layer: planes of Y [B*T][D*H] and of the layer input [B*T][in_pitch(l)]
     int64_t cat, arg, total;
 };
 struct ScratchF32 {
-    int64_t gi, gh, dgi, dgh, dYa, dYb, dhc, dcat, csum, tcw, total;
+    int64_t gi, gh, dgi, dgh, dYa, dYb, dhc, dcat, csum, dgiP, dghP, tcw, part, total;
 };
+static inline int64_t in_pitch(const bigru_plan& p, int l) { return rup(p.in_size(l), 8); }
+// floats taken by n bf16 elements per plane
+static inline int64_t plane_floats(const bigru_plan& p, int64_t n) {
+    return p.prec == BIGRU_PREC_FP32 ? 0 : rup((p.prec == BIGRU_PREC_BF16X3 ? 2 : 1) * n, 128) / 2;
+}
 static StashF32 stash_layout(const bigru_plan& p) {
     StashF32 s{};
     int64_t o = 0;
@@ -53,11 +61,20 @@ static StashF32 stash_layout(const bigru_plan& p) {
         s.Y[l] = o; o += BT * p.D * p.H;
         s.G[l] = o; o += (int64_t)p.D * BT * 4 * p.H;
         s.X[l] = o; o += BT * p.in_size(l);
+        o = rup(o, 64);
+        s.YP[l] = o; o += plane_floats(p, BT * p.D * p.H);
+        s.XP[l] = o; o += plane_floats(p, BT * in_pitch(p, l));
     }
     s.cat = o; o += (int64_t)p.B * 3 * p.H;
     s.arg = o; o += (int64_t)p.B * p.H;
     s.total = o;
     return s;
+}
+// split-K partials of the weight-gradient GEMMs of layer l (floats): dW_ih [splits][D][3H][I], dW_hh [splits][D][3H][H]
+static int64_t dw_part_floats(const bigru_plan& p, int l, int64_t N) {
+    const int64_t BT = (int64_t)p.B * p.T, M = 3LL * p.H;
+    const int s = wg_splits(cdiv64(M, htc::WG_BM) * cdiv64(N, htc::WG_BN) * p.D, cdiv64(BT, htc::WG_BK));
+    return s > 1 ? (int64_t)s * p.D * M * N : 0;
 }
 static ScratchF32 scratch_layout(const bigru_plan& p) {
     ScratchF32 s{};
@@ -73,22 +90,25 @@ static ScratchF32 scratch_layout(const bigru_plan& p) {
     s.dhc = o; o += (int64_t)p.D * p.B * p.H;
     s.dcat = o; o += (int64_t)p.B * 3 * p.H;
     s.csum = o; o += (int64_t)COLSUM_MAX_CHUNKS * (3 * p.H > p.C ? 3 * p.H : p.C);   // colsum_launch partials
-    s.tcw = o;                                                                           // packed bf16 operands of tc_gemm_launch
+    o = rup(o, 64);
+    s.dgiP = o; o += plane_floats(p, (int64_t)p.D * BT * 3 * p.H);                     // planes of dgi, dgh
+    s.dghP = o; o += plane_floats(p, (int64_t)p.D * BT * 3 * p.H);
+    s.tcw = o;                                                                           // packed weights / head operands
+    s.part = o;
     if (p.prec != BIGRU_PREC_FP32) {
         const int64_t H3 = 3LL * p.H, B = p.B, C = p.C, D = p.D;
-        int64_t need = 0;
+        int64_t need = 0, part = 0;
         for (int l = 0; l < p.L; ++l) {
             const int64_t I = p.in_size(l);
-            const int64_t e[4] = {tc_gemm_ws_elems(BT, H3, I, D, p.prec),        // projection
-                                  tc_gemm_ws_elems(H3, I, BT, 1, p.prec),        // dW_ih
-                                  tc_gemm_ws_elems(BT, I, H3, 1, p.prec),        // dX
-                                  tc_gemm_ws_elems(H3, p.H, BT, 1, p.prec)};     // dW_hh
-            for (int64_t v : e) need = need > v ? need : v;
+            need = std::max(need, tc_pack_elems(H3, I, D, p.prec));             // W_ih, projection
+            need = std::max(need, tc_pack_elems(I, H3, D, p.prec));             // W_ih^T, dX
+            part = std::max(part, std::max(dw_part_floats(p, l, I), dw_part_floats(p, l, p.H)));
         }
         const int64_t h[4] = {tc_gemm_ws_elems(B, C, H3, 1, p.prec), tc_gemm_ws_elems(B, H3, C, 1, p.prec),
                               tc_gemm_ws_elems(C, H3, B, 1, p.prec), tc_gemm_ws_elems(H3, p.H, B, 1, p.prec)};   // head, w0
-        for (int64_t v : h) need = need > v ? need : v;
-        o += (need + 1) / 2;
+        for (int64_t v : h) need = std::max(need, v);
+        o += plane_floats(p, need);
+        s.part = o; o += part;
     }
     s.total = o;
     return s;
@@ -116,6 +136,22 @@ static int plan_gemm(const bigru_plan& p, const GemmArgs& g, int cls, float* scr
     return p.prec == BIGRU_PREC_FP32 ? sgemm_launch(g, st)
                                      : tc_gemm_launch(g, p.prec, cls, reinterpret_cast<htc::bf16_t*>(scratch + scratch_layout(p).tcw), st);
 }
+
+// planes [depth][rows][pitch] at float offset off of buf (lo follows hi at bf16x3)
+static Planes plan_planes(const bigru_plan& p, const float* buf, int64_t off, int64_t cols, int64_t rows, int64_t depth,
+                          int64_t pitch) {
+    const htc::bf16_t* hi = reinterpret_cast<const htc::bf16_t*>(buf + off);
+    return Planes{hi, p.prec == BIGRU_PREC_BF16X3 ? hi + depth * rows * pitch : nullptr, cols, rows, depth, pitch};
+}
+// the layer input's planes as the projection and dW_ih read them: its own (layer 0, dropout) or the previous layer's Y
+static Planes input_planes(const bigru_plan& p, const float* stash, int l, bool own) {
+    const StashF32 S = stash_layout(p);
+    const int64_t BT = (int64_t)p.B * p.T;
+    return own ? plan_planes(p, stash, S.XP[l], p.in_size(l), BT, 1, in_pitch(p, l))
+               : plan_planes(p, stash, S.YP[l - 1], (int64_t)p.D * p.H, BT, 1, (int64_t)p.D * p.H);
+}
+static htc::bf16_t* mut(const Planes& q) { return const_cast<htc::bf16_t*>(q.hi); }
+static htc::bf16_t* mut_lo(const Planes& q) { return const_cast<htc::bf16_t*>(q.lo); }
 
 extern "C" int bigru_plan_create(int B, int T, int F, int H, int L, int C, int bidirectional, int precision,
                                  bigru_plan** out) {
@@ -206,20 +242,36 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
             KLAUNCH(KC_MISC, 0.0, 0.0, st, dropout_kernel<<<132 * 8, 256, 0, st>>>(inp, xd, BT * I, T, I, l == 0 ? spatial : 0, drop, seed, (uint32_t)l));
             inp = xd;
         }
-        // gi[d] = X W_ih[d]^T + b_ih[d]   for both directions
-        GemmArgs g = gemm_args(inp, params + p.off_wih(l, 0), scratch + W.gi, (int)BT, 3 * H, I, I, 1, I, 1, 3 * H);
-        g.bias = params + p.off_bih(l, 0);
-        g.batch = D; g.zA = 0; g.zB = p.ld_block(l); g.zBias = p.ld_block(l); g.zC = BT * 3 * H;
-        TRY(plan_gemm(p, g, KC_TC_GEMM, scratch, st));
         float* Y = stash + S.Y[l];
         float* G = stash + S.G[l];
         const float* h0l = h0 ? h0 + (int64_t)l * D * B * H : nullptr;
         float* hnl = hn ? hn + (int64_t)l * D * B * H : nullptr;
         if (p.prec != BIGRU_PREC_FP32) {
-            TRY(tc_scan_fwd(p, l, scratch + W.gi, params + p.off_whh(l, 0), params + p.off_bhh(l, 0), h0l, Y, G, hnl, st));
+            const bool own = l == 0 || do_drop;
+            const Planes xp = input_planes(p, stash, l, own);
+            if (own)
+                KLAUNCH(KC_PACK, 0.0, 0.0, st, htc::to_planes_kernel<<<132 * 8, 256, 0, st>>>(inp, BT, I, (int)xp.pitch, mut(xp), mut_lo(xp)));
+            // gi[d] = X W_ih[d]^T + b_ih[d]   for both directions
+            Planes wp;
+            TRY(tc_pack(params + p.off_wih(l, 0), I, 1, p.ld_block(l), 3 * H, I, D, p.prec, reinterpret_cast<htc::bf16_t*>(scratch + W.tcw),
+                        &wp, st));
+            {
+                ProfScope ps(KC_TC_GEMM, 2.0 * BT * 3 * H * (double)I * D, 0.0, st);
+                htc::WgJob j = wg_job(scratch + W.gi, (int)BT, 3 * H, 3 * H, D, cdiv64(I, htc::WG_BK));
+                j.bias = params + p.off_bih(l, 0); j.zBias = p.ld_block(l); j.zC = BT * 3 * H;
+                j.b.zsel = 1;
+                TRY(wg_gemm(j, xp, false, wp, false, p.prec, st));
+            }
+            const Planes yp = plan_planes(p, stash, S.YP[l], (int64_t)D * H, BT, 1, (int64_t)D * H);
+            TRY(tc_scan_fwd(p, l, scratch + W.gi, params + p.off_whh(l, 0), params + p.off_bhh(l, 0), h0l, Y, G, hnl, mut(yp), mut_lo(yp), st));
             inp = Y;
             continue;
         }
+        // gi[d] = X W_ih[d]^T + b_ih[d]   for both directions
+        GemmArgs g = gemm_args(inp, params + p.off_wih(l, 0), scratch + W.gi, (int)BT, 3 * H, I, I, 1, I, 1, 3 * H);
+        g.bias = params + p.off_bih(l, 0);
+        g.batch = D; g.zA = 0; g.zB = p.ld_block(l); g.zBias = p.ld_block(l); g.zC = BT * 3 * H;
+        TRY(plan_gemm(p, g, KC_TC_GEMM, scratch, st));
         for (int s = 0; s < T; ++s) {
             // gh[d] = h_prev[d] W_hh[d]^T + b_hh[d];  h_prev rows live in Y (or h0 at s == 0)
             const float* hp; int64_t sam, zA;
@@ -292,8 +344,10 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
         float* dgi = scratch + W.dgi;
         float* dgh = scratch + W.dgh;
         if (l != p.L - 1) CUDA_TRY(cudaMemsetAsync(dhc, 0, sizeof(float) * D * B * H, st));
+        const Planes gip = plan_planes(p, scratch, W.dgiP, 3LL * H, BT, D, 3LL * H);
+        const Planes ghp = plan_planes(p, scratch, W.dghP, 3LL * H, BT, D, 3LL * H);
         if (p.prec != BIGRU_PREC_FP32) {
-            TRY(tc_scan_bwd(p, l, G, Y, h0l, dY, dhc, dgi, dgh, params + p.off_whh(l, 0), st));
+            TRY(tc_scan_bwd(p, l, G, Y, h0l, dY, dhc, dgi, dgh, params + p.off_whh(l, 0), mut(gip), mut_lo(gip), mut(ghp), mut_lo(ghp), st));
         } else {
             for (int s = 0; s < T; ++s) {
                 KLAUNCH(KC_GATES_BWD, 0.0, 0.0, st, gru_gates_bwd_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(G, Y, h0l, dY, dhc, dgi, dgh, B, T, H, D, s));
@@ -311,6 +365,58 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
         // layer input as seen by the projection (dropped copy when dropout was applied)
         const float* inp = l == 0 ? (x ? x : stash + S.X[0]) : stash + S.Y[l - 1];     // x == NULL: forward_windows left it in the stash
         if (do_drop && (l == 0 || p.L > 1)) inp = stash + S.X[l];
+        if (p.prec != BIGRU_PREC_FP32) {
+            const int64_t kb = cdiv64(BT, htc::WG_BK), H3 = 3LL * H;
+            float* part = scratch + W.part;
+            // dW_ih[d] = dgi[d]^T X, both directions in one launch
+            const Planes xp = input_planes(p, stash, l, l == 0 || do_drop);
+            {
+                ProfScope ps(KC_TC_GEMM_DWIH, 2.0 * H3 * I * (double)BT * D, 0.0, st);
+                htc::WgJob j = wg_job(grads + p.off_wih(l, 0), (int)H3, I, I, D, kb);
+                j.zC = p.ld_block(l); j.a.zsel = 1; j.part = part;
+                j.splits = wg_splits(cdiv64(H3, htc::WG_BM) * cdiv64(I, htc::WG_BN) * D, kb);
+                TRY(wg_gemm(j, gip, true, xp, true, p.prec, st));
+            }
+            // dW_hh[d] = dgh[d]^T H_prev: H_prev(b,t) = Y[b,t-1] (dir 0) / Y[b,t+1] (dir 1), the columns of direction d.  The
+            // dgh planes are zero at each sequence's first step, whose h0 term the w0 GEMM below adds from fp32 dgh.
+            if (T > 1) {
+                ProfScope ps(KC_TC_GEMM_DWHH, 2.0 * H3 * H * (double)BT * D, 0.0, st);
+                htc::WgJob j = wg_job(grads + p.off_whh(l, 0), (int)H3, H, H, D, kb);
+                j.zC = p.ld_block(l); j.a.zsel = 1; j.part = part;
+                j.b.coff = H; j.b.kshift[0] = -1; j.b.kshift[1] = 1;
+                j.splits = wg_splits(cdiv64(H3, htc::WG_BM) * cdiv64(H, htc::WG_BN) * D, kb);
+                TRY(wg_gemm(j, ghp, true, plan_planes(p, stash, S.YP[l], (int64_t)D * H, BT, 1, (int64_t)D * H), true, p.prec, st));
+            }
+            for (int d = 0; d < D; ++d) {
+                const float* dgi_d = dgi + (int64_t)d * BT * 3 * H;
+                const float* dgh_d = dgh + (int64_t)d * BT * 3 * H;
+                if (h0l) {
+                    const int tf = d == 0 ? 0 : T - 1;
+                    GemmArgs w0 = gemm_args(dgh_d + (int64_t)tf * 3 * H, h0l + (int64_t)d * B * H, grads + p.off_whh(l, d),
+                                            3 * H, H, B, 1, (int64_t)T * 3 * H, 1, H, H);
+                    w0.beta = 1;
+                    TRY(plan_gemm(p, w0, KC_TC_GEMM_DWHH, scratch, st));
+                }
+                TRY(colsum_launch(dgi_d, grads + p.off_bih(l, d), BT, 3 * H, 3 * H, 1, 0, 0, scratch + W.csum, st));
+                TRY(colsum_launch(dgh_d, grads + p.off_bhh(l, d), BT, 3 * H, 3 * H, 1, 0, 0, scratch + W.csum, st));
+            }
+            // dX = sum_d dgi[d] W_ih[d]: one K loop over direction 0, then direction 1
+            float* dxo = l == 0 ? dx : dYnext;
+            if (dxo) {
+                Planes wp;
+                TRY(tc_pack(params + p.off_wih(l, 0), 1, I, p.ld_block(l), I, 3 * H, D, p.prec, reinterpret_cast<htc::bf16_t*>(scratch + W.tcw),
+                            &wp, st));
+                {
+                    ProfScope ps(KC_TC_GEMM_DX, 2.0 * BT * I * (double)H3 * D, 0.0, st);
+                    htc::WgJob j = wg_job(dxo, (int)BT, I, I, 1, D * (H3 / htc::WG_BK));
+                    j.kbd = (int)(H3 / htc::WG_BK); j.kcat = 1; j.a.zsel = 1; j.b.zsel = 1;
+                    TRY(wg_gemm(j, gip, false, wp, false, p.prec, st));
+                }
+                if (do_drop && (l == 0 || p.L > 1))
+                    KLAUNCH(KC_MISC, 0.0, 0.0, st, dropout_kernel<<<132 * 8, 256, 0, st>>>(dxo, dxo, BT * I, T, I, l == 0 ? spatial : 0, drop, seed, (uint32_t)l));
+            }
+            continue;
+        }
         const int splitk = (int)min((int64_t)64, max((int64_t)1, BT / 512));
         for (int d = 0; d < D; ++d) {
             const float* dgi_d = dgi + (int64_t)d * BT * 3 * H;
@@ -517,16 +623,17 @@ extern "C" int bigru_loss(int kind, const float* d_logits, const void* d_target,
     cudaStream_t st = (cudaStream_t)stream;
     CUDA_TRY(cudaMemsetAsync(d_loss, 0, sizeof(float), st));
     if (kind == BIGRU_LOSS_MLSM) { d_weight = nullptr; d_pos_weight = nullptr; }
-    KLAUNCH(KC_LOSS, 0.0, 0.0, st, loss_kernel<<<nblk(B, 128), 128, 0, st>>>(kind, d_logits, d_target, d_weight, d_pos_weight, B, C,
+    KLAUNCH(KC_LOSS, 0.0, 0.0, st, loss_kernel<<<1, 256, 0, st>>>(kind, d_logits, d_target, d_weight, d_pos_weight, B, C,
                                              (float)(1.0 / denom), d_loss, d_dlogits));
     return BIGRU_OK;
 }
 
-extern "C" int bigru_sqnorm(const float* d_g, int64_t n, float* d_out, void* stream) {
-    if (!d_g || !d_out || n < 0) { bigru_set_error("sqnorm: bad argument"); return BIGRU_ERR_ARG; }
+extern "C" int bigru_sqnorm(const float* d_g, int64_t n, float* d_out, float* d_ws, void* stream) {
+    if (!d_g || !d_out || !d_ws || n < 0) { bigru_set_error("sqnorm: bad argument"); return BIGRU_ERR_ARG; }
     if (n == 0) return BIGRU_OK;
-    const unsigned blocks = (unsigned)min((int64_t)132 * 4, cdiv64(n, 256));
-    KLAUNCH(KC_OPTIM, 0.0, 0.0, (cudaStream_t)stream, sqnorm_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d_g, n, d_out));
+    const int blocks = (int)min((int64_t)BIGRU_SQNORM_WS, cdiv64(n, 256));
+    KLAUNCH(KC_OPTIM, 0.0, 0.0, (cudaStream_t)stream, sqnorm_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d_g, n, d_ws));
+    KLAUNCH(KC_OPTIM, 0.0, 0.0, (cudaStream_t)stream, sqnorm_finish_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(d_ws, blocks, d_out));
     return BIGRU_OK;
 }
 

@@ -276,14 +276,14 @@ __global__ void head_bwd_dy_kernel(const float* __restrict__ dcat, const int* __
 }
 
 // ------------------------------------------------------------------------------------------
-// Losses: value (mean over `denom`) + dlogits
+// Losses: value (mean over `denom`) + dlogits.  One block: each thread sums its rows in order, then a fixed-order block
+// reduction, so the loss is bit-reproducible (B x C is small).
 // ------------------------------------------------------------------------------------------
 __global__ void loss_kernel(int kind, const float* __restrict__ logits, const void* __restrict__ target,
                             const float* __restrict__ weight, const float* __restrict__ pos_weight, int B, int C,
                             float inv_denom, float* __restrict__ loss, float* __restrict__ dlogits) {
-    const int b = blockIdx.x * blockDim.x + threadIdx.x;
     float l = 0.f;
-    if (b < B) {
+    for (int b = threadIdx.x; b < B; b += blockDim.x) {
         const float* lg = logits + (int64_t)b * C;
         if (kind == BIGRU_LOSS_CE) {
             const long long tg = ((const long long*)target)[b];
@@ -292,7 +292,7 @@ __global__ void loss_kernel(int kind, const float* __restrict__ logits, const vo
             float s = 0.f;
             for (int c = 0; c < C; ++c) s += expf(lg[c] - m);
             const float lse = m + logf(s);
-            l = lse - lg[tg];
+            l += lse - lg[tg];
             if (dlogits)
                 for (int c = 0; c < C; ++c)
                     dlogits[(int64_t)b * C + c] = (expf(lg[c] - lse) - (c == tg ? 1.f : 0.f)) * inv_denom;
@@ -319,14 +319,16 @@ __global__ void loss_kernel(int kind, const float* __restrict__ logits, const vo
     if (threadIdx.x < 32) {
         float v = threadIdx.x < (blockDim.x >> 5) ? sm[threadIdx.x] : 0.f;
         for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (threadIdx.x == 0) atomicAdd(loss, v * inv_denom);
+        if (threadIdx.x == 0) *loss += v * inv_denom;
     }
 }
 
 // ------------------------------------------------------------------------------------------
 // clip_grad_norm_ + Adam over the flat buffers
 // ------------------------------------------------------------------------------------------
-__global__ void sqnorm_kernel(const float* __restrict__ g, int64_t n, float* __restrict__ out) {
+// sum(g^2): each block reduces its grid-stride share in a fixed order into ws[block]; sqnorm_finish_kernel then adds the
+// block sums in a fixed order into *out (no atomics: bit-reproducible for a given n)
+__global__ void sqnorm_kernel(const float* __restrict__ g, int64_t n, float* __restrict__ ws) {
     float s = 0.f;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         const float v = g[i];
@@ -339,8 +341,15 @@ __global__ void sqnorm_kernel(const float* __restrict__ g, int64_t n, float* __r
     if (threadIdx.x < 32) {
         float v = threadIdx.x < (blockDim.x >> 5) ? sm[threadIdx.x] : 0.f;
         for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (threadIdx.x == 0) atomicAdd(out, v);
+        if (threadIdx.x == 0) ws[blockIdx.x] = v;
     }
+}
+// one warp: lane l adds ws[l], ws[l + 32], ... in order, then a fixed butterfly
+__global__ void sqnorm_finish_kernel(const float* __restrict__ ws, int nblocks, float* __restrict__ out) {
+    float v = 0.f;
+    for (int i = threadIdx.x; i < nblocks; i += 32) v += ws[i];
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (threadIdx.x == 0) *out += v;
 }
 
 __global__ void clip_adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,

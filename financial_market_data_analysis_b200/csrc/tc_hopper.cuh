@@ -2,9 +2,9 @@
 //
 // Both precisions share the data layout and step composition of the fp32 path (api.cu): time steps of the recurrence and
 // all GEMMs read and write the same fp32 buffers.  What changes is where the arithmetic runs:
-//   * tc_gemm_launch      - the strided GEMM of kernels_f32.cuh (same GemmArgs: NT / NN / TN by strides, batches, split-K,
-//                           bias, accumulate, the h_{t-1} row mask): operands packed once into K-major bf16 images, then a
-//                           TMA + mbarrier pipelined wgmma kernel (wg_gemm_kernel).
+//   * wg_gemm             - a persistent TMA + mbarrier pipelined wgmma GEMM (wg_gemm_kernel) over bf16 operand planes that
+//                           the scans and to_planes_kernel write next to the fp32 activations; deterministic split-K.
+//                           tc_gemm_launch keeps the GemmArgs contract for the small head / h0 GEMMs (operands packed).
 //   * gru_scan_fwd_kernel - one layer's whole forward recurrence in one launch: a thread-block cluster per (direction,
 //                           16-row batch tile); CTA c of the cluster owns hidden units [64c, 64c+64) and keeps their W_hh
 //                           rows (3 gates x 64 units x H) resident in shared memory for all T steps.  Each step it multiplies
@@ -21,6 +21,7 @@
 #pragma once
 #include "common.cuh"
 #include "kernels_f32.cuh"
+#include <algorithm>
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -78,18 +79,23 @@ __device__ __forceinline__ uint32_t cluster_rank() {
 }
 
 // ------------------------------------------------------------------------------------------------------
-// GEMM: C[z][m,n] (+)= sum_k A(m,k) B(n,k) (+ bias[n]), the contract of sgemm_kernel (kernels_f32.cuh), in two passes:
-//   tc_pack_kernel  - each operand is read once (any strides, the dW_hh row mask) and written as a zero-padded K-major bf16
-//                     image [batch][rows / 128 * 128][K / 64 * 64]: one plane at bf16, hi and lo planes at bf16x3;
-//   wg_gemm_kernel  - 128 x 128 output tiles, warp-specialised: one thread streams 64-deep k-blocks of every plane into a
-//                     STAGES-deep shared-memory ring with TMA (128-byte swizzle) and mbarrier completion, two consumer
-//                     warpgroups (64 rows each) multiply them with wgmma.m64n128k16 (fp32 accumulation) and release the
-//                     slot; bf16x3 issues hi*hi + hi*lo + lo*hi per k-step.  Epilogue: bias, accumulate, split-K atomics.
+// GEMM: C[z][m,n] (+)= sum_k A(m,k) B(n,k) (+ bias[n]) on bf16 planes (hi, and lo at bf16x3) that TMA reads straight from
+// where their producers left them: the scans write Y, dgi and dgh planes next to their fp32 copies, the layer input gets
+// planes from to_planes_kernel, and the small weight operands are packed per call by tc_pack_kernel.
+//   * operands are K-major (box 64 K x 128 rows) or MN-major (two boxes 64 MN x 64 K rows; the k = b*t reduction of the
+//     weight gradients runs down the rows of the activations), all with 128-byte swizzle; TMA's out-of-bounds zero fill
+//     covers ragged M, N and K edges, and the +-1 row shift of h_{t-1} in dW_hh;
+//   * persistent: at most one CTA per SM strides over (tile, split) units.  One thread streams 64-deep k-blocks through a
+//     STAGES-deep mbarrier ring and runs ahead across unit boundaries; two consumer warpgroups (64 rows each) multiply with
+//     wgmma.m64n128k16 (fp32 accumulation), keep one wgmma group in flight and release the previous stage;
+//     bf16x3 issues hi*hi + hi*lo + lo*hi per k-step;
+//   * split-K units write fp32 partials; splitk_reduce_kernel adds them in split order (no atomics: bit-reproducible).
 // ------------------------------------------------------------------------------------------------------
 constexpr int WG_BM = 128, WG_BN = 128, WG_BK = 64;
 
+// packs a small fp32 operand (weights, head activations) into a zero-padded K-major image [batch][Rp][Kp], hi and lo planes
 __global__ void tc_pack_kernel(const float* __restrict__ src, int64_t s_r, int64_t s_k, int64_t zsrc, int R, int K, int Rp, int Kp,
-                               int mask_period, int mask_skip, bf16_t* __restrict__ hi, bf16_t* __restrict__ lo) {
+                               bf16_t* __restrict__ hi, bf16_t* __restrict__ lo) {
     __shared__ float tile[32][33];
     const int z = blockIdx.z, r0 = blockIdx.y * 32, k0 = blockIdx.x * 32;
     const float* a = src + z * zsrc;
@@ -97,7 +103,7 @@ __global__ void tc_pack_kernel(const float* __restrict__ src, int64_t s_r, int64
     for (int j = threadIdx.y; j < 32; j += 8) {
         const int r = r0 + (kfast ? j : threadIdx.x), k = k0 + (kfast ? threadIdx.x : j);
         float v = 0.f;
-        if (r < R && k < K && !(mask_period && (k % mask_period) == mask_skip)) v = a[(int64_t)r * s_r + (int64_t)k * s_k];
+        if (r < R && k < K) v = a[(int64_t)r * s_r + (int64_t)k * s_k];
         if (kfast) tile[j][threadIdx.x] = v; else tile[threadIdx.x][j] = v;
     }
     __syncthreads();
@@ -106,6 +112,19 @@ __global__ void tc_pack_kernel(const float* __restrict__ src, int64_t s_r, int64
         const int64_t o = ((int64_t)z * Rp + r) * Kp + k;
         bf16_t h, l;
         split_bf16(tile[j][threadIdx.x], h, l);
+        hi[o] = h;
+        if (lo) lo[o] = l;
+    }
+}
+
+// bf16 planes of a row-major fp32 matrix [rows][cols]; row pitch `pitch` elements (a multiple of 8: 16-byte TMA strides)
+__global__ void to_planes_kernel(const float* __restrict__ src, int64_t rows, int cols, int pitch, bf16_t* __restrict__ hi,
+                                 bf16_t* __restrict__ lo) {
+    const int64_t n = rows * cols;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = i / cols, c = i % cols, o = r * pitch + c;
+        bf16_t h, l;
+        split_bf16(src[i], h, l);
         hi[o] = h;
         if (lo) lo[o] = l;
     }
@@ -142,30 +161,43 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         }
     }
 }
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+                 ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-// wgmma shared-memory descriptor of a K-major tile with 128-byte swizzle: rows of 64 bf16, 8-row groups 1024 B apart
-__device__ __forceinline__ uint64_t wg_desc(uint32_t saddr) {
-    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
+// wgmma shared-memory descriptor, 128-byte swizzle.  K-major: rows of 64 bf16 (128 B), 8-row groups 1024 B apart.
+// MN-major: lines of 64 MN elements per k, 8-k groups 1024 B apart (stride byte offset), 64-element MN blocks 8 KB apart
+// (leading byte offset: one 64 x 64 TMA box).
+__device__ __forceinline__ uint64_t wg_desc(uint32_t saddr, uint32_t lbo) {
+    return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
+// TA / TB: 1 = MN-major ("transposed") shared-memory operand
+template <int TA, int TB>
 __device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, uint64_t db) {
-    asm volatile("wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, 1, 1, 1, 0, 0;"
+    asm volatile("wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, 1, 1, 1, %66, %67;"
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-                 : "l"(da), "l"(db));
+                 : "l"(da), "l"(db), "n"(TA), "n"(TB));
 }
 
-struct WgOut {
-    float* C; const float* bias;
-    int M, N, kblocks, Mp, Np, splitk, beta;
+// one operand of a GEMM: tensor maps are 3-D [depth][rows][cols] (cols innermost).  For the k-block of direction dz:
+// K-major coordinates (k, r0, dz * zsel); MN-major (r0 + dz * coff, k + kshift[dz], dz * zsel)
+struct WgOp {
+    int zsel, coff, kshift[2];
+};
+struct WgJob {
+    WgOp a, b;
+    float* C; const float* bias; float* part;  // part: [splits][batch][M][N] fp32 partials when splits > 1
+    int M, N, tm, tn, batch, splits;
+    int kblocks, kbd;                           // k-blocks per unit's full K range; per direction when kcat
+    int kcat;                                   // 1: the K loop runs over direction 0, then direction 1 (dz = kb / kbd)
+    int beta;
     int64_t ldc, zC, zBias;
 };
 
-template <int NS, int STAGES>
+template <int NS, int STAGES, int AMN, int BMN>
 __global__ void __launch_bounds__(384, 1)
 wg_gemm_kernel(const __grid_constant__ CUtensorMap ta_hi, const __grid_constant__ CUtensorMap ta_lo,
-               const __grid_constant__ CUtensorMap tb_hi, const __grid_constant__ CUtensorMap tb_lo, WgOut o) {
+               const __grid_constant__ CUtensorMap tb_hi, const __grid_constant__ CUtensorMap tb_lo, const WgJob j) {
     constexpr int NH = NS == 1 ? 1 : 2;
     constexpr int PLANE = WG_BM * WG_BK * 2;                  // 16 KB: one 128 x 64 bf16 tile
     constexpr int STAGE = 2 * NH * PLANE;                     // A planes, then B planes
@@ -174,77 +206,139 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap ta_hi, const __grid_constant_
     uint64_t* full = reinterpret_cast<uint64_t*>(sm + STAGES * STAGE);
     uint64_t* empty = full + STAGES;
     const int wgi = threadIdx.x / 128, tid = threadIdx.x % 128;
-    const int zb = blockIdx.z / o.splitk, zs = blockIdx.z % o.splitk;
-    const int m0 = blockIdx.y * WG_BM, n0 = blockIdx.x * WG_BN;
-    const int per = (o.kblocks + o.splitk - 1) / o.splitk;
-    const int kb0 = zs * per, kb1 = min(o.kblocks, kb0 + per);
+    const int units = j.tm * j.tn * j.batch * j.splits;
+    const int per = (j.kblocks + j.splits - 1) / j.splits;
     if (threadIdx.x == 0) {
         for (int i = 0; i < STAGES; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
+    // unit u: split fastest, then n tile, m tile, batch (consecutive units share the A rows of a tile row)
+    auto decode = [&](int u, int& s, int& zb, int& m0, int& n0) {
+        s = u % j.splits; u /= j.splits;
+        n0 = (u % j.tn) * WG_BN; u /= j.tn;
+        m0 = (u % j.tm) * WG_BM; zb = u / j.tm;
+    };
 
     if (wgi == 0) {                                           // producer
         if (tid == 0) {
-            for (int kb = kb0, i = 0; kb < kb1; ++kb, ++i) {
-                const int st = i % STAGES;
-                if (i >= STAGES) mbar_wait(empty + st, ((i / STAGES) - 1) & 1);
-                uint8_t* base = sm + st * STAGE;
-                mbar_arrive_expect_tx(full + st, STAGE);
-                const int kc = kb * WG_BK, ra = zb * o.Mp + m0, rb = zb * o.Np + n0;
-                tma_load_2d(base, &ta_hi, full + st, kc, ra);
-                if (NH == 2) tma_load_2d(base + PLANE, &ta_lo, full + st, kc, ra);
-                tma_load_2d(base + NH * PLANE, &tb_hi, full + st, kc, rb);
-                if (NH == 2) tma_load_2d(base + (NH + 1) * PLANE, &tb_lo, full + st, kc, rb);
+            uint32_t it = 0;
+            for (int u = blockIdx.x; u < units; u += gridDim.x) {
+                int s, zb, m0, n0;
+                decode(u, s, zb, m0, n0);
+                const int kb1 = min(j.kblocks, (s + 1) * per);
+                for (int kb = s * per; kb < kb1; ++kb, ++it) {
+                    const int st = it % STAGES;
+                    if (it >= STAGES) mbar_wait(empty + st, ((it / STAGES) - 1) & 1);
+                    const uint32_t base = smem_u32(sm + st * STAGE);
+                    mbar_arrive_expect_tx(full + st, STAGE);
+                    const int dz = j.kcat ? kb / j.kbd : zb, kc = (j.kcat ? kb % j.kbd : kb) * WG_BK;
+#pragma unroll
+                    for (int h = 0; h < NH; ++h) {
+                        const CUtensorMap* ma = h ? &ta_lo : &ta_hi;
+                        const CUtensorMap* mb = h ? &tb_lo : &tb_hi;
+                        const uint32_t da = base + h * PLANE, db = base + (NH + h) * PLANE;
+                        if (AMN) {
+                            const int k = kc + (dz ? j.a.kshift[1] : j.a.kshift[0]), r = m0 + dz * j.a.coff;
+                            tma_load_3d(da, ma, full + st, r, k, dz * j.a.zsel);
+                            tma_load_3d(da + PLANE / 2, ma, full + st, r + 64, k, dz * j.a.zsel);
+                        } else {
+                            tma_load_3d(da, ma, full + st, kc, m0, dz * j.a.zsel);
+                        }
+                        if (BMN) {
+                            const int k = kc + (dz ? j.b.kshift[1] : j.b.kshift[0]), r = n0 + dz * j.b.coff;
+                            tma_load_3d(db, mb, full + st, r, k, dz * j.b.zsel);
+                            tma_load_3d(db + PLANE / 2, mb, full + st, r + 64, k, dz * j.b.zsel);
+                        } else {
+                            tma_load_3d(db, mb, full + st, kc, n0, dz * j.b.zsel);
+                        }
+                    }
+                }
             }
         }
         return;
     }
     const int cg = wgi - 1;                                   // consumer warpgroup: rows cg*64 .. +64 of the tile
-    float d[64];
-#pragma unroll
-    for (int i = 0; i < 64; ++i) d[i] = 0.f;
-    for (int kb = kb0, i = 0; kb < kb1; ++kb, ++i) {
-        const int st = i % STAGES;
-        mbar_wait(full + st, (i / STAGES) & 1);
-        const uint32_t base = smem_u32(sm + st * STAGE);
-        const uint32_t a_hi = base + cg * 64 * 128, a_lo = a_hi + PLANE;
-        const uint32_t b_hi = base + NH * PLANE, b_lo = b_hi + PLANE;
-        asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int ks = 0; ks < WG_BK / 16; ++ks) {
-            wgmma_m64n128k16(d, wg_desc(a_hi + ks * 32), wg_desc(b_hi + ks * 32));
-            if (NS != 1) {
-                wgmma_m64n128k16(d, wg_desc(a_hi + ks * 32), wg_desc(b_lo + ks * 32));
-                wgmma_m64n128k16(d, wg_desc(a_lo + ks * 32), wg_desc(b_hi + ks * 32));
-            }
-        }
-        asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
-        asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
-        if (tid == 0) mbar_arrive(empty + st);
-    }
     const int w = tid / 32, l = tid % 32;
-    float* C = o.C + zb * o.zC;
-    const float* bias = o.bias ? o.bias + zb * o.zBias : nullptr;
+    // per k-step (16 deep) address advance: 32 B along a K-major row, 16 lines of 128 B down an MN-major box
+    constexpr uint32_t AKS = AMN ? 2048 : 32, BKS = BMN ? 2048 : 32;
+    constexpr uint32_t ALBO = AMN ? PLANE / 2 : 16, BLBO = BMN ? PLANE / 2 : 16;
+    uint32_t it = 0;
+    for (int u = blockIdx.x; u < units; u += gridDim.x) {
+        int s, zb, m0, n0;
+        decode(u, s, zb, m0, n0);
+        const int kb1 = min(j.kblocks, (s + 1) * per);
+        float d[64];
 #pragma unroll
-    for (int i = 0; i < 16; ++i)
+        for (int i = 0; i < 64; ++i) d[i] = 0.f;
+        int prev = -1;
+        for (int kb = s * per; kb < kb1; ++kb, ++it) {
+            const int st = it % STAGES;
+            mbar_wait(full + st, (it / STAGES) & 1);
+            const uint32_t base = smem_u32(sm + st * STAGE);
+            const uint32_t a_hi = base + cg * (PLANE / 2), a_lo = a_hi + PLANE;
+            const uint32_t b_hi = base + NH * PLANE, b_lo = b_hi + PLANE;
+            asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const int gm = m0 + cg * 64 + w * 16 + (l >> 2) + (e >= 2 ? 8 : 0);
-            const int gn = n0 + 8 * i + 2 * (l & 3) + (e & 1);
-            if (gm >= o.M || gn >= o.N) continue;
-            float v = d[4 * i + e];
-            if (bias && zs == 0) v += bias[gn];
-            float* c = C + (int64_t)gm * o.ldc + gn;
-            if (o.splitk > 1) atomicAdd(c, v);
-            else if (o.beta) *c += v;
-            else *c = v;
+            for (int ks = 0; ks < WG_BK / 16; ++ks) {
+                wgmma_m64n128k16<AMN, BMN>(d, wg_desc(a_hi + ks * AKS, ALBO), wg_desc(b_hi + ks * BKS, BLBO));
+                if (NS != 1) {
+                    wgmma_m64n128k16<AMN, BMN>(d, wg_desc(a_hi + ks * AKS, ALBO), wg_desc(b_lo + ks * BKS, BLBO));
+                    wgmma_m64n128k16<AMN, BMN>(d, wg_desc(a_lo + ks * AKS, ALBO), wg_desc(b_hi + ks * BKS, BLBO));
+                }
+            }
+            asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+            asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");   // the previous k-block's group is done
+            if (prev >= 0 && tid == 0) mbar_arrive(empty + prev);
+            prev = st;
         }
+        asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+        if (prev >= 0 && tid == 0) mbar_arrive(empty + prev);
+        float* C;
+        int64_t ldc;
+        const float* bias = nullptr;
+        if (j.splits > 1) {
+            C = j.part + ((int64_t)s * j.batch + zb) * j.M * j.N;
+            ldc = j.N;
+        } else {
+            C = j.C + zb * j.zC;
+            ldc = j.ldc;
+            if (j.bias) bias = j.bias + zb * j.zBias;
+        }
+#pragma unroll
+        for (int i = 0; i < 16; ++i)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int gm = m0 + cg * 64 + w * 16 + (l >> 2) + (e >= 2 ? 8 : 0);
+                const int gn = n0 + 8 * i + 2 * (l & 3) + (e & 1);
+                if (gm >= j.M || gn >= j.N) continue;
+                float v = d[4 * i + e];
+                if (bias) v += bias[gn];
+                float* c = C + (int64_t)gm * ldc + gn;
+                if (j.beta && j.splits == 1) *c += v;
+                else *c = v;
+            }
+    }
+}
+
+// C[z][m][n] (+)= sum over s = 0, 1, ... of part[s][z][m][n]: the split-K partial sums in a fixed order
+__global__ void splitk_reduce_kernel(const float* __restrict__ part, int splits, int batch, int M, int N, float* __restrict__ C,
+                                     int64_t ldc, int64_t zC, int beta) {
+    const int64_t per = (int64_t)M * N, n = per * batch;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        float v = 0.f;
+        for (int s = 0; s < splits; ++s) v += part[(int64_t)s * n + i];
+        const int64_t z = i / per, r = i % per;
+        float* c = C + z * zC + (r / N) * ldc + r % N;
+        *c = beta ? *c + v : v;
+    }
 }
 
 // ------------------------------------------------------------------------------------------------------
 // Forward recurrence of one layer, both directions.  Layouts are those of gru_gates_fwd_kernel:
 //   gi [D][B*T][3H] (x W_ih^T + b_ih), Y [B][T][D*H], G [D][B*T][4H] = (r, z, n, W_hn h + b_hn), hn [D][B][H].
+// Y also goes out as bf16 planes (yh, and yl at bf16x3) in Y's layout: the next layer's projection and the weight gradients
+// read them.
 // Grid (CS, B/16, D), cluster (CS, 1, 1), 256 threads.  Warp w owns units 16*(w/2) .. +16 of the CTA's slice and batch
 // columns 8*(w%2) .. +8: its r, z and n accumulators hold the same (unit, column) pairs, so the gate math needs no exchange.
 // ------------------------------------------------------------------------------------------------------
@@ -263,7 +357,7 @@ template <int H, int NS>
 __global__ void __launch_bounds__(SCAN_THREADS, 1)
 gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh, const float* __restrict__ bhh, int64_t zW,
                     const float* __restrict__ h0, float* __restrict__ Y, float* __restrict__ G, float* __restrict__ hn_out,
-                    int B, int T, int D) {
+                    bf16_t* __restrict__ yh, bf16_t* __restrict__ yl, int B, int T, int D) {
     using S = FwdSmem<H, NS>;
     constexpr int U = SCAN_U, CS = H / U, NH = S::NH;
     extern __shared__ __align__(128) uint8_t smem[];
@@ -362,27 +456,34 @@ gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh,
             float* gs = G + ((int64_t)d * B * T + row) * 4 * H + j;
             gs[0] = r; gs[H] = z; gs[2 * H] = n; gs[3 * H] = hnv;
             if (hn_out && s == T - 1) hn_out[((int64_t)d * B + b) * H + j] = h;
-            if (s + 1 < T) {
-                bf16_t hi, lo;
-                split_bf16(h, hi, lo);
-                const uint32_t off = swz<H * 2>(bcol[e & 1], j);
-                const uint32_t la = smem_u32(Hsm + nbuf * NH * S::HBYTES) + off;
+            bf16_t hi, lo;
+            split_bf16(h, hi, lo);
+            const uint32_t off = swz<H * 2>(bcol[e & 1], j);
+            const uint32_t la = smem_u32(Hsm + nbuf * NH * S::HBYTES) + off;
 #pragma unroll
-                for (int p = 0; p < CS; ++p) {
-                    st_cluster_b16(mapa(la, p), hi);
-                    if (NH == 2) st_cluster_b16(mapa(la + S::HBYTES, p), lo);
-                }
+            for (int p = 0; p < CS; ++p) {
+                st_cluster_b16(mapa(la, p), hi);
+                if (NH == 2) st_cluster_b16(mapa(la + S::HBYTES, p), lo);
             }
         }
         cluster_arrive();
         cluster_wait();
+        // the Y planes of this CTA's units: h_t is now in the h tile (hi / lo, every unit), so copy the own slice out with
+        // 16-byte stores.  Nobody writes this buffer again before the next step's barrier.
+        for (int i = tid; i < NH * SCAN_NB * (U / 8); i += SCAN_THREADS) {
+            const int h = i / (SCAN_NB * U / 8), r = (i / (U / 8)) % SCAN_NB, k = c * U + (i % (U / 8)) * 8;
+            const uint4 v = *reinterpret_cast<const uint4*>(Hsm + (nbuf * NH + h) * S::HBYTES + swz<H * 2>(r, k));
+            *reinterpret_cast<uint4*>((h ? yl : yh) + ((int64_t)(bt0 + r) * T + t) * DH + d * H + k) = v;
+        }
     }
 }
 
 // ------------------------------------------------------------------------------------------------------
 // Backward recurrence of one layer, both directions.  Layouts are those of gru_gates_bwd_kernel: G, Y, h0 as in the
 // forward; dY [B][T][D*H]; dhc [D][B][H] carries dh into the layer's last step (head / zero) and returns dh_{-1};
-// dgi, dgh [D][B*T][3H].  Shared memory: W^T rows (H) x own gate rows (192) | dgh tile [16][192] | receive slots of the
+// dgi, dgh [D][B*T][3H], and their bf16 planes gih/gil, ghh/ghl in the same layout for the GEMMs.  The dgh planes hold
+// zeros at each sequence's first step (t = 0 for d = 0, t = T-1 for d = 1): that row pairs with h0 (covered from fp32 dgh),
+// so dW_hh = dgh^T H_prev needs no row mask.  Shared memory: W^T rows (H) x own gate rows (192) | dgh tile [16][192] | receive slots of the
 // peers' partial sums [CS-1][16][64] fp32 (this CTA's own partial goes into the dgh tile's space, which is free by then).
 // Cluster barrier phases per step: (1) partials of the step have landed; (2) every CTA has read its receive slots, so
 // the next step's partials may be written.
@@ -403,7 +504,8 @@ template <int H, int NS>
 __global__ void __launch_bounds__(SCAN_THREADS, 1)
 gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, const float* __restrict__ h0,
                     const float* __restrict__ dY, float* __restrict__ dhc, float* __restrict__ dgi, float* __restrict__ dgh,
-                    const float* __restrict__ Whh, int64_t zW, int B, int T, int D) {
+                    const float* __restrict__ Whh, int64_t zW, bf16_t* __restrict__ gih, bf16_t* __restrict__ gil,
+                    bf16_t* __restrict__ ghh, bf16_t* __restrict__ ghl, int B, int T, int D) {
     using S = BwdSmem<H, NS>;
     constexpr int U = SCAN_U, CS = H / U, NH = S::NH, Q = S::Q, NB = SCAN_NB;
     constexpr int MT = H / 16 / 8;                           // m-tiles (16 rows of W^T) per warp
@@ -480,8 +582,23 @@ gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, co
                 *reinterpret_cast<bf16_t*>(Dsm + swz<S::WP>(bl, gte * U + u)) = hi;
                 if (NH == 2) *reinterpret_cast<bf16_t*>(Dsm + S::DBYTES + swz<S::WP>(bl, gte * U + u)) = lo;
             }
+            // dgi's n gate is dan (dgh's is dgn = dan * r); its r and z gates equal dgh's and leave from the dgh tile below
+            bf16_t hi, lo;
+            split_bf16(dan, hi, lo);
+            const int64_t po = ((int64_t)d * B * T + row) * 3 * H + 2 * H + j;
+            gih[po] = hi;
+            if (NH == 2) gil[po] = lo;
         }
         __syncthreads();
+        // planes of this step's rows from the dgh tile, 16-byte stores: dgh (zeros at a sequence's first step) and dgi's r, z
+        for (int i = tid; i < NH * NB * (Q / 8); i += SCAN_THREADS) {
+            const int h = i / (NB * Q / 8), r = (i / (Q / 8)) % NB, q = (i % (Q / 8)) * 8, gte = q / U;
+            uint4 v = *reinterpret_cast<const uint4*>(Dsm + h * S::DBYTES + swz<S::WP>(r, q));
+            const int64_t o = ((int64_t)d * B * T + (int64_t)(bt0 + r) * T + t) * 3 * H + gte * H + c * U + q % U;
+            if (gte < 2) *reinterpret_cast<uint4*>((h ? gil : gih) + o) = v;
+            if (first) v = make_uint4(0u, 0u, 0u, 0u);
+            *reinterpret_cast<uint4*>((h ? ghl : ghh) + o) = v;
+        }
         // partial dh_{t-1}[k, b] = sum over this CTA's gate rows q of W[q, k] dgh[b, q], for all H units k
         float acc[MT][2][4];
 #pragma unroll
@@ -549,76 +666,141 @@ gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, co
 
 // ---- host launchers ----------------------------------------------------------------------------------------
 static inline int64_t rup(int64_t v, int64_t m) { return (v + m - 1) / m * m; }
-// bf16 elements of the packed operand images of one GEMM (what tc_gemm_launch needs in its workspace)
-static inline int64_t tc_gemm_ws_elems(int64_t M, int64_t N, int64_t K, int64_t batch, int prec) {
-    const int nh = prec == BIGRU_PREC_BF16X3 ? 2 : 1;
-    return nh * batch * (rup(M, htc::WG_BM) + rup(N, htc::WG_BN)) * rup(K, htc::WG_BK);
+// bf16 elements of a zero-padded K-major image [batch][rup(R, 128)][rup(K, 64)] written by tc_pack_kernel (hi and lo planes)
+static inline int64_t tc_pack_elems(int64_t R, int64_t K, int64_t batch, int prec) {
+    return (prec == BIGRU_PREC_BF16X3 ? 2 : 1) * batch * rup(R, htc::WG_BM) * rup(K, htc::WG_BK);
 }
+// bf16 elements of both packed operands of tc_gemm_launch
+static inline int64_t tc_gemm_ws_elems(int64_t M, int64_t N, int64_t K, int64_t batch, int prec) {
+    return tc_pack_elems(M, K, batch, prec) + tc_pack_elems(N, K, batch, prec);
+}
+// Split-K count of a weight-gradient GEMM (K = B*T).  Four units per SM of a 132-SM H100 keep the spread of unit times
+// (the last split is shorter, the tile count rarely divides 132) small next to the work per SM: dW_ih of layer 1 at
+// configs[1] has 48 tiles -> 11 splits = 528 units; dW_hh 24 tiles -> 22 splits.  At least 8 k-blocks per split keep the
+// pipeline fill small.  The count is fixed (not taken from the device) so that the summation order, and with it every
+// bit of the result, depends on the shape only.
+static inline int wg_splits(int64_t tiles, int64_t kblocks) {
+    const int64_t s = std::min(cdiv64(4 * 132, tiles), kblocks / 8);
+    if (s <= 1) return 1;
+    const int64_t per = cdiv64(kblocks, s);
+    return (int)cdiv64(kblocks, per);                 // no empty split
+}
+
+// bf16 planes [depth][rows][pitch] (cols <= pitch used; pitch % 8 == 0); lo is null at bf16
+struct Planes {
+    const htc::bf16_t* hi; const htc::bf16_t* lo;
+    int64_t cols, rows, depth, pitch;
+};
 
 typedef CUresult (*PFN_encodeTiled_t)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                       const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                       CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-// tensor map over a packed image [rows][Kp] bf16: boxes of 64 (K) x 128 rows with 128-byte swizzle
-static int make_pack_map(CUtensorMap* m, const void* base, int64_t rows, int64_t Kp) {
+// 3-D tensor map over one plane with 128-byte swizzle and zero fill out of bounds: boxes of 64 (K) x 128 rows for a K-major
+// operand, 64 (MN) x 64 (K) rows for an MN-major one
+static int make_plane_map(CUtensorMap* m, const htc::bf16_t* base, const Planes& p, bool mn) {
     static PFN_encodeTiled_t enc = nullptr;
     if (!enc) {
-        void* p = nullptr;
+        void* f = nullptr;
         cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) {
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) {
             bigru_set_error("tc_gemm: cuTensorMapEncodeTiled is unavailable");
             return BIGRU_ERR_CUDA;
         }
-        enc = (PFN_encodeTiled_t)p;
+        enc = (PFN_encodeTiled_t)f;
     }
-    const cuuint64_t dims[2] = {(cuuint64_t)Kp, (cuuint64_t)rows};
-    const cuuint64_t strides[1] = {(cuuint64_t)Kp * 2};
-    const cuuint32_t box[2] = {(cuuint32_t)htc::WG_BK, 128u}, es[2] = {1u, 1u};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const cuuint64_t dims[3] = {(cuuint64_t)p.cols, (cuuint64_t)p.rows, (cuuint64_t)p.depth};
+    const cuuint64_t strides[2] = {(cuuint64_t)p.pitch * 2, (cuuint64_t)(p.pitch * p.rows) * 2};
+    const cuuint32_t box[3] = {64u, mn ? 64u : 128u, 1u}, es[3] = {1u, 1u, 1u};
+    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<htc::bf16_t*>(base), dims, strides, box, es,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { bigru_set_error("tc_gemm: cuTensorMapEncodeTiled failed (%d)", (int)r); return BIGRU_ERR_CUDA; }
     return BIGRU_OK;
 }
 
-// prec: BIGRU_PREC_BF16 (NS = 1) or BIGRU_PREC_BF16X3 (NS = 3); ws: tc_gemm_ws_elems(...) bf16 elements
-static int tc_gemm_launch(const GemmArgs& g, int prec, int cls, htc::bf16_t* ws, cudaStream_t st) {
-    if (g.M <= 0 || g.N <= 0 || g.K <= 0) return BIGRU_OK;
-    const bool x3 = prec == BIGRU_PREC_BF16X3;
-    ProfScope ps(cls, 2.0 * g.M * g.N * (double)g.K * g.batch, 0.0, st);
-    const int Mp = (int)rup(g.M, htc::WG_BM), Np = (int)rup(g.N, htc::WG_BN), Kp = (int)rup(g.K, htc::WG_BK);
-    const int64_t asz = (int64_t)g.batch * Mp * Kp, bsz = (int64_t)g.batch * Np * Kp;
-    htc::bf16_t* a_hi = ws;
-    htc::bf16_t* a_lo = x3 ? a_hi + asz : nullptr;
-    htc::bf16_t* b_hi = a_hi + (x3 ? 2 : 1) * asz;
-    htc::bf16_t* b_lo = x3 ? b_hi + bsz : nullptr;
-    htc::tc_pack_kernel<<<dim3(Kp / 32, Mp / 32, g.batch), dim3(32, 8), 0, st>>>(g.A, g.sam, g.sak, g.zA, g.M, g.K, Mp, Kp, g.mask_period,
-                                                                                g.mask_skip, a_hi, a_lo);
-    LAUNCH_CHECK();
-    htc::tc_pack_kernel<<<dim3(Kp / 32, Np / 32, g.batch), dim3(32, 8), 0, st>>>(g.B, g.sbn, g.sbk, g.zB, g.N, g.K, Np, Kp, g.mask_period,
-                                                                                g.mask_skip, b_hi, b_lo);
-    LAUNCH_CHECK();
-    CUtensorMap ta_hi, ta_lo, tb_hi, tb_lo;
-    TRY(make_pack_map(&ta_hi, a_hi, (int64_t)g.batch * Mp, Kp));
-    TRY(make_pack_map(&tb_hi, b_hi, (int64_t)g.batch * Np, Kp));
-    if (x3) {
-        TRY(make_pack_map(&ta_lo, a_lo, (int64_t)g.batch * Mp, Kp));
-        TRY(make_pack_map(&tb_lo, b_lo, (int64_t)g.batch * Np, Kp));
-    } else {
-        ta_lo = ta_hi; tb_lo = tb_hi;
-    }
-    htc::WgOut o{g.C, g.bias, g.M, g.N, Kp / htc::WG_BK, Mp, Np, g.splitk, g.beta, g.ldc, g.zC, g.zBias};
-    dim3 grid(Np / htc::WG_BN, Mp / htc::WG_BM, g.batch * g.splitk);
-    constexpr int X3_STAGES = 3, BF_STAGES = 4;
-    if (x3) {
-        const int smem = X3_STAGES * 2 * 2 * 16384 + 1024 + 2 * X3_STAGES * 8;
-        CUDA_TRY(cudaFuncSetAttribute(htc::wg_gemm_kernel<3, X3_STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        htc::wg_gemm_kernel<3, X3_STAGES><<<grid, 384, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, o);
-    } else {
-        const int smem = BF_STAGES * 2 * 16384 + 1024 + 2 * BF_STAGES * 8;
-        CUDA_TRY(cudaFuncSetAttribute(htc::wg_gemm_kernel<1, BF_STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        htc::wg_gemm_kernel<1, BF_STAGES><<<grid, 384, smem, st>>>(ta_hi, ta_lo, tb_hi, tb_lo, o);
-    }
+template <int NS, int AMN, int BMN>
+static int wg_launch(const CUtensorMap (&tm)[4], const htc::WgJob& j, int grid, cudaStream_t st) {
+    constexpr int STAGES = NS == 1 ? 4 : 3;
+    const int smem = STAGES * 2 * (NS == 1 ? 1 : 2) * 16384 + 1024 + 2 * STAGES * 8;
+    auto k = htc::wg_gemm_kernel<NS, STAGES, AMN, BMN>;
+    CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    k<<<grid, 384, smem, st>>>(tm[0], tm[1], tm[2], tm[3], j);
     LAUNCH_CHECK();
     return BIGRU_OK;
+}
+
+// runs j (M, N, batch, kblocks, kbd, kcat, C, bias, beta, ldc, zC, zBias, a/b coordinates set; tm, tn, part filled here)
+// over planes A and B; split-K partials (j.splits > 1) go to j.part and are reduced into C in split order
+static int wg_gemm(htc::WgJob j, const Planes& A, bool amn, const Planes& B, bool bmn, int prec, cudaStream_t st) {
+    if (j.M <= 0 || j.N <= 0) return BIGRU_OK;
+    const bool x3 = prec == BIGRU_PREC_BF16X3;
+    if (x3 != (A.lo != nullptr) || x3 != (B.lo != nullptr) || amn != bmn) {
+        bigru_set_error("tc_gemm: operand planes do not match the precision / majors");
+        return BIGRU_ERR_ARG;
+    }
+    j.tm = (int)cdiv64(j.M, htc::WG_BM);
+    j.tn = (int)cdiv64(j.N, htc::WG_BN);
+    CUtensorMap tm[4];
+    TRY(make_plane_map(&tm[0], A.hi, A, amn));
+    TRY(make_plane_map(&tm[2], B.hi, B, bmn));
+    if (x3) {
+        TRY(make_plane_map(&tm[1], A.lo, A, amn));
+        TRY(make_plane_map(&tm[3], B.lo, B, bmn));
+    } else {
+        tm[1] = tm[0]; tm[3] = tm[2];
+    }
+    int dev = 0, nsm = 132;
+    CUDA_TRY(cudaGetDevice(&dev));
+    CUDA_TRY(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
+    const int64_t units = (int64_t)j.tm * j.tn * j.batch * j.splits;
+    const int grid = (int)std::min<int64_t>(units, nsm);
+    const int rc = amn ? (x3 ? wg_launch<3, 1, 1>(tm, j, grid, st) : wg_launch<1, 1, 1>(tm, j, grid, st))
+                       : (x3 ? wg_launch<3, 0, 0>(tm, j, grid, st) : wg_launch<1, 0, 0>(tm, j, grid, st));
+    TRY(rc);
+    if (j.splits > 1) {
+        const int64_t n = (int64_t)j.batch * j.M * j.N;
+        htc::splitk_reduce_kernel<<<(unsigned)std::min<int64_t>(cdiv64(n, 256), 132 * 8), 256, 0, st>>>(j.part, j.splits, j.batch, j.M,
+                                                                                                        j.N, j.C, j.ldc, j.zC, j.beta);
+        LAUNCH_CHECK();
+    }
+    return BIGRU_OK;
+}
+
+static htc::WgJob wg_job(float* C, int M, int N, int64_t ldc, int batch, int64_t kblocks) {
+    htc::WgJob j{};
+    j.C = C; j.M = M; j.N = N; j.ldc = ldc; j.batch = batch; j.kblocks = (int)kblocks; j.kbd = (int)kblocks; j.splits = 1;
+    return j;
+}
+
+// packs batch x [R][K] fp32 (element (r, k) at src[z * zsrc + r * s_r + k * s_k]) into K-major planes at ws (timed as pack_bf16)
+static int tc_pack(const float* src, int64_t s_r, int64_t s_k, int64_t zsrc, int R, int K, int batch, int prec, htc::bf16_t* ws,
+                   Planes* out, cudaStream_t st) {
+    const bool x3 = prec == BIGRU_PREC_BF16X3;
+    const int Rp = (int)rup(R, htc::WG_BM), Kp = (int)rup(K, htc::WG_BK);
+    const int64_t sz = (int64_t)batch * Rp * Kp;
+    *out = Planes{ws, x3 ? ws + sz : nullptr, Kp, Rp, batch, Kp};
+    KLAUNCH(KC_PACK, 0.0, (4.0 + (x3 ? 4.0 : 2.0)) * batch * (double)R * K, st,
+            htc::tc_pack_kernel<<<dim3(Kp / 32, Rp / 32, batch), dim3(32, 8), 0, st>>>(src, s_r, s_k, zsrc, R, K, Rp, Kp, ws,
+                                                                                     x3 ? ws + sz : nullptr));
+    return BIGRU_OK;
+}
+
+// the strided fp32 GEMM contract of sgemm_kernel (GemmArgs; no split-K, no row mask) for the small head and h0 GEMMs:
+// both operands packed, then wg_gemm.  ws: tc_gemm_ws_elems(...) bf16 elements
+static int tc_gemm_launch(const GemmArgs& g, int prec, int cls, htc::bf16_t* ws, cudaStream_t st) {
+    if (g.M <= 0 || g.N <= 0 || g.K <= 0) return BIGRU_OK;
+    if (g.splitk != 1 || g.mask_period) {
+        bigru_set_error("tc_gemm_launch: split-K and row masks are not supported");
+        return BIGRU_ERR_ARG;
+    }
+    Planes A, B;
+    TRY(tc_pack(g.A, g.sam, g.sak, g.zA, g.M, g.K, g.batch, prec, ws, &A, st));
+    TRY(tc_pack(g.B, g.sbn, g.sbk, g.zB, g.N, g.K, g.batch, prec, ws + tc_pack_elems(g.M, g.K, g.batch, prec), &B, st));
+    ProfScope ps(cls, 2.0 * g.M * g.N * (double)g.K * g.batch, 0.0, st);
+    htc::WgJob j = wg_job(g.C, g.M, g.N, g.ldc, g.batch, cdiv64(g.K, htc::WG_BK));
+    j.bias = g.bias; j.beta = g.beta; j.zC = g.zC; j.zBias = g.zBias;
+    j.a.zsel = 1; j.b.zsel = 1;
+    return wg_gemm(j, A, false, B, false, prec, st);
 }
 
 template <typename... KArgs, typename... Args>
@@ -639,11 +821,11 @@ static int launch_cluster(void (*kernel)(KArgs...), int cs, int ntiles, int D, i
 
 // one layer's forward recurrence; shapes were validated by the plan (H in {128, 256, 512}, B % 16 == 0)
 static int tc_scan_fwd(const bigru_plan& p, int l, const float* gi, const float* Whh, const float* bhh, const float* h0,
-                       float* Y, float* G, float* hn, cudaStream_t st) {
+                       float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, cudaStream_t st) {
     const int H = p.H, D = p.D, B = p.B, T = p.T, cs = H / htc::SCAN_U, nt = B / htc::SCAN_NB;
     const int64_t zW = p.ld_block(l);
     ProfScope ps(KC_TC_SCAN_FWD, 2.0 * D * B * (double)T * 3 * H * H, 0.0, st);
-#define FWD(HH, NS) return launch_cluster(htc::gru_scan_fwd_kernel<HH, NS>, cs, nt, D, htc::FwdSmem<HH, NS>::TOTAL, st, gi, Whh, bhh, zW, h0, Y, G, hn, B, T, D)
+#define FWD(HH, NS) return launch_cluster(htc::gru_scan_fwd_kernel<HH, NS>, cs, nt, D, htc::FwdSmem<HH, NS>::TOTAL, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D)
     if (p.prec == BIGRU_PREC_BF16X3) {
         if (H == 128) FWD(128, 3);
         if (H == 256) FWD(256, 3);
@@ -658,11 +840,12 @@ static int tc_scan_fwd(const bigru_plan& p, int l, const float* gi, const float*
 }
 
 static int tc_scan_bwd(const bigru_plan& p, int l, const float* G, const float* Y, const float* h0, const float* dY, float* dhc,
-                       float* dgi, float* dgh, const float* Whh, cudaStream_t st) {
+                       float* dgi, float* dgh, const float* Whh, htc::bf16_t* gih, htc::bf16_t* gil, htc::bf16_t* ghh,
+                       htc::bf16_t* ghl, cudaStream_t st) {
     const int H = p.H, D = p.D, B = p.B, T = p.T, cs = H / htc::SCAN_U, nt = B / htc::SCAN_NB;
     const int64_t zW = p.ld_block(l);
     ProfScope ps(KC_TC_SCAN_BWD, 2.0 * D * B * (double)T * 3 * H * H, 0.0, st);
-#define BWD(HH, NS) return launch_cluster(htc::gru_scan_bwd_kernel<HH, NS>, cs, nt, D, htc::BwdSmem<HH, NS>::TOTAL, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, B, T, D)
+#define BWD(HH, NS) return launch_cluster(htc::gru_scan_bwd_kernel<HH, NS>, cs, nt, D, htc::BwdSmem<HH, NS>::TOTAL, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D)
     if (p.prec == BIGRU_PREC_BF16X3) {
         if (H == 128) BWD(128, 3);
         if (H == 256) BWD(256, 3);

@@ -116,10 +116,12 @@ int  bigru_loss(int kind, const float* d_logits, const void* d_target, const flo
                 float* d_dlogits, void* stream);
 
 /* --- nn.utils.clip_grad_norm_ + optimizer.step() (biGRU_model.py:208-210, Adam, notebook raw :1194)
- *  bigru_sqnorm accumulates sum(g^2) into *d_out (caller zeroes it first);
+ *  bigru_sqnorm accumulates sum(g^2) into *d_out (caller zeroes it first); d_ws: BIGRU_SQNORM_WS floats of
+ *  device scratch for the per-block partial sums, which are added in a fixed order (bit-reproducible);
  *  bigru_clip_adam_step: g *= grad_scale; coef = min(1, clip/(sqrt(*d_sqnorm)*grad_scale+1e-6));
  *  g *= coef; Adam(lr,b1,b2,eps) with bias correction for `step` (1-based). */
-int  bigru_sqnorm(const float* d_g, int64_t n, float* d_out, void* stream);
+#define BIGRU_SQNORM_WS 528
+int  bigru_sqnorm(const float* d_g, int64_t n, float* d_out, float* d_ws, void* stream);
 int  bigru_clip_adam_step(float* d_params, float* d_grads, float* d_m, float* d_v, int64_t n,
                           const float* d_sqnorm, float clip, float lr, float b1, float b2, float eps,
                           int step, float grad_scale, void* stream);
