@@ -35,14 +35,12 @@ SIGNATURES = {
     "bigru_backward_layers": (_i, [_vp, _vp, _vp, _vp, _f, _i, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     "bigru_loss": (_i, [_i, _vp, _vp, _vp, _vp, _i, _i, _d, _vp, _vp, _vp]),
     "bigru_sqnorm": (_i, [_vp, _i64, _vp, _vp, _vp]),
-    "bigru_clip_adam_step": (_i, [_vp, _vp, _vp, _vp, _i64, _vp, _f, _f, _f, _f, _f, _i, _f, _vp]),
     "bigru_adam_tick": (_i, [_vp, _vp, _vp]),
     "bigru_clip_adam_step_dev": (_i, [_vp, _vp, _vp, _vp, _i64, _vp, _f, _f, _f, _f, _f, _vp, _f, _vp]),
     "bigru_launch_count_add": (None, [C.c_longlong]),
     "bigru_window_gather_norm": (_i, [_vp, _vp, _vp, _i64, _i64, _i, _i, _i, _vp, _vp]),
     "bigru_window_targets": (_i, [_vp, _i64, _i64, _i, _i, _i, _vp, _vp]),
     "bigru_multilabel_counts": (_i, [_vp, _vp, _i, _i, _vp, _vp]),
-    "bigru_forward_windows": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _i64, _f, _i, _i, _u64, _vp, _vp, _vp, _vp, _vp]),
     "bigru_chunk_minmax": (_i, [_vp, _i64, _i, _i64, _i64, _vp, _vp, _vp]),
     "bigru_infer_window": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "bigru_window_features": (_i, [_vp, _vp, _vp, _vp, _vp, _i64, C.POINTER(_i), _i, C.POINTER(_i), _i, C.POINTER(_i), _i, _i, _f, _i,

@@ -42,6 +42,20 @@ def _stream_ptr(device=None):
     return torch.cuda.current_stream(device).cuda_stream
 
 
+def _pad_batch(x, h0, Bp):
+    """x [B, T, F] and h0 [L*D, B, H] (or None) with zero rows appended up to batch Bp (BiGRU._padded_batch)."""
+    B = x.shape[0]
+    if Bp == B:
+        return x, h0
+    xp = x.new_zeros((Bp,) + tuple(x.shape[1:]))
+    xp[:B] = x
+    if h0 is not None:
+        hp = h0.new_zeros(h0.shape[0], Bp, h0.shape[2])
+        hp[:, :B] = h0
+        h0 = hp
+    return xp, h0
+
+
 class _GRUWeights(nn.Module):
     """Holds the recurrent parameters under torch.nn.GRU's names, shapes, registration order and
     initialisation (U(-1/sqrt(H), 1/sqrt(H)), drawn in registration order), i.e. what
@@ -113,14 +127,7 @@ class _BiGRUFunction(torch.autograd.Function):
         lib = _lib.load()
         B = x.shape[0]
         Bp = model._padded_batch(B)
-        if Bp != B:                                       # whole batch tiles on the tensor-core paths: zero rows appended
-            xp = x.new_zeros((Bp,) + tuple(x.shape[1:]))
-            xp[:B] = x
-            x = xp
-            if h0 is not None:
-                hp = h0.new_zeros(h0.shape[0], Bp, h0.shape[2])
-                hp[:, :B] = h0
-                h0 = hp
+        x, h0 = _pad_batch(x, h0, Bp)
         plan = model._plan_for(x)
         ctx.dev_guard = torch.cuda.device(x.device)      # the C ABI launches on the CURRENT device: make it the model's
         ctx.dev_guard.__enter__()
@@ -719,17 +726,6 @@ class BiGRU(nn.Module):
             wv, pwv = self._loss_vec(w, C), self._loss_vec(pw, C)
             st = self._fused_state(dev)
             x_real = x
-
-            def padded(x, h0):                                # whole batch tiles on the tensor-core paths (see _padded_batch)
-                if Bp == B:
-                    return x, h0
-                xp = x.new_zeros(Bp, x.shape[1], x.shape[2])
-                xp[:B] = x
-                if h0 is not None:
-                    hp = h0.new_zeros(h0.shape[0], Bp, h0.shape[2])
-                    hp[:, :B] = h0
-                    h0 = hp
-                return xp, h0
             h0 = self._pad_last(h0, self.plan_hidden(B))
             self._last_batch = B
             if self.use_cuda_graph and not training and h0 is None and not torch.cuda.is_current_stream_capturing():
@@ -738,7 +734,7 @@ class BiGRU(nn.Module):
                 try:
                     ent = self._graphs.get(key)
                     if ent is None:
-                        ent = self._graph_for(key, padded(x, None)[0], tgt, kind, wv, pwv, denom, g)
+                        ent = self._graph_for(key, _pad_batch(x, None, Bp)[0], tgt, kind, wv, pwv, denom, g)
                 except Exception as e:                        # capture is an optimisation: fall back to plain launches
                     import warnings
                     warnings.warn(f"BiGRU.train_step: CUDA-graph capture failed ({e}); using plain launches")
@@ -759,7 +755,7 @@ class BiGRU(nn.Module):
                     self._bump_step(st, 1)
                     lib.bigru_launch_count_add(ent["launches"])
                     return st["loss"].clone(), ent["logits"][:B].clone()
-            x, h0 = padded(x, h0)
+            x, h0 = _pad_batch(x, h0, Bp)
             plan = self._plan_for(x)
             logits = torch.empty(Bp, C, device=dev, dtype=torch.float32)
             dlogits = torch.zeros_like(logits) if Bp != B else torch.empty_like(logits)
@@ -781,9 +777,9 @@ class BiGRU(nn.Module):
             self._launch_update(lib, g, st, s)
             return st["loss"].clone(), (logits[:B] if Bp != B else logits)
 
-    # ------------------------------------------------------------------ zero-copy windows (SURVEY.md 8(f) N1)
+    # ------------------------------------------------------------------ windows of a chunk-resident dataset (SURVEY.md 8(f) N1)
     def _window_args(self, dataset, start, count):
-        if dataset.device != self._flat.device:
+        if dataset.device != self.flat_parameters().device:
             raise RuntimeError("dataset and model live on different devices")
         if dataset.n_features != self.n_features:
             raise ValueError(f"dataset has {dataset.n_features} features, the model expects {self.n_features}")
@@ -791,71 +787,23 @@ class BiGRU(nn.Module):
             raise ValueError(f"windows [{start}, {start + count}) of width {dataset.window} exceed the {dataset.n_rows}-row chunk")
 
     def forward_windows(self, dataset, start: int, count: int):
-        """Logits for windows start .. start+count-1 of a chunk-resident ``MySQLBatchLoader`` without materialising
-        x[count, window, F]: the first kernel of the path reads (and normalises) the rows of the chunk directly."""
-        if not self._is_flat():
-            self._flatten()
-        lib = _lib.load()
+        """Logits (no autograd graph) for windows start .. start+count-1 of a chunk-resident ``MySQLBatchLoader``: only the
+        chunk's rows cross the host link; the windows are collated and normalised on the device (one gather kernel), then
+        ``forward`` runs on them."""
         self._window_args(dataset, start, count)
-        if self._padded_batch(count) != count or self.plan_hidden(count) != self.hidden_size:      # padded shapes: collate on the device first
-            self._win_ctx = None
+        with torch.no_grad():
             return self.forward(dataset.collate(start, count)[0])
-        plan = self._plan_for(torch.empty(count, dataset.window, 0, device=self._flat.device))     # keyed by (B, T)
-        logits = torch.empty(count, self.output_size, device=self._flat.device, dtype=torch.float32)
-        stash = plan.acquire_stash()
-        training = bool(self.training and self.dropout_p > 0)
-        seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if training else 0
-        with torch.cuda.device(self._flat.device):
-            _lib.check(lib.bigru_forward_windows(plan.handle, _lib.ptr(self._flat), _lib.ptr(dataset.x_raw), _lib.ptr(dataset.x_min),
-                                                 _lib.ptr(dataset.x_max), int(start), dataset.n_rows, float(self.dropout_p),
-                                                 int(bool(self.spatial_dropout)), int(training), seed, _lib.ptr(stash),
-                                                 _lib.ptr(plan.scratch), _lib.ptr(logits), None, _stream_ptr(self._flat.device)),
-                       "bigru_forward_windows")
-        self._win_ctx = (plan, stash, training, seed)
-        return logits
 
     def train_step_windows(self, dataset, start: int, count: int):
-        """``train_step`` on windows of a chunk-resident dataset (inputs and targets gathered on the device, the
-        fp32 batch never exists).  Returns (loss, logits)."""
-        spec, g = self._loss_spec(), self._adam_spec()
-        if spec is None or g is None:
+        """``train_step`` on windows of a chunk-resident dataset, inputs and targets collated on the device.
+        Returns (loss, logits)."""
+        spec = self._loss_spec()
+        if spec is None or self._adam_spec() is None:
             raise RuntimeError("train_step_windows needs a fusable loss and torch.optim.Adam (see train_step)")
-        lib = _lib.load()
-        kind, w, pw = spec
-        if self._padded_batch(count) != count or self.plan_hidden(count) != self.hidden_size:      # padded shapes: collate, then train_step
-            self._window_args(dataset, start, count)
-            x, y = dataset.collate(start, count)
-            tgt = y.reshape(count, -1)[:, 0].to(torch.int64) if kind == _lib.LOSS_CE else y.reshape(count, self.output_size)
-            return self.train_step(x, tgt)
-        logits = self.forward_windows(dataset, start, count)
-        plan, stash, training, seed = self._win_ctx
-        dev, B, C = logits.device, count, self.output_size
-        with torch.cuda.device(dev):
-            y = torch.empty(count, 1, dataset.n_targets, device=dev, dtype=torch.float32)
-            s = _stream_ptr(dev)
-            _lib.check(lib.bigru_window_targets(_lib.ptr(dataset.y), int(start), dataset.n_rows, count, dataset.window,
-                                                dataset.n_targets, _lib.ptr(y), s), "bigru_window_targets")
-            if kind == _lib.LOSS_CE:
-                tgt = y.reshape(count, -1)[:, 0].to(torch.int64).contiguous()
-                denom = float(B * self._dp_world)
-            else:
-                tgt = y.reshape(count, C).contiguous()
-                denom = float(B * C * self._dp_world)
-            st = self._fused_state(dev)
-            dlogits = torch.empty_like(logits)
-            wv, pwv = self._loss_vec(w, C), self._loss_vec(pw, C)
-            _lib.check(lib.bigru_loss(kind, _lib.ptr(logits), _lib.ptr(tgt), _lib.ptr(wv), _lib.ptr(pwv), B, C, denom,
-                                      _lib.ptr(st["loss"]), _lib.ptr(dlogits), s), "bigru_loss")
-            _lib.check(lib.bigru_backward(plan.handle, _lib.ptr(self._flat), None, None, float(self.dropout_p),
-                                          int(bool(self.spatial_dropout)), int(training), seed, _lib.ptr(stash),
-                                          _lib.ptr(plan.scratch), _lib.ptr(dlogits), _lib.ptr(st["grad"]), None, None, s),
-                       "bigru_backward")
-            plan.release_stash(stash)
-            self._win_ctx = None
-            if self._dp_world > 1:
-                allreduce_flat_(st["gext"], self._dp_group)
-            self._launch_update(lib, g, st, s)
-            return st["loss"].clone(), logits
+        self._window_args(dataset, start, count)
+        x, y = dataset.collate(start, count)
+        tgt = y.reshape(count, -1)[:, 0].to(torch.int64) if spec[0] == _lib.LOSS_CE else y.reshape(count, self.output_size)
+        return self.train_step(x, tgt)
 
     def _generic_step(self, x, target):
         """Any loss / optimiser: autograd drives the same CUDA forward/backward kernels."""

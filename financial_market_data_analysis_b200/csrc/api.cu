@@ -17,7 +17,7 @@ void bigru_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* bigru_last_error(void) { return g_err; }
-extern "C" int bigru_version(void) { return 200; }
+extern "C" int bigru_version(void) { return 201; }
 
 extern "C" int bigru_device_check(int dev) {
     int n = 0;
@@ -320,8 +320,9 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
     const StashF32 S = stash_layout(p);
     const ScratchF32 W = scratch_layout(p);
     const int B = p.B, T = p.T, H = p.H, D = p.D, C = p.C;
-    const int64_t BT = (int64_t)B * T;
+    const int64_t BT = (int64_t)B * T, H3 = 3LL * H;
     const bool do_drop = training && drop > 0.f;
+    const bool tc = p.prec != BIGRU_PREC_FP32;
     float* dhc = scratch + W.dhc;
     if (layer_from == p.L - 1) {
         CUDA_TRY(cudaMemsetAsync(grads, 0, sizeof(float) * p.nparams, st));
@@ -336,6 +337,7 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
     for (int l = layer_from; l >= layer_to; --l) {
         const int I = (int)p.in_size(l);
         const bool even = (p.L - 1 - l) % 2 == 0;
+        const bool drop_l = do_drop && (l == 0 || p.L > 1);
         float* dY = scratch + (even ? W.dYa : W.dYb);
         float* dYnext = scratch + (even ? W.dYb : W.dYa);
         const float* Y = stash + S.Y[l];
@@ -344,9 +346,10 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
         float* dgi = scratch + W.dgi;
         float* dgh = scratch + W.dgh;
         if (l != p.L - 1) CUDA_TRY(cudaMemsetAsync(dhc, 0, sizeof(float) * D * B * H, st));
-        const Planes gip = plan_planes(p, scratch, W.dgiP, 3LL * H, BT, D, 3LL * H);
-        const Planes ghp = plan_planes(p, scratch, W.dghP, 3LL * H, BT, D, 3LL * H);
-        if (p.prec != BIGRU_PREC_FP32) {
+        const Planes gip = plan_planes(p, scratch, W.dgiP, H3, BT, D, H3);
+        const Planes ghp = plan_planes(p, scratch, W.dghP, H3, BT, D, H3);
+        // recurrence: dgi, dgh [D][B*T][3H] and dh0 in dhc
+        if (tc) {
             TRY(tc_scan_bwd(p, l, G, Y, h0l, dY, dhc, dgi, dgh, params + p.off_whh(l, 0), mut(gip), mut_lo(gip), mut(ghp), mut_lo(ghp), st));
         } else {
             for (int s = 0; s < T; ++s) {
@@ -362,23 +365,19 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
         }
         if (dh0) CUDA_TRY(cudaMemcpyAsync(dh0 + (int64_t)l * D * B * H, dhc, sizeof(float) * D * B * H,
                                           cudaMemcpyDeviceToDevice, st));
-        // layer input as seen by the projection (dropped copy when dropout was applied)
-        const float* inp = l == 0 ? (x ? x : stash + S.X[0]) : stash + S.Y[l - 1];     // x == NULL: forward_windows left it in the stash
-        if (do_drop && (l == 0 || p.L > 1)) inp = stash + S.X[l];
-        if (p.prec != BIGRU_PREC_FP32) {
-            const int64_t kb = cdiv64(BT, htc::WG_BK), H3 = 3LL * H;
+        // dW_ih[d] = dgi[d]^T X and dW_hh[d] = dgh[d]^T H_prev, H_prev(b,t) = Y[b,t-1] (dir 0) / Y[b,t+1] (dir 1), the columns
+        // of direction d.  The first step's h_prev is h0: its term is the w0 GEMM below.
+        if (tc) {
+            const int64_t kb = cdiv64(BT, htc::WG_BK);
             float* part = scratch + W.part;
-            // dW_ih[d] = dgi[d]^T X, both directions in one launch
-            const Planes xp = input_planes(p, stash, l, l == 0 || do_drop);
             {
                 ProfScope ps(KC_TC_GEMM_DWIH, 2.0 * H3 * I * (double)BT * D, 0.0, st);
                 htc::WgJob j = wg_job(grads + p.off_wih(l, 0), (int)H3, I, I, D, kb);
                 j.zC = p.ld_block(l); j.a.zsel = 1; j.part = part;
                 j.splits = wg_splits(cdiv64(H3, htc::WG_BM) * cdiv64(I, htc::WG_BN) * D, kb);
-                TRY(wg_gemm(j, gip, true, xp, true, p.prec, st));
+                TRY(wg_gemm(j, gip, true, input_planes(p, stash, l, l == 0 || do_drop), true, p.prec, st));
             }
-            // dW_hh[d] = dgh[d]^T H_prev: H_prev(b,t) = Y[b,t-1] (dir 0) / Y[b,t+1] (dir 1), the columns of direction d.  The
-            // dgh planes are zero at each sequence's first step, whose h0 term the w0 GEMM below adds from fp32 dgh.
+            // the dgh planes are zero at each sequence's first step, so the ±1-row shift needs no mask
             if (T > 1) {
                 ProfScope ps(KC_TC_GEMM_DWHH, 2.0 * H3 * H * (double)BT * D, 0.0, st);
                 htc::WgJob j = wg_job(grads + p.off_whh(l, 0), (int)H3, H, H, D, kb);
@@ -387,57 +386,34 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
                 j.splits = wg_splits(cdiv64(H3, htc::WG_BM) * cdiv64(H, htc::WG_BN) * D, kb);
                 TRY(wg_gemm(j, ghp, true, plan_planes(p, stash, S.YP[l], (int64_t)D * H, BT, 1, (int64_t)D * H), true, p.prec, st));
             }
+        } else {
+            // the layer input as the projection saw it (the dropped copy when dropout was applied)
+            const float* inp = drop_l ? stash + S.X[l] : l == 0 ? x : stash + S.Y[l - 1];
+            const int splitk = (int)min((int64_t)64, max((int64_t)1, BT / 512));
             for (int d = 0; d < D; ++d) {
                 const float* dgi_d = dgi + (int64_t)d * BT * 3 * H;
                 const float* dgh_d = dgh + (int64_t)d * BT * 3 * H;
-                if (h0l) {
-                    const int tf = d == 0 ? 0 : T - 1;
-                    GemmArgs w0 = gemm_args(dgh_d + (int64_t)tf * 3 * H, h0l + (int64_t)d * B * H, grads + p.off_whh(l, d),
-                                            3 * H, H, B, 1, (int64_t)T * 3 * H, 1, H, H);
-                    w0.beta = 1;
-                    TRY(plan_gemm(p, w0, KC_TC_GEMM_DWHH, scratch, st));
+                GemmArgs wi = gemm_args(dgi_d, inp, grads + p.off_wih(l, d), 3 * H, I, (int)BT, 1, 3 * H, 1, I, I);
+                wi.splitk = splitk;
+                TRY(sgemm_launch(wi, st));
+                if (T > 1) {
+                    const float* hp = Y + (int64_t)d * H + (d == 0 ? -(int64_t)D * H : (int64_t)D * H);
+                    GemmArgs wh = gemm_args(dgh_d, hp, grads + p.off_whh(l, d), 3 * H, H, (int)BT, 1, 3 * H, 1,
+                                            (int64_t)D * H, H);
+                    wh.splitk = splitk; wh.mask_period = T; wh.mask_skip = d == 0 ? 0 : T - 1;
+                    TRY(sgemm_launch(wh, st));
                 }
-                TRY(colsum_launch(dgi_d, grads + p.off_bih(l, d), BT, 3 * H, 3 * H, 1, 0, 0, scratch + W.csum, st));
-                TRY(colsum_launch(dgh_d, grads + p.off_bhh(l, d), BT, 3 * H, 3 * H, 1, 0, 0, scratch + W.csum, st));
             }
-            // dX = sum_d dgi[d] W_ih[d]: one K loop over direction 0, then direction 1
-            float* dxo = l == 0 ? dx : dYnext;
-            if (dxo) {
-                Planes wp;
-                TRY(tc_pack(params + p.off_wih(l, 0), 1, I, p.ld_block(l), I, 3 * H, D, p.prec, reinterpret_cast<htc::bf16_t*>(scratch + W.tcw),
-                            &wp, st));
-                {
-                    ProfScope ps(KC_TC_GEMM_DX, 2.0 * BT * I * (double)H3 * D, 0.0, st);
-                    htc::WgJob j = wg_job(dxo, (int)BT, I, I, 1, D * (H3 / htc::WG_BK));
-                    j.kbd = (int)(H3 / htc::WG_BK); j.kcat = 1; j.a.zsel = 1; j.b.zsel = 1;
-                    TRY(wg_gemm(j, gip, false, wp, false, p.prec, st));
-                }
-                if (do_drop && (l == 0 || p.L > 1))
-                    KLAUNCH(KC_MISC, 0.0, 0.0, st, dropout_kernel<<<132 * 8, 256, 0, st>>>(dxo, dxo, BT * I, T, I, l == 0 ? spatial : 0, drop, seed, (uint32_t)l));
-            }
-            continue;
         }
-        const int splitk = (int)min((int64_t)64, max((int64_t)1, BT / 512));
+        // dW_hh[d] += dgh[d]_first^T h0[d]; bias gradients are column sums of dgi and dgh
         for (int d = 0; d < D; ++d) {
             const float* dgi_d = dgi + (int64_t)d * BT * 3 * H;
             const float* dgh_d = dgh + (int64_t)d * BT * 3 * H;
-            // dW_ih = dgi^T X
-            GemmArgs wi = gemm_args(dgi_d, inp, grads + p.off_wih(l, d), 3 * H, I, (int)BT, 1, 3 * H, 1, I, I);
-            wi.splitk = splitk;
-            TRY(plan_gemm(p, wi, KC_TC_GEMM_DWIH, scratch, st));
-            // dW_hh = dgh^T H_prev ; H_prev(b,t) = Y[b,t-1] (dir 0) / Y[b,t+1] (dir 1), h0 at the first step
-            if (T > 1) {
-                const float* hp = Y + (int64_t)d * H + (d == 0 ? -(int64_t)D * H : (int64_t)D * H);
-                GemmArgs wh = gemm_args(dgh_d, hp, grads + p.off_whh(l, d), 3 * H, H, (int)BT, 1, 3 * H, 1,
-                                        (int64_t)D * H, H);
-                wh.splitk = splitk; wh.mask_period = T; wh.mask_skip = d == 0 ? 0 : T - 1;
-                TRY(plan_gemm(p, wh, KC_TC_GEMM_DWHH, scratch, st));
-            }
             if (h0l) {
                 const int tf = d == 0 ? 0 : T - 1;
                 GemmArgs w0 = gemm_args(dgh_d + (int64_t)tf * 3 * H, h0l + (int64_t)d * B * H, grads + p.off_whh(l, d),
                                         3 * H, H, B, 1, (int64_t)T * 3 * H, 1, H, H);
-                w0.splitk = 2;       // forces the atomic-accumulate epilogue onto the existing sums
+                w0.beta = 1;
                 TRY(plan_gemm(p, w0, KC_TC_GEMM_DWHH, scratch, st));
             }
             TRY(colsum_launch(dgi_d, grads + p.off_bih(l, d), BT, 3 * H, 3 * H, 1, 0, 0, scratch + W.csum, st));
@@ -445,18 +421,27 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
         }
         // dX = sum_d dgi[d] W_ih[d]
         float* dxo = l == 0 ? dx : dYnext;
-        if (dxo) {
+        if (!dxo) continue;
+        if (tc) {
+            // one K loop over direction 0, then direction 1
+            Planes wp;
+            TRY(tc_pack(params + p.off_wih(l, 0), 1, I, p.ld_block(l), I, 3 * H, D, p.prec, reinterpret_cast<htc::bf16_t*>(scratch + W.tcw),
+                        &wp, st));
+            ProfScope ps(KC_TC_GEMM_DX, 2.0 * BT * I * (double)H3 * D, 0.0, st);
+            htc::WgJob j = wg_job(dxo, (int)BT, I, I, 1, D * (H3 / htc::WG_BK));
+            j.kbd = (int)(H3 / htc::WG_BK); j.kcat = 1; j.a.zsel = 1; j.b.zsel = 1;
+            TRY(wg_gemm(j, gip, false, wp, false, p.prec, st));
+        } else {
             for (int d = 0; d < D; ++d) {
                 GemmArgs gx = gemm_args(dgi + (int64_t)d * BT * 3 * H, params + p.off_wih(l, d), dxo, (int)BT, I, 3 * H,
                                         3 * H, 1, 1, I, I);
                 gx.beta = d;
-                TRY(plan_gemm(p, gx, KC_TC_GEMM_DX, scratch, st));
-            }
-            if (do_drop && (l == 0 || p.L > 1)) {
-                // d(dropout): same mask, in place.  dropout_kernel(in=dxo) multiplies by mask/(1-p)
-                KLAUNCH(KC_MISC, 0.0, 0.0, st, dropout_kernel<<<132 * 8, 256, 0, st>>>(dxo, dxo, BT * I, T, I, l == 0 ? spatial : 0, drop, seed, (uint32_t)l));
+                TRY(sgemm_launch(gx, st));
             }
         }
+        // d(dropout): the same mask, in place (dropout_kernel multiplies by mask / (1 - p))
+        if (drop_l)
+            KLAUNCH(KC_MISC, 0.0, 0.0, st, dropout_kernel<<<132 * 8, 256, 0, st>>>(dxo, dxo, BT * I, T, I, l == 0 ? spatial : 0, drop, seed, (uint32_t)l));
     }
     return BIGRU_OK;
 }
@@ -480,7 +465,7 @@ extern "C" int bigru_backward(const bigru_plan* plan, const float* d_params, con
                               float dropout_p, int spatial, int training, uint64_t seed, const void* d_stash,
                               void* d_scratch, const float* d_dlogits, float* d_grads, float* d_dx, float* d_dh0,
                               void* stream) {
-    if (!plan || !d_params || !d_stash || !d_scratch || !d_dlogits || !d_grads) {
+    if (!plan || !d_params || !d_x || !d_stash || !d_scratch || !d_dlogits || !d_grads) {
         bigru_set_error("backward: null argument");
         return BIGRU_ERR_ARG;
     }
@@ -492,7 +477,7 @@ extern "C" int bigru_backward_layers(const bigru_plan* plan, const float* d_para
                                      float dropout_p, int spatial, int training, uint64_t seed, const void* d_stash,
                                      void* d_scratch, const float* d_dlogits, float* d_grads, float* d_dx, float* d_dh0,
                                      int layer_from, int layer_to, void* stream) {
-    if (!plan || !d_params || !d_stash || !d_scratch || !d_dlogits || !d_grads) {
+    if (!plan || !d_params || !d_x || !d_stash || !d_scratch || !d_dlogits || !d_grads) {
         bigru_set_error("backward_layers: null argument");
         return BIGRU_ERR_ARG;
     }
@@ -506,27 +491,6 @@ extern "C" int bigru_backward_layers(const bigru_plan* plan, const float* d_para
     }
     return backward_plan(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, (const float*)d_stash,
                          (float*)d_scratch, d_dlogits, d_grads, d_dx, d_dh0, (cudaStream_t)stream, layer_from, layer_to);
-}
-
-extern "C" int bigru_forward_windows(const bigru_plan* plan, const float* d_params, const float* d_src, const float* d_xmin,
-                                     const float* d_xmax, int64_t start, int64_t N, float dropout_p, int spatial,
-                                     int training, uint64_t seed, void* d_stash, void* d_scratch, float* d_logits,
-                                     float* d_hn, void* stream) {
-    if (!plan || !d_params || !d_src || !d_stash || !d_scratch || !d_logits || ((d_xmin == nullptr) != (d_xmax == nullptr))) {
-        bigru_set_error("forward_windows: null argument");
-        return BIGRU_ERR_ARG;
-    }
-    if (start < 0 || start + plan->B + plan->T - 1 > N) {
-        bigru_set_error("forward_windows: windows [%lld, %lld) exceed the %lld-row chunk", (long long)start,
-                        (long long)(start + plan->B + plan->T - 1), (long long)N);
-        return BIGRU_ERR_ARG;
-    }
-    if (dropout_p < 0.f || dropout_p >= 1.f) { bigru_set_error("forward_windows: dropout_p must be in [0,1)"); return BIGRU_ERR_ARG; }
-    // collate into the stash slot of the layer-0 input (the backward reads it there), then the ordinary forward
-    float* xw = (float*)d_stash + stash_layout(*plan).X[0];
-    TRY(bigru_window_gather_norm(d_src, d_xmin, d_xmax, start, N, plan->B, plan->T, plan->F, xw, stream));
-    return forward_plan(*plan, d_params, xw, nullptr, dropout_p, spatial, training, seed, (float*)d_stash,
-                        (float*)d_scratch, d_logits, d_hn, (cudaStream_t)stream);
 }
 
 extern "C" int bigru_chunk_minmax(const float* d_table, int64_t N, int F, int64_t row_lo, int64_t row_hi, float* d_min,
@@ -634,20 +598,6 @@ extern "C" int bigru_sqnorm(const float* d_g, int64_t n, float* d_out, float* d_
     const int blocks = (int)min((int64_t)BIGRU_SQNORM_WS, cdiv64(n, 256));
     KLAUNCH(KC_OPTIM, 0.0, 0.0, (cudaStream_t)stream, sqnorm_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d_g, n, d_ws));
     KLAUNCH(KC_OPTIM, 0.0, 0.0, (cudaStream_t)stream, sqnorm_finish_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(d_ws, blocks, d_out));
-    return BIGRU_OK;
-}
-
-extern "C" int bigru_clip_adam_step(float* d_params, float* d_grads, float* d_m, float* d_v, int64_t n,
-                                    const float* d_sqnorm, float clip, float lr, float b1, float b2, float eps,
-                                    int step, float grad_scale, void* stream) {
-    if (!d_params || !d_grads || !d_m || !d_v || !d_sqnorm || n <= 0 || step < 1) {
-        bigru_set_error("clip_adam_step: bad argument");
-        return BIGRU_ERR_ARG;
-    }
-    const double bc1 = 1.0 - pow((double)b1, step), bc2 = 1.0 - pow((double)b2, step);
-    const unsigned blocks = (unsigned)min((int64_t)132 * 8, cdiv64(n, 256));
-    KLAUNCH(KC_OPTIM, 0.0, 0.0, (cudaStream_t)stream, clip_adam_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d_params, d_grads, d_m, d_v, n, d_sqnorm, clip, lr, b1,
-                                                                b2, eps, (float)bc1, (float)sqrt(bc2), grad_scale));
     return BIGRU_OK;
 }
 

@@ -352,24 +352,7 @@ __global__ void sqnorm_finish_kernel(const float* __restrict__ ws, int nblocks, 
     if (threadIdx.x == 0) *out += v;
 }
 
-__global__ void clip_adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
-                                 float* __restrict__ v, int64_t n, const float* __restrict__ sqnorm, float clip,
-                                 float lr, float b1, float b2, float eps, float bc1, float bc2_sqrt, float gscale) {
-    const float norm = sqrtf(*sqnorm) * gscale;
-    const float coef = fminf(1.f, clip / (norm + 1e-6f)) * gscale;
-    const float step = lr / bc1;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        const float gq = g[i] * coef;
-        g[i] = gq;
-        const float mi = m[i] + (gq - m[i]) * (1.f - b1);        // lerp, as torch.optim.Adam does
-        const float vi = v[i] * b2 + (1.f - b2) * gq * gq;
-        m[i] = mi; v[i] = vi;
-        const float denom = sqrtf(vi) / bc2_sqrt + eps;
-        p[i] = p[i] - step * (mi / denom);
-    }
-}
-
-// device-resident step counter variant (CUDA-graph friendly: nothing about the step number is baked into the launch):
+// device-resident step counter (CUDA-graph friendly: nothing about the step number is baked into the launch):
 // adam_tick increments *step and clears the squared-norm accumulator; the update kernel forms the bias corrections itself
 __global__ void adam_tick_kernel(int* __restrict__ step, float* __restrict__ sqnorm) {
     if (threadIdx.x == 0 && blockIdx.x == 0) { *step += 1; *sqnorm = 0.f; }
@@ -386,7 +369,7 @@ __global__ void clip_adam_dev_kernel(float* __restrict__ p, float* __restrict__ 
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         const float gq = g[i] * coef;
         g[i] = gq;
-        const float mi = m[i] + (gq - m[i]) * (1.f - b1);
+        const float mi = m[i] + (gq - m[i]) * (1.f - b1);        // lerp, as torch.optim.Adam does
         const float vi = v[i] * b2 + (1.f - b2) * gq * gq;
         m[i] = mi; v[i] = vi;
         const float denom = sqrtf(vi) / bc2_sqrt + eps;

@@ -12,8 +12,8 @@
  *  - `stream` is a cudaStream_t passed as void*; all calls are asynchronous on that stream and
  *    never synchronise; a plan may be used from one stream at a time;
  *  - every function returns 0 on success, <0 on error (BIGRU_ERR_*); bigru_last_error() returns
- *    a thread-local message.  There is no CPU fallback anywhere: without a CUDA device of
- *    compute capability 10.x every compute call fails with BIGRU_ERR_DEVICE.
+ *    a thread-local message.  There is no CPU fallback anywhere: without an sm_90 (H100)
+ *    device every compute call fails with BIGRU_ERR_DEVICE.
  *
  * Flat parameter vector ("params", "grads", Adam moments): float32, order
  *     for l in [0,L): for d in [0,D):  w_ih[3H,I_l]  w_hh[3H,H]  b_ih[3H]  b_hh[3H]
@@ -60,7 +60,7 @@ typedef struct bigru_plan bigru_plan;
 
 const char* bigru_last_error(void);
 int  bigru_version(void);
-/* 0 when device `dev` exists and is compute capability 10.x */
+/* 0 when device `dev` exists and is an sm_90 (H100) device */
 int  bigru_device_check(int dev);
 
 /* --- plan: shapes, offsets, workspace sizes.  Replaces BiGRU.__init__ bookkeeping
@@ -89,9 +89,8 @@ int  bigru_forward(const bigru_plan* plan, const float* d_params, const float* d
                    void* d_stash, void* d_scratch, float* d_logits, float* d_hn, void* stream);
 
 /* --- loss.backward() through the model (biGRU_model.py:204): every parameter gradient into
- *  d_grads (flat, overwritten), optional d_dx[B,T,F] and d_dh0[L*D,B,H].  d_x may be NULL after
- *  bigru_forward_windows (the input is then taken from the stash).  Must follow
- *  bigru_forward on the same plan/stash with the same dropout arguments. */
+ *  d_grads (flat, overwritten), optional d_dx[B,T,F] and d_dh0[L*D,B,H].  d_x (required) is the
+ *  input the forward read.  Must follow bigru_forward on the same plan/stash with the same dropout arguments. */
 int  bigru_backward(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
                     float dropout_p, int spatial, int training, uint64_t seed,
                     const void* d_stash, void* d_scratch, const float* d_dlogits,
@@ -117,18 +116,13 @@ int  bigru_loss(int kind, const float* d_logits, const void* d_target, const flo
 
 /* --- nn.utils.clip_grad_norm_ + optimizer.step() (biGRU_model.py:208-210, Adam, notebook raw :1194)
  *  bigru_sqnorm accumulates sum(g^2) into *d_out (caller zeroes it first); d_ws: BIGRU_SQNORM_WS floats of
- *  device scratch for the per-block partial sums, which are added in a fixed order (bit-reproducible);
- *  bigru_clip_adam_step: g *= grad_scale; coef = min(1, clip/(sqrt(*d_sqnorm)*grad_scale+1e-6));
- *  g *= coef; Adam(lr,b1,b2,eps) with bias correction for `step` (1-based). */
+ *  device scratch for the per-block partial sums, which are added in a fixed order (bit-reproducible).
+ *  Adam's step count lives in device memory, so that the train step can be captured in a CUDA graph (SURVEY.md 8(f) N5):
+ *  bigru_adam_tick: *d_step += 1, *d_sqnorm = 0 (one tiny launch, before bigru_sqnorm);
+ *  bigru_clip_adam_step_dev: g *= grad_scale; coef = min(1, clip/(sqrt(*d_sqnorm)*grad_scale+1e-6));
+ *  g *= coef; Adam(lr,b1,b2,eps) with bias correction for step *d_step (1-based). */
 #define BIGRU_SQNORM_WS 528
 int  bigru_sqnorm(const float* d_g, int64_t n, float* d_out, float* d_ws, void* stream);
-int  bigru_clip_adam_step(float* d_params, float* d_grads, float* d_m, float* d_v, int64_t n,
-                          const float* d_sqnorm, float clip, float lr, float b1, float b2, float eps,
-                          int step, float grad_scale, void* stream);
-
-/* Device-resident step counter variant of the same update, for CUDA-graph capture of the train step (SURVEY.md 8(f) N5):
- *  bigru_adam_tick: *d_step += 1, *d_sqnorm = 0 (one tiny launch, before bigru_sqnorm);
- *  bigru_clip_adam_step_dev: as bigru_clip_adam_step with the bias corrections formed on the device from *d_step. */
 int  bigru_adam_tick(int* d_step, float* d_sqnorm, void* stream);
 int  bigru_clip_adam_step_dev(float* d_params, float* d_grads, float* d_m, float* d_v, int64_t n,
                               const float* d_sqnorm, float clip, float lr, float b1, float b2, float eps,
@@ -141,14 +135,6 @@ int  bigru_window_gather_norm(const float* d_src, const float* d_xmin, const flo
                               int64_t start, int64_t N, int B, int T, int F, float* d_out, void* stream);
 int  bigru_window_targets(const float* d_y, int64_t start, int64_t N, int B, int T, int C,
                           float* d_out, void* stream);
-
-/* --- SURVEY.md 8(f) N1, zero-copy windows: forward straight from the HBM-resident chunk src[N,F] - the batch
- *  x[b,t,:] = (src[start+b+t,:] - xmin) / (xmax - xmin) is formed inside the first kernel of the path and never
- *  materialised as fp32 [B,T,F] by the caller (sql_pytorch_dataloader.py:239-245 + biGRU_model.py:63).  Pair it with
- *  bigru_backward(..., d_x = NULL, ...): the backward then takes the layer-0 input from the stash. */
-int  bigru_forward_windows(const bigru_plan* plan, const float* d_params, const float* d_src, const float* d_xmin,
-                           const float* d_xmax, int64_t start, int64_t N, float dropout_p, int spatial, int training,
-                           uint64_t seed, void* d_stash, void* d_scratch, float* d_logits, float* d_hn, void* stream);
 
 /* --- SURVEY.md 8(f) N3, chunk statistics on the GPU: per-feature MIN / MAX over rows [row_lo, row_hi) of a
  *  table[N,F] (NaN = SQL NULL, ignored), i.e. the two aggregate queries of MySQLChunkLoader

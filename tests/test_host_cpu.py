@@ -56,6 +56,14 @@ def test_plan_bookkeeping_without_gpu(pkg):
     if not torch.cuda.is_available():
         assert lib.bigru_device_check(0) == pkg._lib.ERR_DEVICE      # fails loudly, no fallback
         assert b"no CPU fallback" in lib.bigru_last_error()
+        # the backward needs the input the forward read: a null d_x is refused before anything is launched (a call that got
+        # past the argument checks would fail here with ERR_CUDA at its first memset)
+        assert lib.bigru_plan_create(32, 4, 8, 128, 1, 3, 1, pkg._lib.PREC_BF16X3, C.byref(h)) == 0
+        dev = C.c_void_p(256)                                        # stands for a device pointer; never dereferenced
+        assert lib.bigru_backward(h, dev, None, None, 0.0, 0, 0, 0, dev, dev, dev, dev, None, None, None) == pkg._lib.ERR_ARG
+        assert lib.bigru_backward_layers(h, dev, None, None, 0.0, 0, 0, 0, dev, dev, dev, dev, None, None, 0, 0, None) == pkg._lib.ERR_ARG
+        assert b"null argument" in lib.bigru_last_error()
+        lib.bigru_plan_destroy(h)
 
 
 def test_model_surface_and_state_dict(pkg, golden_dir):
