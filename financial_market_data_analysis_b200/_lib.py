@@ -30,6 +30,7 @@ SIGNATURES = {
     "bigru_param_offset": (_i, [_vp, _i, _i, _i, C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_i64)]),
     "bigru_workspace_bytes": (_i, [_vp, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
     "bigru_stash_argmax_offset": (_i, [_vp, C.POINTER(C.c_size_t)]),
+    "bigru_stash_output_offset": (_i, [_vp, _i, C.POINTER(C.c_size_t)]),
     "bigru_forward": (_i, [_vp, _vp, _vp, _vp, _f, _i, _i, _u64, _vp, _vp, _vp, _vp, _vp]),
     "bigru_backward": (_i, [_vp, _vp, _vp, _vp, _f, _i, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_backward_layers": (_i, [_vp, _vp, _vp, _vp, _f, _i, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),

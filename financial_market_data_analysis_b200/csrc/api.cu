@@ -17,7 +17,7 @@ void bigru_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* bigru_last_error(void) { return g_err; }
-extern "C" int bigru_version(void) { return 201; }
+extern "C" int bigru_version(void) { return 202; }
 
 extern "C" int bigru_device_check(int dev) {
     int n = 0;
@@ -213,6 +213,13 @@ extern "C" int bigru_workspace_bytes(const bigru_plan* p, size_t* stash_bytes, s
 extern "C" int bigru_stash_argmax_offset(const bigru_plan* p, size_t* byte_offset) {
     if (!p || !byte_offset) { bigru_set_error("stash_argmax_offset: null argument"); return BIGRU_ERR_ARG; }
     *byte_offset = (size_t)stash_layout(*p).arg * sizeof(float);
+    return BIGRU_OK;
+}
+
+// where the forward keeps layer l's output Y[B][T][D*H] (fp32) inside the stash
+extern "C" int bigru_stash_output_offset(const bigru_plan* p, int layer, size_t* byte_offset) {
+    if (!p || !byte_offset || layer < 0 || layer >= p->L) { bigru_set_error("stash_output_offset: bad argument"); return BIGRU_ERR_ARG; }
+    *byte_offset = (size_t)stash_layout(*p).Y[layer] * sizeof(float);
     return BIGRU_OK;
 }
 

@@ -79,6 +79,9 @@ int  bigru_workspace_bytes(const bigru_plan* plan, size_t* stash_bytes, size_t* 
  * biGRU_model.py:125).  The max-pool's gradient routing is discontinuous where two time steps tie to within rounding;
  * parity tests read the routing that was actually taken (tests/test_gpu_parity.py). */
 int  bigru_stash_argmax_offset(const bigru_plan* plan, size_t* byte_offset);
+/* byte offset, inside the same stash, of layer `layer`'s fp32 output Y[B][T][D*H] (the nn.GRU output of that layer, direction
+ * d in columns [d*H, d*H+H)); lets tests compare every layer at every time step. */
+int  bigru_stash_output_offset(const bigru_plan* plan, int layer, size_t* byte_offset);
 
 /* --- BiGRU.forward (biGRU_model.py:63-138): dropout :87-94, nn.GRU :102, head :111-137.
  *  d_x[B,T,F]; d_h0 nullable [L*D,B,H] (the `hidden` argument); d_logits[B,C];

@@ -18,8 +18,8 @@ pytestmark = pytest.mark.gpu
 # fp32 path: logits <= 1e-4 rel (BASELINE.json north_star); gradients rel-L2 <= 1e-3 (SURVEY.md 8(d))
 # step: Adam divides by |g| so elements with |g| ~ eps flip freely; bound the element error by a
 # fraction of lr (1e-3) and the whole update by rel-L2
-# bf16 path: operands, the gate stash and dgi/dgh are bf16 (fp32 accumulate/state), so the error of BPTT grows
-# with T and L; bounds: per-tensor rel-L2 "grads", whole flat gradient "gflat"
+# bf16 path: only the GEMM and recurrence operands are bf16 (fp32 accumulate, state, gate stash, dgi/dgh), so the error
+# of BPTT grows with T and L; bounds: per-tensor rel-L2 "grads", whole flat gradient "gflat"
 # bf16x3 path ("fp32-class" on tensor cores: split bf16 operand pairs, fp32 accumulate / gate math / stash): the SAME bounds as
 # the fp32 path - it is the variant BASELINE.json configs[1] ("fp32 tolerance check") is measured on
 TOL = {"fp32": dict(logits=1e-4, grads=1e-3, gflat=1e-3, kat=1e-5, step=2e-4, update=2e-2),

@@ -224,3 +224,161 @@ def test_features_oracle_against_reference_sql(golden_dir):
     assert np.array_equal(np.isnan(f), np.isnan(z["features"]))
     np.testing.assert_allclose(np.nan_to_num(f), np.nan_to_num(z["features"]), rtol=1e-12, atol=1e-9)
     assert np.array_equal(t, z["targets"])
+
+
+# ---- rounding model of the tensor-core precisions (oracle/bigru_ref.c, prec / mask) ------------------------------------
+def _rand_case(B, T, F, H, L, C, D, use_h0, seed):
+    rng = np.random.default_rng(seed)
+    k = 1 / np.sqrt(H)                                       # torch.nn.GRU / nn.Linear initialisation scale
+    flat = rng.uniform(-k, k, oracle_c.lib().bigru_ref_param_count(F, H, L, C, D)).astype(np.float32)
+    x = rng.standard_normal((B, T, F)).astype(np.float32)
+    h0 = (rng.standard_normal((L * D, B, H)) * 0.5).astype(np.float32) if use_h0 else None
+    dl = rng.standard_normal((B, C)).astype(np.float32)
+    return flat, x, h0, dl
+
+
+def _model_run(case, dims, prec, mask=oracle_c.ALL_POINTS):
+    flat, x, h0, dl = case
+    H, L, C, D = dims
+    logits, hn, stash = oracle_c.forward(flat, x, H, L, C, D, h0, keep=True, prec=prec, mask=mask)
+    grads, dx, dh0 = oracle_c.backward(flat, x, stash, dl, H, L, C, D, prec=prec, mask=mask)
+    return dict(logits=logits, hn=hn, stash=stash, grads=grads, dx=dx, dh0=dh0)
+
+
+def test_exact_mode_is_the_pinned_oracle(golden_dir):
+    """The exact mode, through the old entry points and through the precision-aware ones, is bit for bit what the oracle
+    computed before the rounding modes existed (tests/golden/make_oracle_exact_golden.py)."""
+    z = np.load(os.path.join(golden_dir, "oracle_exact.npz"))
+    for name in ("a", "b"):
+        g = {k.split(":", 1)[1]: z[k] for k in z.files if k.startswith(name + ":")}
+        B, T, F, H, L, C, D = [int(v) for v in g["meta"]]
+        h0 = g.get("h0")
+        runs = [_model_run((g["flat"], g["x"], h0, g["dlogits"]), (H, L, C, D), oracle_c.EXACT)]
+        lib = oracle_c.lib()
+        p = oracle_c._p
+        logits, hn = np.zeros_like(g["logits"]), np.zeros_like(g["hn"])
+        stash = np.zeros_like(g["stash"])
+        assert lib.bigru_ref_forward(B, T, F, H, L, C, D, p(g["flat"]), p(g["x"]), p(h0), p(logits), p(hn), p(stash, oracle_c.C.c_double)) == 0
+        grads, dx, dh0 = np.zeros_like(g["grads"]), np.zeros_like(g["dx"]), np.zeros_like(g["dh0"])
+        assert lib.bigru_ref_backward(B, T, F, H, L, C, D, p(g["flat"]), p(g["x"]), p(stash, oracle_c.C.c_double), p(g["dlogits"]),
+                                      p(grads), p(dx), p(dh0)) == 0
+        runs.append(dict(logits=logits, hn=hn, stash=stash, grads=grads, dx=dx, dh0=dh0))
+        for r in runs:
+            for k in ("logits", "hn", "stash", "grads", "dx", "dh0"):
+                assert r[k].tobytes() == g[k].tobytes(), (name, k)
+
+
+def _rounded(v, prec):
+    """(hi + lo, hi, lo) of a float64 tensor as the kernels store a GEMM operand: fp32, then bf16 (lo = 0) or a bf16 pair."""
+    v32 = v.float()
+    hi = v32.bfloat16().float()
+    lo = (v32 - hi).bfloat16().float() if prec == oracle_c.BF16X3 else torch.zeros_like(hi)
+    return (hi.double() + lo.double()), hi.double(), lo.double()
+
+
+def _mm(a, b, prec):
+    """a [M,K] b[N,K]^T with both operands rounded: ah bh + ah bl + al bh."""
+    af, ah, al = _rounded(a, prec)
+    bf, bh, bl = _rounded(b, prec)
+    return ah @ bf.T + al @ bh.T
+
+
+def _torch_forward(flat, x, h0, H, L, C, D, prec):
+    """An independent float64 restatement of the rounding model's forward: per-layer outputs Y[B,T,D*H], cat and logits."""
+    flat = torch.from_numpy(flat).double()
+    inp = torch.from_numpy(x).double()
+    B, T, _ = inp.shape
+    off, ys = 0, []
+
+    def take(*shape):
+        nonlocal off
+        n = int(np.prod(shape))
+        off += n
+        return flat[off - n:off].reshape(shape)
+
+    for l in range(L):
+        I = inp.shape[2]
+        dirs = []
+        for d in range(D):
+            w_ih, w_hh, b_ih, b_hh = take(3 * H, I), take(3 * H, H), take(3 * H), take(3 * H)
+            gi = (_mm(inp.reshape(B * T, I), w_ih, prec) + b_ih).reshape(B, T, 3 * H)
+            h = torch.from_numpy(h0[l * D + d]).double() if h0 is not None else torch.zeros(B, H, dtype=torch.float64)
+            y = torch.zeros(B, T, H, dtype=torch.float64)
+            for s in range(T):
+                t = s if d == 0 else T - 1 - s
+                gh = _mm(h, w_hh, prec) + b_hh
+                r = torch.sigmoid(gi[:, t, :H] + gh[:, :H])
+                zg = torch.sigmoid(gi[:, t, H:2 * H] + gh[:, H:2 * H])
+                n = torch.tanh(gi[:, t, 2 * H:] + r * gh[:, 2 * H:])
+                h = (1 - zg) * n + zg * h
+                y[:, t] = h
+            dirs.append(y)
+        inp = torch.cat(dirs, 2)
+        ys.append(inp)
+    top = ys[-1]
+    s = top[..., :H] + top[..., H:] if D == 2 else top
+    last = top[:, T - 1, :H] + (top[:, 0, H:] if D == 2 else 0)
+    cat = torch.cat([last, s.max(1).values, s.sum(1) / T], 1)
+    lin_w, lin_b = take(C, 3 * H), take(C)
+    return [y.numpy() for y in ys], cat.numpy(), (_mm(cat, lin_w, prec) + lin_b).numpy()
+
+
+@pytest.mark.parametrize("prec", ["bf16", "bf16x3"])
+@pytest.mark.parametrize("shape", [(3, 4, 5, 8, 2, 3, 2, True), (2, 5, 9, 16, 1, 2, 1, False)])
+def test_rounding_model_forward_matches_torch_restatement(prec, shape):
+    B, T, F, H, L, C, D, use_h0 = shape
+    flat, x, h0, _ = _rand_case(*shape, seed=7)
+    p = oracle_c.PRECISION[prec]
+    logits, _, stash = oracle_c.forward(flat, x, H, L, C, D, h0, keep=True, prec=p)
+    ys, cat, want_logits = _torch_forward(flat, x, h0, H, L, C, D, p)
+    for y, want in zip(oracle_c.layer_outputs(stash, B, T, H, L, D), ys):
+        assert np.abs(y - want).max() <= 1e-12 * np.abs(want).max()
+    got_cat = stash[-4 * B * H:-B * H].reshape(B, 3 * H)
+    assert np.abs(got_cat - cat).max() <= 1e-12 * np.abs(cat).max()
+    want32 = want_logits.astype(np.float32)
+    assert np.all(np.abs(logits - want32) <= np.spacing(np.abs(want32))), (logits, want32)
+    # and the rounding is really there: the exact forward is far from it
+    exact = oracle_c.forward(flat, x, H, L, C, D, h0)[0]
+    assert np.abs(exact - want32).max() > 20 * np.spacing(np.abs(want32)).max()
+
+
+FORWARD_POINTS = {"proj_x", "proj_w", "rec_h", "rec_w", "head_cat", "head_w", "rec_h0"}
+
+
+@pytest.mark.parametrize("prec", ["bf16", "bf16x3"])
+def test_every_rounding_point_is_wired(prec):
+    """Leaving one rounding point exact must change the result, and only where that point acts: a forward point moves the
+    logits, a backward point leaves the forward alone and moves the gradients."""
+    B, T, F, H, L, C, D = 3, 4, 5, 8, 2, 3, 2
+    case = _rand_case(B, T, F, H, L, C, D, True, seed=3)
+    p = oracle_c.PRECISION[prec]
+    full = _model_run(case, (H, L, C, D), p)
+    for point in oracle_c.ROUNDING_POINTS:
+        r = _model_run(case, (H, L, C, D), p, oracle_c.without(point))
+        moved = {k for k in full if not np.array_equal(full[k], r[k])}
+        if point in FORWARD_POINTS:
+            assert "logits" in moved, (point, moved)
+        else:
+            assert moved and moved <= {"grads", "dx", "dh0"}, (point, moved)
+
+
+def test_rounding_model_distance_from_exact():
+    """The model's own error: about 1e-3 rel-L2 on the forward at bf16 and a few 1e-6 at bf16x3 (three of the four bf16
+    products of the split operands).  The gradients pass through twice as many rounded products and sit near 1e-2 at bf16."""
+    B, T, F, H, L, C, D = 8, 16, 16, 64, 2, 3, 2
+    case = _rand_case(B, T, F, H, L, C, D, True, seed=5)
+    exact = _model_run(case, (H, L, C, D), oracle_c.EXACT)
+
+    def dist(r):
+        y = [oracle_c.layer_outputs(s["stash"], B, T, H, L, D)[-1] for s in (r, exact)]
+        return {k: np.linalg.norm(a - b) / np.linalg.norm(b)
+                for k, (a, b) in dict(y=y, logits=(r["logits"], exact["logits"]), grads=(r["grads"], exact["grads"]),
+                                      dx=(r["dx"], exact["dx"]), dh0=(r["dh0"], exact["dh0"])).items()}
+
+    d16 = dist(_model_run(case, (H, L, C, D), oracle_c.BF16))
+    d3 = dist(_model_run(case, (H, L, C, D), oracle_c.BF16X3))
+    print("bf16", d16, "bf16x3", d3)
+    assert 5e-4 < d16["y"] < 5e-3 and 5e-4 < d16["logits"] < 5e-3, d16
+    assert all(5e-4 < v < 5e-2 for v in d16.values()), d16
+    assert all(5e-7 < v < 2e-5 for v in d3.values()), d3
+    assert all(d3[k] < 1e-2 * d16[k] for k in d16), (d16, d3)
