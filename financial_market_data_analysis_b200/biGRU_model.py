@@ -42,18 +42,137 @@ def _stream_ptr(device=None):
     return torch.cuda.current_stream(device).cuda_stream
 
 
-def _pad_batch(x, h0, Bp):
-    """x [B, T, F] and h0 [L*D, B, H] (or None) with zero rows appended up to batch Bp (BiGRU._padded_batch)."""
-    B = x.shape[0]
-    if Bp == B:
-        return x, h0
-    xp = x.new_zeros((Bp,) + tuple(x.shape[1:]))
-    xp[:B] = x
-    if h0 is not None:
-        hp = h0.new_zeros(h0.shape[0], Bp, h0.shape[2])
-        hp[:, :B] = h0
-        h0 = hp
-    return xp, h0
+class _Padding:
+    """What the C plans of one model run at, and the zero padding between the model's own shapes and the plan's.
+
+    The tensor-core kernels exist for whole batch tiles (32 rows at "bf16x3" and at "bf16" with 512 hidden units, 16 rows
+    otherwise at "bf16") and for 128 / 256 (/ 512 at "bf16") hidden units.  Other batch sizes run with zero rows appended:
+    batch rows are independent and the padded rows receive a zero upstream gradient.  Smaller hidden sizes run with zero
+    units appended (see BiGRU.plan_hidden).  Logits, loss and every gradient of the real rows and parameters are those of
+    the unpadded model (up to summation order)."""
+
+    def __init__(self, model, device):
+        H = model.hidden_size
+        prec = model.precision if model.precision != "auto" else ("bf16x3" if H <= 256 else "fp32")
+        sizes = {"bf16x3": (128, 256), "bf16": (128, 256, 512)}.get(prec, ())
+        self.precision = prec
+        self.hidden = next((hp for hp in sizes if H <= hp), H)
+        self.tile = 32 if (prec == "bf16x3" or (prec == "bf16" and self.hidden == 512)) else (16 if prec == "bf16" else 1)
+        self.padded = self.hidden != H
+        self._dims = (H, model.n_directions, model.n_layers, model.n_features, model.output_size)
+        self._device = device
+        self._index = None
+
+    def batch(self, B: int) -> int:
+        """The batch size a plan runs for B real rows."""
+        return (B + self.tile - 1) // self.tile * self.tile
+
+    def pad(self, t, Bp, dim=0, units=False):
+        """t with zero rows appended along `dim` up to Bp and, when `units`, zero hidden units up to the plan's (last dim)."""
+        if t is None:
+            return None
+        shape = list(t.shape)
+        shape[dim] = Bp
+        if units:
+            shape[-1] = self.hidden
+        if list(t.shape) == shape:
+            return t
+        out = t.new_zeros(shape)
+        out[tuple(slice(0, n) for n in t.shape)] = t
+        return out
+
+    def crop(self, t, B, dim=0, units=False):
+        """The first B rows along `dim` of a plan-sized tensor and, when `units`, its real hidden units."""
+        if t is None:
+            return None
+        if units and t.shape[-1] != self._dims[0]:
+            t = t[..., :self._dims[0]]
+        return t if t.shape[dim] == B else t.narrow(dim, 0, B)
+
+    def _map(self):
+        """(index tensor, padded parameter count): position of every real parameter inside the padded plan's flat vector."""
+        if self._index is None:
+            H, D, L, F, C = self._dims
+            Hp = self.hidden
+            idx, off_p = [], 0
+
+            def rows(n_cols_pad, col_map):
+                # a [3H][cols] block -> padded [3Hp][cols_pad]: row g*H + j -> g*Hp + j, column through col_map
+                r = (np.arange(3)[:, None] * Hp + np.arange(H)[None, :]).reshape(-1)
+                return (r[:, None] * n_cols_pad + col_map[None, :]).reshape(-1)
+
+            for l in range(L):
+                Ip = F if l == 0 else D * Hp
+                cm = np.arange(F) if l == 0 else (np.arange(D)[:, None] * Hp + np.arange(H)[None, :]).reshape(-1)
+                for d in range(D):
+                    idx.append(off_p + rows(Ip, cm)); off_p += 3 * Hp * Ip                         # W_ih
+                    idx.append(off_p + rows(Hp, np.arange(H))); off_p += 3 * Hp * Hp               # W_hh
+                    b = (np.arange(3)[:, None] * Hp + np.arange(H)[None, :]).reshape(-1)
+                    idx.append(off_p + b); off_p += 3 * Hp                                        # b_ih
+                    idx.append(off_p + b); off_p += 3 * Hp                                        # b_hh
+            cmh = (np.arange(3)[:, None] * Hp + np.arange(H)[None, :]).reshape(-1)                # head: last | max | avg, H wide each
+            idx.append(off_p + (np.arange(C)[:, None] * 3 * Hp + cmh[None, :]).reshape(-1)); off_p += C * 3 * Hp
+            idx.append(off_p + np.arange(C)); off_p += C
+            self._index = (torch.from_numpy(np.concatenate(idx).astype(np.int64)).to(self._device), off_p)
+        return self._index
+
+    def params(self, flat, out=None):
+        """The flat parameter vector as the plan sees it: `flat` itself, or its entries scattered into a zero-padded vector
+        (`out` when given; its padded entries must be zero)."""
+        if not self.padded:
+            return flat
+        index, n = self._map()
+        assert index.numel() == flat.numel()
+        if out is None:
+            out = flat.new_zeros(n)
+        return out.index_copy_(0, index, flat.detach())
+
+    def grads(self, pgrad, out=None):
+        """The real parameters' entries of a plan-sized gradient vector (into `out` when given)."""
+        if not self.padded:
+            return pgrad
+        return torch.index_select(pgrad, 0, self._map()[0], out=out) if out is not None else torch.index_select(pgrad, 0, self._map()[0])
+
+
+class _AdamState:
+    """Optimiser state of the fused step.  The flat gradient and the scalar loss share one buffer (``gext`` = P gradients + 1
+    loss), so that data parallelism needs exactly one all-reduce per step.  Adam's step count lives on the device too
+    (``dstep``), so that a captured CUDA graph of the step stays valid from one step to the next; ``step`` counts on the host."""
+
+    def __init__(self, flat, pad):
+        P, dev = flat.numel(), flat.device
+        self.gext = torch.empty(P + 1, device=dev, dtype=torch.float32)
+        self.grad, self.loss = self.gext[:P], self.gext[P:P + 1]
+        self.m, self.v = torch.zeros_like(flat), torch.zeros_like(flat)
+        self.step, self.dstep = 0, torch.zeros(1, device=dev, dtype=torch.int32)
+        self.scal = torch.zeros(2, device=dev, dtype=torch.float32)
+        self.sqws = torch.empty(_lib.SQNORM_WS, device=dev, dtype=torch.float32)
+        # the plan's own parameter / gradient vectors: zero-padded ones when the plan pads hidden units, else the flat ones
+        self.pflat = pad.params(flat)
+        self.pgrad = torch.empty_like(self.pflat) if pad.padded else self.grad
+        self.mirror_steps = []           # optimizer.state[p]["step"] tensors, kept equal to `step`
+
+    def __getitem__(self, name):
+        """Read access by name (``st["grad"]``) for callers that index the state like a dict."""
+        return getattr(self, name)
+
+    def advance(self):
+        """Host-side bookkeeping of one executed step (the device counter advances inside bigru_adam_tick)."""
+        self.step += 1
+        if self.mirror_steps:
+            torch._foreach_add_(self.mirror_steps, 1.0)
+
+
+class _StepBuffers:
+    """What one fused train step reads and writes: the plan and a stash of its pool, the padded inputs, the targets of the
+    real rows, the loss arguments, logits / dlogits of the padded batch and the dropout arguments of the C calls."""
+
+    def __init__(self, plan, x, h0, tgt, loss, C, drop):
+        Bp = x.shape[0]
+        self.plan, self.stash, self.x, self.h0, self.tgt, self.loss, self.drop = plan, plan.acquire_stash(), x, h0, tgt, loss, drop
+        self.logits = torch.empty(Bp, C, device=x.device, dtype=torch.float32)
+        # the loss writes dlogits of the real rows only: the padded rows stay zero
+        self.dlogits = (torch.zeros if Bp != tgt.shape[0] else torch.empty)(Bp, C, device=x.device, dtype=torch.float32)
 
 
 class _GRUWeights(nn.Module):
@@ -125,62 +244,42 @@ class _BiGRUFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, model, x, h0, *params):
         lib = _lib.load()
+        pad = model._pad
         B = x.shape[0]
         Bp = model._padded_batch(B)
-        x, h0 = _pad_batch(x, h0, Bp)
+        x, h0 = pad.pad(x, Bp), pad.pad(h0, Bp, dim=1, units=True)
         plan = model._plan_for(x)
-        ctx.dev_guard = torch.cuda.device(x.device)      # the C ABI launches on the CURRENT device: make it the model's
-        ctx.dev_guard.__enter__()
-        try:
-            out = _BiGRUFunction._forward(ctx, lib, plan, model, x, h0, Bp)
-            ctx.real_batch = B
-            model._last_batch = B
-            if Bp != B:
-                model._last_hidden = model._last_hidden[:, :B]
-                out = out[:B]
-            return out
-        finally:
-            ctx.dev_guard.__exit__(None, None, None)
-
-    @staticmethod
-    def _forward(ctx, lib, plan, model, x, h0, B):
-        Hp = model.plan_hidden(B)
-        pflat = model._plan_params()                     # zero-padded hidden units scattered in when Hp > hidden_size
-        h0 = model._pad_last(h0, Hp)
-        logits = torch.empty(B, model.output_size, device=x.device, dtype=torch.float32)
-        hn = torch.empty(model.n_layers * model.n_directions, B, Hp, device=x.device, dtype=torch.float32)
-        need_grad = any(ctx.needs_input_grad)        # grad mode is off inside Function.forward; ask the ctx
-        stash = plan.acquire_stash()
-        training = bool(model.training and model.dropout_p > 0)
-        seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if training else 0
-        model._last_seed = seed                       # the dropout masks are a pure function of (seed, element index)
-        _lib.check(lib.bigru_forward(plan.handle, _lib.ptr(pflat), _lib.ptr(x), _lib.ptr(h0),
-                                     float(model.dropout_p), int(bool(model.spatial_dropout)), int(training), seed,
-                                     _lib.ptr(stash), _lib.ptr(plan.scratch), _lib.ptr(logits), _lib.ptr(hn),
-                                     _stream_ptr(x.device)), "bigru_forward")
-        model._last_hidden = hn if Hp == model.hidden_size else hn[..., :model.hidden_size]
-        ctx.pflat = pflat if need_grad else None
-        model._last_plan_stash = (plan, stash)
-        if need_grad:
-            ctx.model, ctx.plan, ctx.stash, ctx.seed, ctx.training = model, plan, stash, seed, training
-            ctx.save_for_backward(x, h0 if h0 is not None else torch.empty(0, device=x.device))
-            ctx.has_h0 = h0 is not None
-        else:
-            plan.release_stash(stash)
-        return logits
+        with torch.cuda.device(x.device):                 # the C ABI launches on the CURRENT device: make it the model's
+            pflat = model._plan_params()
+            logits = torch.empty(Bp, model.output_size, device=x.device, dtype=torch.float32)
+            hn = torch.empty(model.n_layers * model.n_directions, Bp, pad.hidden, device=x.device, dtype=torch.float32)
+            need_grad = any(ctx.needs_input_grad)        # grad mode is off inside Function.forward; ask the ctx
+            stash = plan.acquire_stash()
+            training = bool(model.training and model.dropout_p > 0)
+            seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if training else 0
+            model._last_seed = seed                       # the dropout masks are a pure function of (seed, element index)
+            _lib.check(lib.bigru_forward(plan.handle, _lib.ptr(pflat), _lib.ptr(x), _lib.ptr(h0),
+                                         float(model.dropout_p), int(bool(model.spatial_dropout)), int(training), seed,
+                                         _lib.ptr(stash), _lib.ptr(plan.scratch), _lib.ptr(logits), _lib.ptr(hn),
+                                         _stream_ptr(x.device)), "bigru_forward")
+            model._last_hidden = pad.crop(hn, B, dim=1, units=True)
+            model._last_forward = (plan, stash, B)
+            if need_grad:
+                ctx.model, ctx.pad, ctx.plan, ctx.stash, ctx.seed, ctx.training = model, pad, plan, stash, seed, training
+                ctx.pflat, ctx.real_batch, ctx.has_h0 = pflat, B, h0 is not None
+                ctx.save_for_backward(x, h0 if h0 is not None else torch.empty(0, device=x.device))
+            else:
+                plan.release_stash(stash)
+            return pad.crop(logits, B)
 
     @staticmethod
     def backward(ctx, dlogits):
         lib = _lib.load()
-        model, plan = ctx.model, ctx.plan
+        model, pad, plan = ctx.model, ctx.pad, ctx.plan
         x, h0 = ctx.saved_tensors
         h0 = h0 if ctx.has_h0 else None
-        dlogits = dlogits.contiguous().float()
-        B, Bp = ctx.real_batch, x.shape[0]
-        if Bp != B:                                       # padded rows: zero upstream gradient
-            dl = dlogits.new_zeros(Bp, dlogits.shape[1])
-            dl[:B] = dlogits
-            dlogits = dl
+        B = ctx.real_batch
+        dlogits = pad.pad(dlogits.contiguous().float(), x.shape[0])       # padded rows: zero upstream gradient
         grads = torch.empty_like(ctx.pflat)
         dx = torch.empty_like(x) if ctx.needs_input_grad[1] else None
         dh0 = torch.empty_like(h0) if (h0 is not None and ctx.needs_input_grad[2]) else None
@@ -190,16 +289,10 @@ class _BiGRUFunction(torch.autograd.Function):
                                           ctx.seed, _lib.ptr(ctx.stash), _lib.ptr(plan.scratch), _lib.ptr(dlogits),
                                           _lib.ptr(grads), _lib.ptr(dx), _lib.ptr(dh0), _stream_ptr(x.device)), "bigru_backward")
         plan.release_stash(ctx.stash)
-        ctx.stash = None
-        if Bp != B:
-            dx = dx[:B] if dx is not None else None
-            dh0 = dh0[:, :B] if dh0 is not None else None
+        ctx.stash = ctx.pflat = None
         grads = model._plan_grads(grads)                  # drop the padded hidden units' entries
-        if dh0 is not None and dh0.shape[-1] != model.hidden_size:
-            dh0 = dh0[..., :model.hidden_size]
-        ctx.pflat = None
         pg = tuple(grads[o:o + n].view(shape) for (o, n, shape) in model._views)
-        return (None, dx, dh0) + pg
+        return (None, pad.crop(dx, B), pad.crop(dh0, B, dim=1, units=True)) + pg
 
 
 class BiGRU(nn.Module):
@@ -247,11 +340,11 @@ class BiGRU(nn.Module):
         self._flat = None            # all parameters, one contiguous fp32 vector (C-ABI order)
         self._views = []             # (offset, numel, shape) per parameter in C-ABI order
         self._plans = {}
-        self._adam = None            # fused-step optimiser state (flat m, v, step)
+        self._adam = None            # fused-step optimiser state (_AdamState)
         self._dp_group = None
         self._dp_world = 1
         self._last_hidden = None
-        self._last_plan_stash = None
+        self._last_forward = None    # (plan, stash, real batch) of the last forward
         self._last_seed = 0
         self._graphs = {}
         self.use_cuda_graph = os.environ.get("BIGRU_B200_CUDA_GRAPH", "1") != "0"
@@ -286,14 +379,15 @@ class BiGRU(nn.Module):
                 off += n
         old = getattr(self, "_adam", None)
         self._flat, self._views = flat, views
+        self._pad = _Padding(self, dev)
         self._plans = {}
         self._graphs = {}
         self._adam = None
-        if old is not None and old["m"].numel() == total:        # keep the Adam moments across a re-flatten (.to() / .cuda())
-            st = self._fused_state(dev)
-            st["m"].copy_(old["m"].to(dev)); st["v"].copy_(old["v"].to(dev))
-            st["step"] = old["step"]
-            st["dstep"].fill_(old["step"])
+        if old is not None and old.m.numel() == total:          # keep the Adam moments across a re-flatten (.to() / .cuda())
+            st = self._fused_state()
+            st.m.copy_(old.m.to(dev)); st.v.copy_(old.v.to(dev))
+            st.step = old.step
+            st.dstep.fill_(old.step)
             self._mirror_optimizer_state()
 
     def _is_flat(self):
@@ -319,89 +413,26 @@ class BiGRU(nn.Module):
     # ------------------------------------------------------------------ plans
     def resolved_precision(self, batch: int = 0) -> str:
         """The precision a batch runs at ("auto": the fp32-class tensor-core path wherever it applies, i.e. hidden_size <= 256)."""
-        if self.precision != "auto":
-            return self.precision
-        return "bf16x3" if self.hidden_size <= 256 else "fp32"
+        return self._pad.precision
 
     def plan_hidden(self, batch: int = 0) -> int:
         """Hidden size of the C plan.  The tensor-core kernels exist for 128 / 256 (/ 512 at "bf16") hidden units; smaller models run
         ZERO-PADDED to the next of these: a padded unit has zero weights and biases, so r = z = 1/2, n = 0 and its state stays 0
         from h0 = 0 on; it feeds zero columns of W_hh / W_ih / the head.  Logits, loss and the gradients of the real parameters are
         exactly those of the unpadded model (up to summation order); the padded gradient entries are dropped."""
-        prec, H = self.resolved_precision(batch), self.hidden_size
-        sizes = {"bf16x3": (128, 256), "bf16": (128, 256, 512)}.get(prec, ())
-        for hp in sizes:
-            if H <= hp:
-                return hp
-        return H
-
-    def _pad_map(self, dev):
-        """(index tensor, padded parameter count): position of every real parameter inside the padded plan's flat vector."""
-        Hp, H = self.plan_hidden(), self.hidden_size
-        if Hp == H:
-            return None
-        key = (Hp, dev.index)
-        hit = getattr(self, "_pad_cache", None)
-        if hit is not None and hit[0] == key:
-            return hit[1]
-        D, L, F, C = self.n_directions, self.n_layers, self.n_features, self.output_size
-        idx, off_p = [], 0
-
-        def rows(n_cols_small, n_cols_pad, col_map):
-            # a [3H][cols] block -> padded [3Hp][cols_pad]: row g*H + j -> g*Hp + j, column through col_map
-            r = (np.arange(3)[:, None] * Hp + np.arange(H)[None, :]).reshape(-1)
-            return (r[:, None] * n_cols_pad + col_map[None, :]).reshape(-1)
-
-        for l in range(L):
-            I, Ip = (F, F) if l == 0 else (D * H, D * Hp)
-            cm = np.arange(F) if l == 0 else (np.arange(D)[:, None] * Hp + np.arange(H)[None, :]).reshape(-1)
-            for d in range(D):
-                idx.append(off_p + rows(I, Ip, cm)); off_p += 3 * Hp * Ip                     # W_ih
-                idx.append(off_p + rows(H, Hp, np.arange(H))); off_p += 3 * Hp * Hp           # W_hh
-                b = (np.arange(3)[:, None] * Hp + np.arange(H)[None, :]).reshape(-1)
-                idx.append(off_p + b); off_p += 3 * Hp                                        # b_ih
-                idx.append(off_p + b); off_p += 3 * Hp                                        # b_hh
-        cmh = (np.arange(3)[:, None] * Hp + np.arange(H)[None, :]).reshape(-1)                # head: last | max | avg, H wide each
-        idx.append(off_p + (np.arange(C)[:, None] * 3 * Hp + cmh[None, :]).reshape(-1)); off_p += C * 3 * Hp
-        idx.append(off_p + np.arange(C)); off_p += C
-        index = torch.from_numpy(np.concatenate(idx).astype(np.int64)).to(dev)
-        assert index.numel() == self._flat.numel()
-        self._pad_cache = (key, (index, off_p))
-        return self._pad_cache[1]
-
-    def _plan_params(self, buf=None):
-        """The flat parameter vector as the C plan sees it (zero-padded hidden units scattered in when plan_hidden() > hidden_size)."""
-        pm = self._pad_map(self._flat.device)
-        if pm is None:
-            return self._flat
-        index, P = pm
-        if buf is None:
-            buf = torch.zeros(P, device=self._flat.device, dtype=torch.float32)
-        buf.index_copy_(0, index, self._flat.detach())
-        return buf
-
-    def _plan_grads(self, pgrad, out=None):
-        pm = self._pad_map(self._flat.device)
-        if pm is None:
-            return pgrad
-        return torch.index_select(pgrad, 0, pm[0], out=out) if out is not None else torch.index_select(pgrad, 0, pm[0])
-
-    @staticmethod
-    def _pad_last(t, Hp):
-        """[.., .., H] -> [.., .., Hp] with zeros (initial hidden states)."""
-        if t is None or t.shape[-1] == Hp:
-            return t
-        out = t.new_zeros(tuple(t.shape[:-1]) + (Hp,))
-        out[..., :t.shape[-1]] = t
-        return out
+        return self._pad.hidden
 
     def _padded_batch(self, batch: int) -> int:
-        """The tensor-core paths work on whole batch tiles (32 rows at bf16x3, 16 at bf16): other batch sizes run zero-padded
-        to the next multiple.  Batch rows are independent and the padded rows receive a zero upstream gradient, so logits,
-        loss and every gradient of the real rows are unchanged."""
-        prec = self.resolved_precision(batch)
-        mult = 32 if (prec == "bf16x3" or (prec == "bf16" and self.plan_hidden(batch) == 512)) else (16 if prec == "bf16" else 1)
-        return (batch + mult - 1) // mult * mult
+        """The batch size a plan runs for `batch` real rows (whole batch tiles on the tensor-core paths, _Padding)."""
+        return self._pad.batch(batch)
+
+    def _plan_params(self, out=None):
+        """The flat parameter vector as the C plan sees it (zero-padded hidden units scattered in when plan_hidden() > hidden_size)."""
+        return self._pad.params(self._flat, out)
+
+    def _plan_grads(self, pgrad, out=None):
+        """The real parameters' entries of a plan-sized gradient vector."""
+        return self._pad.grads(pgrad, out)
 
     def _plan_for(self, x) -> _Plan:
         key = (int(x.shape[0]), int(x.shape[1]), self.resolved_precision(int(x.shape[0])), x.device.index)
@@ -432,12 +463,12 @@ class BiGRU(nn.Module):
     def pooled_argmax(self) -> torch.Tensor:
         """argmax_t of the max-pooled direction sum [batch, hidden] as taken by the last ``forward`` (the routing of the
         max-pool gradient, biGRU_model.py:125).  Valid until the next forward of the same shape."""
-        plan, stash = self._last_plan_stash
+        plan, stash, B = self._last_forward
         off = _lib.C.c_size_t()
         _lib.check(_lib.load().bigru_stash_argmax_offset(plan.handle, _lib.C.byref(off)), "bigru_stash_argmax_offset")
-        Hp = self.plan_hidden(plan.B)
-        n = plan.B * Hp * 4
-        return stash[off.value:off.value + n].view(torch.int32).view(plan.B, Hp)[:getattr(self, "_last_batch", plan.B), :self.hidden_size].clone()
+        Hp = self._pad.hidden
+        arg = stash[off.value:off.value + plan.B * Hp * 4].view(torch.int32).view(plan.B, Hp)
+        return self._pad.crop(arg, B, units=True).clone()
 
     # ------------------------------------------------------------------ reference surface
     def forward(self, input_seq, hidden=None):
@@ -513,33 +544,12 @@ class BiGRU(nn.Module):
             hit = self._loss_cache[key] = v.contiguous()
         return hit
 
-    def _fused_state(self, dev):
-        """Optimiser state of the fused step.  The flat gradient and the scalar loss share one buffer (``gext`` = P gradients
-        + 1 loss), so that data parallelism needs exactly one all-reduce per step.  ``step`` lives on the device too
-        (``dstep``), so that a captured CUDA graph of the step stays valid from one step to the next."""
-        st = self._adam
-        if st is None:
-            P = self._flat.numel()
-            gext = torch.empty(P + 1, device=dev, dtype=torch.float32)
-            st = self._adam = {"m": torch.zeros_like(self._flat), "v": torch.zeros_like(self._flat), "step": 0,
-                               "dstep": torch.zeros(1, device=dev, dtype=torch.int32),
-                               "gext": gext, "grad": gext[:P], "loss": gext[P:P + 1],
-                               "scal": torch.zeros(2, device=dev, dtype=torch.float32),
-                               "sqws": torch.empty(_lib.SQNORM_WS, device=dev, dtype=torch.float32)}
-            pm = self._pad_map(dev)
-            if pm is not None:                                # zero-padded hidden units (plan_hidden): the plan's own parameter / gradient vectors
-                st["pflat"] = torch.zeros(pm[1], device=dev, dtype=torch.float32)
-                st["pgrad"] = torch.empty(pm[1], device=dev, dtype=torch.float32)
-            self._import_optimizer_state(st)
+    def _fused_state(self):
+        if self._adam is None:
+            self._adam = _AdamState(self._flat, self._pad)
+            self._import_optimizer_state(self._adam)
             self._mirror_optimizer_state()
-        return st
-
-    @staticmethod
-    def _bump_step(st, k):
-        st["step"] += k
-        ms = st.get("mirror_steps")
-        if ms:
-            torch._foreach_add_(ms, float(k))
+        return self._adam
 
     def _import_optimizer_state(self, st):
         """Moments the user's torch.optim.Adam already holds (generic steps taken before, or a loaded optimizer.state_dict())
@@ -558,10 +568,10 @@ class BiGRU(nn.Module):
         with torch.no_grad():
             for p, (off, n, _) in zip(self._ordered_params(), self._views):
                 ps = opt.state[p]
-                st["m"][off:off + n].copy_(ps["exp_avg"].reshape(-1).to(st["m"].device))
-                st["v"][off:off + n].copy_(ps["exp_avg_sq"].reshape(-1).to(st["v"].device))
-        st["step"] = steps[0]
-        st["dstep"].fill_(steps[0])
+                st.m[off:off + n].copy_(ps["exp_avg"].reshape(-1).to(st.m.device))
+                st.v[off:off + n].copy_(ps["exp_avg_sq"].reshape(-1).to(st.v.device))
+        st.step = steps[0]
+        st.dstep.fill_(steps[0])
 
     def _mirror_optimizer_state(self):
         """optimizer.state[p] = views of the flat moments + a step tensor, in torch.optim.Adam's own format: optimizer.state_dict()
@@ -570,131 +580,72 @@ class BiGRU(nn.Module):
         if opt is None or st is None or self._adam_spec() is None:
             return
         for p, (off, n, shape) in zip(self._ordered_params(), self._views):
-            opt.state[p] = {"step": torch.tensor(float(st["step"])), "exp_avg": st["m"][off:off + n].view(shape),
-                            "exp_avg_sq": st["v"][off:off + n].view(shape)}
-        st["mirror_steps"] = [opt.state[p]["step"] for p in self._ordered_params()]
+            opt.state[p] = {"step": torch.tensor(float(st.step)), "exp_avg": st.m[off:off + n].view(shape),
+                            "exp_avg_sq": st.v[off:off + n].view(shape)}
+        st.mirror_steps = [opt.state[p]["step"] for p in self._ordered_params()]
 
-    def _launch_fwd_loss_bwd(self, lib, plan, x, h0, tgt, kind, wv, pwv, denom, logits, dlogits, stash, args, st, s, part="all"):
-        """part = "all": forward, loss, backward.  Data parallelism splits the backward so that the all-reduce of the upper layers'
-        gradients overlaps the lowest layer's backward: "upper" = forward + loss + layers L-1 .. 1 (+ head), "lower" = layer 0."""
-        # the loss sees the REAL batch rows (tgt's); logits / dlogits may carry zero-padded rows behind them (whole batch tiles)
-        B, C = tgt.shape[0], logits.shape[1]
-        padded = "pflat" in st
-        pflat = (self._plan_params(st["pflat"]) if part != "lower" else st["pflat"]) if padded else self._flat
-        pgrad = st["pgrad"] if padded else st["grad"]
-        if part != "lower":
-            _lib.check(lib.bigru_forward(plan.handle, _lib.ptr(pflat), _lib.ptr(x), _lib.ptr(h0), *args,
-                                         _lib.ptr(stash), _lib.ptr(plan.scratch), _lib.ptr(logits), None, s), "bigru_forward")
-            _lib.check(lib.bigru_loss(kind, _lib.ptr(logits), _lib.ptr(tgt), _lib.ptr(wv), _lib.ptr(pwv), B, C, denom,
-                                      _lib.ptr(st["loss"]), _lib.ptr(dlogits), s), "bigru_loss")
-        if part == "all":
-            _lib.check(lib.bigru_backward(plan.handle, _lib.ptr(pflat), _lib.ptr(x), _lib.ptr(h0), *args,
-                                          _lib.ptr(stash), _lib.ptr(plan.scratch), _lib.ptr(dlogits), _lib.ptr(pgrad),
-                                          None, None, s), "bigru_backward")
-        else:
-            lo_hi = (self.n_layers - 1, 1) if part == "upper" else (0, 0)
-            _lib.check(lib.bigru_backward_layers(plan.handle, _lib.ptr(pflat), _lib.ptr(x), _lib.ptr(h0), *args,
-                                                 _lib.ptr(stash), _lib.ptr(plan.scratch), _lib.ptr(dlogits), _lib.ptr(pgrad),
-                                                 None, None, lo_hi[0], lo_hi[1], s), "bigru_backward_layers")
-        if padded and part != "upper":
-            self._plan_grads(pgrad, out=st["grad"])
-
-    def _dp_split(self, st) -> int:
-        """Offset (in the flat gradient) where the upper layers' parameters start, or 0 when the data-parallel step is not split:
-        needs more than one layer, a tensor-core plan (bigru_backward_layers) and no hidden-size padding (the padded plan's
-        gradients are gathered only after the whole backward)."""
-        if self._dp_world <= 1 or self.n_layers < 2 or "pflat" in st or self.resolved_precision() == "fp32":
-            return 0
-        if os.environ.get("BIGRU_B200_DP_OVERLAP", "0") != "1":      # opt-in: two collectives per step instead of one
-            return 0
-        per_dir0 = 3 * self.hidden_size * (self.n_features + self.hidden_size + 2)
-        return self.n_directions * per_dir0
-
-    def _dp_allreduce_overlapped(self, st, split, dev, lower):
-        """All-reduce of [split, P] + loss on a side stream (issued after the upper layers' backward), `lower()` = the lowest
-        layer's backward on the main stream meanwhile, then the all-reduce of [0, split) and the join."""
-        main = torch.cuda.current_stream(dev)
-        side = st.get("side")
-        if side is None:
-            side = st["side"] = torch.cuda.Stream(device=dev)
-        side.wait_stream(main)
-        with torch.cuda.stream(side):
-            allreduce_flat_(st["gext"][split:], self._dp_group)          # upper layers + head + the loss (last element)
-        lower()
-        allreduce_flat_(st["gext"][:split], self._dp_group)
-        main.wait_stream(side)
-
-    def _launch_update(self, lib, g, st, s):
-        """clip_grad_norm_(clip) + Adam on the flat buffers; the step counter is incremented on the device."""
-        sq = st["scal"][1:2]
-        _lib.check(lib.bigru_adam_tick(_lib.ptr(st["dstep"]), _lib.ptr(sq), s), "bigru_adam_tick")
-        _lib.check(lib.bigru_sqnorm(_lib.ptr(st["grad"]), st["grad"].numel(), _lib.ptr(sq), _lib.ptr(st["sqws"]), s), "bigru_sqnorm")
-        b1, b2 = g["betas"]
-        _lib.check(lib.bigru_clip_adam_step_dev(_lib.ptr(self._flat), _lib.ptr(st["grad"]), _lib.ptr(st["m"]),
-                                                _lib.ptr(st["v"]), self._flat.numel(), _lib.ptr(sq), float(self.clip),
-                                                float(g["lr"]), float(b1), float(b2), float(g["eps"]), _lib.ptr(st["dstep"]),
-                                                1.0, s), "bigru_clip_adam_step_dev")
-        self._bump_step(st, 1)
-
-    def _graph_for(self, key, x, tgt, kind, wv, pwv, denom, g):
-        """CUDA graph(s) of the train step for one (shape, loss) key (SURVEY.md 8(f) N5): static input / output buffers, the
-        C-ABI calls captured once.  One graph at world size 1; with data parallelism two (forward+loss+backward | update) with
-        the gradient all-reduce issued between them."""
-        ent = self._graphs.get(key)
-        if ent is not None:
-            return ent
+    def _launch_compute(self, buf, st, s):
+        """Forward, loss and backward of one step on stream `s`: the loss into st.loss and the gradient of the real parameters
+        into st.grad."""
         lib = _lib.load()
-        dev = x.device
-        plan = self._plan_for(x)
-        st = self._fused_state(dev)
-        B, C = x.shape[0], self.output_size               # x arrives padded to whole batch tiles; tgt has the real rows
-        ent = {"x": torch.zeros_like(x), "tgt": torch.empty_like(tgt), "logits": torch.empty(B, C, device=dev, dtype=torch.float32),
-               "dlogits": torch.zeros(B, C, device=dev, dtype=torch.float32), "stash": plan.acquire_stash(), "plan": plan}
-        args = (float(self.dropout_p), int(bool(self.spatial_dropout)), 0, 0)
-        ent["x"].copy_(x); ent["tgt"].copy_(tgt)
-        # one eager pass on the static buffers first (first-use work such as shared-memory opt-ins happens outside the capture);
-        # its parameter update is real: it is the step the caller asked for
-        s = _stream_ptr(dev)
-        split = self._dp_split(st)
-        fwd_bwd = lambda part, s_: self._launch_fwd_loss_bwd(lib, plan, ent["x"], None, ent["tgt"], kind, wv, pwv, denom, ent["logits"],
-                                                             ent["dlogits"], ent["stash"], args, st, s_, part)
-        if split:
-            fwd_bwd("upper", s)
-            self._dp_allreduce_overlapped(st, split, dev, lambda: fwd_bwd("lower", s))
-        else:
-            fwd_bwd("all", s)
-            if self._dp_world > 1:
-                allreduce_flat_(st["gext"], self._dp_group)
-        self._launch_update(lib, g, st, s)
+        plan, kind, wv, pwv, denom = buf.plan, *buf.loss
+        pflat = self._plan_params(st.pflat)
+        # the loss sees the real batch rows (tgt's); logits / dlogits may carry zero-padded rows behind them
+        B, C = buf.tgt.shape[0], buf.logits.shape[1]
+        _lib.check(lib.bigru_forward(plan.handle, _lib.ptr(pflat), _lib.ptr(buf.x), _lib.ptr(buf.h0), *buf.drop,
+                                     _lib.ptr(buf.stash), _lib.ptr(plan.scratch), _lib.ptr(buf.logits), None, s), "bigru_forward")
+        _lib.check(lib.bigru_loss(kind, _lib.ptr(buf.logits), _lib.ptr(buf.tgt), _lib.ptr(wv), _lib.ptr(pwv), B, C, denom,
+                                  _lib.ptr(st.loss), _lib.ptr(buf.dlogits), s), "bigru_loss")
+        _lib.check(lib.bigru_backward(plan.handle, _lib.ptr(pflat), _lib.ptr(buf.x), _lib.ptr(buf.h0), *buf.drop,
+                                      _lib.ptr(buf.stash), _lib.ptr(plan.scratch), _lib.ptr(buf.dlogits), _lib.ptr(st.pgrad),
+                                      None, None, s), "bigru_backward")
+        self._plan_grads(st.pgrad, st.grad)
+
+    def _launch_update(self, g, st, s):
+        """clip_grad_norm_(clip) + Adam on the flat buffers on stream `s`; Adam's step counter is incremented on the device."""
+        lib = _lib.load()
+        sq = st.scal[1:2]
+        _lib.check(lib.bigru_adam_tick(_lib.ptr(st.dstep), _lib.ptr(sq), s), "bigru_adam_tick")
+        _lib.check(lib.bigru_sqnorm(_lib.ptr(st.grad), st.grad.numel(), _lib.ptr(sq), _lib.ptr(st.sqws), s), "bigru_sqnorm")
+        b1, b2 = g["betas"]
+        _lib.check(lib.bigru_clip_adam_step_dev(_lib.ptr(self._flat), _lib.ptr(st.grad), _lib.ptr(st.m),
+                                                _lib.ptr(st.v), self._flat.numel(), _lib.ptr(sq), float(self.clip),
+                                                float(g["lr"]), float(b1), float(b2), float(g["eps"]), _lib.ptr(st.dstep),
+                                                1.0, s), "bigru_clip_adam_step_dev")
+
+    def _capture(self, key, buf, st, g):
+        """CUDA graph(s) of the step on the static buffers `buf` (SURVEY.md 8(f) N5): one graph at world size 1; with data
+        parallelism two (compute | update), replayed with the gradient all-reduce between them."""
+        lib = _lib.load()
+        dev = buf.x.device
         torch.cuda.current_stream(dev).synchronize()
         n0 = lib.bigru_launch_count()
         # an explicit capture stream ON THE MODEL'S DEVICE: torch's default capture stream is created once per process, on whichever
         # device was current then
         cap = torch.cuda.Stream(device=dev)
-        ga = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(ga, stream=cap, capture_error_mode="thread_local"):
-            s = _stream_ptr(dev)
-            fwd_bwd("upper" if split else "all", s)
-            if self._dp_world == 1:
-                self._launch_update(lib, g, st, s)
-        ga2 = None
-        if split:                                         # the lowest layer's backward: replayed while the upper layers' gradients are reduced
-            ga2 = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(ga2, stream=cap, capture_error_mode="thread_local"):
-                fwd_bwd("lower", _stream_ptr(dev))
-        gb = None
-        if self._dp_world > 1:
-            gb = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(gb, stream=cap, capture_error_mode="thread_local"):
-                self._launch_update(lib, g, st, _stream_ptr(dev))
-        self._bump_step(st, -1)                                   # the capture ran the host-side bookkeeping once without stepping
-        ent["launches"] = int(lib.bigru_launch_count() - n0)
-        lib.bigru_launch_count_add(-ent["launches"])      # captured, not executed
-        ent["ga"], ent["ga2"], ent["gb"], ent["fresh"], ent["split"] = ga, ga2, gb, True, split
+        try:
+            ga, gb = torch.cuda.CUDAGraph(), None
+            with torch.cuda.graph(ga, stream=cap, capture_error_mode="thread_local"):
+                self._launch_compute(buf, st, _stream_ptr(dev))
+                if self._dp_world == 1:
+                    self._launch_update(g, st, _stream_ptr(dev))
+            if self._dp_world > 1:
+                gb = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(gb, stream=cap, capture_error_mode="thread_local"):
+                    self._launch_update(g, st, _stream_ptr(dev))
+        except Exception as e:                            # capture is an optimisation: fall back to plain launches
+            import warnings
+            warnings.warn(f"BiGRU.train_step: CUDA-graph capture failed ({e}); using plain launches")
+            self.use_cuda_graph = False
+            ga = None
+        launches = int(lib.bigru_launch_count() - n0)
+        lib.bigru_launch_count_add(-launches)             # captured, not executed
+        if ga is None:
+            buf.plan.release_stash(buf.stash)
+            return
         if len(self._graphs) > 4:
             self._graphs.clear()
-        self._graphs[key] = ent
-        return ent
+        self._graphs[key] = (buf, ga, gb, launches)
 
     def train_step(self, input_seq, target, hidden=None):
         """One optimisation step = the body of the reference loop (biGRU_model.py:198-210):
@@ -721,61 +672,43 @@ class BiGRU(nn.Module):
                 raise ValueError(f"target must be [{B}, {C}]")
             denom = float(B * C * self._dp_world)
         training = bool(self.training and self.dropout_p > 0)
-        Bp = self._padded_batch(B)
         with torch.cuda.device(dev):
+            graphed = self.use_cuda_graph and not training and h0 is None and not torch.cuda.is_current_stream_capturing()
             wv, pwv = self._loss_vec(w, C), self._loss_vec(pw, C)
-            st = self._fused_state(dev)
-            x_real = x
-            h0 = self._pad_last(h0, self.plan_hidden(B))
-            self._last_batch = B
-            if self.use_cuda_graph and not training and h0 is None and not torch.cuda.is_current_stream_capturing():
+            st = self._fused_state()
+            s = _stream_ptr(dev)
+            key = ent = None
+            if graphed:
                 key = (B, int(x.shape[1]), self.precision, kind, id(wv), id(pwv), denom, float(g["lr"]), tuple(g["betas"]),
                        float(g["eps"]), float(self.clip), self._dp_world, dev.index)
-                try:
-                    ent = self._graphs.get(key)
-                    if ent is None:
-                        ent = self._graph_for(key, _pad_batch(x, None, Bp)[0], tgt, kind, wv, pwv, denom, g)
-                except Exception as e:                        # capture is an optimisation: fall back to plain launches
-                    import warnings
-                    warnings.warn(f"BiGRU.train_step: CUDA-graph capture failed ({e}); using plain launches")
-                    self.use_cuda_graph = False
-                    ent = None
-                if ent is not None:
-                    if ent.pop("fresh", False):               # the warm-up pass inside _graph_for WAS this step
-                        return st["loss"].clone(), ent["logits"][:B].clone()
-                    ent["x"][:B].copy_(x_real, non_blocking=True)      # rows >= B of the static buffer stay zero
-                    ent["tgt"].copy_(tgt, non_blocking=True)
-                    ent["ga"].replay()
-                    if ent["gb"] is not None:
-                        if ent["ga2"] is not None:
-                            self._dp_allreduce_overlapped(st, ent["split"], dev, ent["ga2"].replay)
-                        else:
-                            allreduce_flat_(st["gext"], self._dp_group)
-                        ent["gb"].replay()
-                    self._bump_step(st, 1)
-                    lib.bigru_launch_count_add(ent["launches"])
-                    return st["loss"].clone(), ent["logits"][:B].clone()
-            x, h0 = _pad_batch(x, h0, Bp)
-            plan = self._plan_for(x)
-            logits = torch.empty(Bp, C, device=dev, dtype=torch.float32)
-            dlogits = torch.zeros_like(logits) if Bp != B else torch.empty_like(logits)
-            stash = plan.acquire_stash()
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if training else 0
-            self._last_seed = seed
-            s = _stream_ptr(dev)
-            args = (float(self.dropout_p), int(bool(self.spatial_dropout)), int(training), seed)
-            split = self._dp_split(st)
-            if split:                                                # upper layers' gradients are reduced while layer 0 runs its backward
-                self._launch_fwd_loss_bwd(lib, plan, x, h0, tgt, kind, wv, pwv, denom, logits, dlogits, stash, args, st, s, "upper")
-                self._dp_allreduce_overlapped(st, split, dev, lambda: self._launch_fwd_loss_bwd(
-                    lib, plan, x, h0, tgt, kind, wv, pwv, denom, logits, dlogits, stash, args, st, s, "lower"))
+                ent = self._graphs.get(key)
+            if ent is not None:
+                buf, ga, gb, launches = ent
+                buf.x[:B].copy_(x, non_blocking=True)      # rows >= B of the static buffer stay zero
+                buf.tgt.copy_(tgt, non_blocking=True)
+                compute, update = ga.replay, (gb.replay if gb is not None else lambda: None)
+                lib.bigru_launch_count_add(launches)
             else:
-                self._launch_fwd_loss_bwd(lib, plan, x, h0, tgt, kind, wv, pwv, denom, logits, dlogits, stash, args, st, s)
-                if self._dp_world > 1:
-                    allreduce_flat_(st["gext"], self._dp_group)      # ONE all-reduce: shard gradients of the global-mean loss + the loss
-            plan.release_stash(stash)
-            self._launch_update(lib, g, st, s)
-            return st["loss"].clone(), (logits[:B] if Bp != B else logits)
+                seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if training else 0
+                self._last_seed = seed
+                Bp = self._padded_batch(B)
+                x, h0 = self._pad.pad(x, Bp), self._pad.pad(h0, Bp, dim=1, units=True)
+                if graphed:                               # a new graph key: this step runs on the graph's static buffers
+                    x, tgt = x.clone(), tgt.clone()
+                buf = _StepBuffers(self._plan_for(x), x, h0, tgt, (kind, wv, pwv, denom), C,
+                                   (float(self.dropout_p), int(bool(self.spatial_dropout)), int(training), seed))
+                compute, update = (lambda: self._launch_compute(buf, st, s)), (lambda: self._launch_update(g, st, s))
+            compute()
+            if self._dp_world > 1:
+                allreduce_flat_(st.gext, self._dp_group)  # ONE all-reduce: shard gradients of the global-mean loss + the loss
+            update()
+            st.advance()
+            if not graphed:
+                buf.plan.release_stash(buf.stash)
+            elif ent is None:
+                self._capture(key, buf, st, g)
+            logits = self._pad.crop(buf.logits, B)
+            return st.loss.clone(), (logits.clone() if graphed else logits)
 
     # ------------------------------------------------------------------ windows of a chunk-resident dataset (SURVEY.md 8(f) N1)
     def _window_args(self, dataset, start, count):

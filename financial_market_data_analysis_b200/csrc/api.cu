@@ -17,7 +17,7 @@ void bigru_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* bigru_last_error(void) { return g_err; }
-extern "C" int bigru_version(void) { return 202; }
+extern "C" int bigru_version(void) { return 203; }
 
 extern "C" int bigru_device_check(int dev) {
     int n = 0;
@@ -313,13 +313,11 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
 }
 
 // ------------------------------------------------------------------------------------------
-// backward of layers layer_from .. layer_to (descending); the head when layer_from is the top layer.  The upstream
-// gradient of layer l lives in dYa when L-1-l is even, else in dYb, so a split call picks up where the first left off.
+// backward: the head, then layers L-1 .. 0.  The upstream gradient of layer l lives in dYa when L-1-l is even, else in dYb.
 // ------------------------------------------------------------------------------------------
 static int backward_plan(const bigru_plan& p, const float* params, const float* x, const float* h0, float drop,
                          int spatial, int training, uint64_t seed, const float* stash, float* scratch,
-                         const float* dlogits, float* grads, float* dx, float* dh0, cudaStream_t st,
-                         int layer_from, int layer_to) {
+                         const float* dlogits, float* grads, float* dx, float* dh0, cudaStream_t st) {
     if (p.prec == BIGRU_PREC_BF16 && (h0 || dh0)) {
         bigru_set_error("BIGRU_PREC_BF16: initial hidden state / its gradient are not supported");
         return BIGRU_ERR_UNSUPPORTED;
@@ -331,17 +329,15 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
     const bool do_drop = training && drop > 0.f;
     const bool tc = p.prec != BIGRU_PREC_FP32;
     float* dhc = scratch + W.dhc;
-    if (layer_from == p.L - 1) {
-        CUDA_TRY(cudaMemsetAsync(grads, 0, sizeof(float) * p.nparams, st));
-        // head: dcat = dlogits lin_w ; dlin_w = dlogits^T cat ; dlin_b = colsum(dlogits)
-        GemmArgs a = gemm_args(dlogits, params + p.off_linw(), scratch + W.dcat, B, 3 * H, C, C, 1, 1, 3 * H, 3 * H);
-        TRY(plan_gemm(p, a, KC_HEAD, scratch, st));
-        GemmArgs w = gemm_args(dlogits, stash + S.cat, grads + p.off_linw(), C, 3 * H, B, 1, C, 1, 3 * H, 3 * H);
-        TRY(plan_gemm(p, w, KC_HEAD, scratch, st));
-        TRY(colsum_launch(dlogits, grads + p.off_linb(), B, C, C, 1, 0, 0, scratch + W.csum, st));
-        KLAUNCH(KC_HEAD, 0.0, 0.0, st, head_bwd_dy_kernel<<<nblk(BT * H, 256), 256, 0, st>>>(scratch + W.dcat, (const int*)(stash + S.arg), scratch + W.dYa, dhc, B, T, H, D));
-    }
-    for (int l = layer_from; l >= layer_to; --l) {
+    CUDA_TRY(cudaMemsetAsync(grads, 0, sizeof(float) * p.nparams, st));
+    // head: dcat = dlogits lin_w ; dlin_w = dlogits^T cat ; dlin_b = colsum(dlogits)
+    GemmArgs a = gemm_args(dlogits, params + p.off_linw(), scratch + W.dcat, B, 3 * H, C, C, 1, 1, 3 * H, 3 * H);
+    TRY(plan_gemm(p, a, KC_HEAD, scratch, st));
+    GemmArgs w = gemm_args(dlogits, stash + S.cat, grads + p.off_linw(), C, 3 * H, B, 1, C, 1, 3 * H, 3 * H);
+    TRY(plan_gemm(p, w, KC_HEAD, scratch, st));
+    TRY(colsum_launch(dlogits, grads + p.off_linb(), B, C, C, 1, 0, 0, scratch + W.csum, st));
+    KLAUNCH(KC_HEAD, 0.0, 0.0, st, head_bwd_dy_kernel<<<nblk(BT * H, 256), 256, 0, st>>>(scratch + W.dcat, (const int*)(stash + S.arg), scratch + W.dYa, dhc, B, T, H, D));
+    for (int l = p.L - 1; l >= 0; --l) {
         const int I = (int)p.in_size(l);
         const bool even = (p.L - 1 - l) % 2 == 0;
         const bool drop_l = do_drop && (l == 0 || p.L > 1);
@@ -477,27 +473,7 @@ extern "C" int bigru_backward(const bigru_plan* plan, const float* d_params, con
         return BIGRU_ERR_ARG;
     }
     return backward_plan(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, (const float*)d_stash,
-                         (float*)d_scratch, d_dlogits, d_grads, d_dx, d_dh0, (cudaStream_t)stream, plan->L - 1, 0);
-}
-
-extern "C" int bigru_backward_layers(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
-                                     float dropout_p, int spatial, int training, uint64_t seed, const void* d_stash,
-                                     void* d_scratch, const float* d_dlogits, float* d_grads, float* d_dx, float* d_dh0,
-                                     int layer_from, int layer_to, void* stream) {
-    if (!plan || !d_params || !d_x || !d_stash || !d_scratch || !d_dlogits || !d_grads) {
-        bigru_set_error("backward_layers: null argument");
-        return BIGRU_ERR_ARG;
-    }
-    if (layer_from >= plan->L || layer_to < 0 || layer_to > layer_from) {
-        bigru_set_error("backward_layers: bad layer range %d..%d for %d layers", layer_from, layer_to, plan->L);
-        return BIGRU_ERR_ARG;
-    }
-    if (plan->prec == BIGRU_PREC_FP32) {
-        bigru_set_error("backward_layers: the fp32 path runs its layers in one call (bigru_backward)");
-        return BIGRU_ERR_UNSUPPORTED;
-    }
-    return backward_plan(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, (const float*)d_stash,
-                         (float*)d_scratch, d_dlogits, d_grads, d_dx, d_dh0, (cudaStream_t)stream, layer_from, layer_to);
+                         (float*)d_scratch, d_dlogits, d_grads, d_dx, d_dh0, (cudaStream_t)stream);
 }
 
 extern "C" int bigru_chunk_minmax(const float* d_table, int64_t N, int F, int64_t row_lo, int64_t row_hi, float* d_min,

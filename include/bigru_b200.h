@@ -49,7 +49,7 @@ extern "C" {
                                       batch sizes: append zero rows to x (and zero rows to d_logits) up to the next multiple -
                                       batch rows are independent; the Python mirror does exactly that.  Smaller hidden sizes:
                                       zero-pad the parameters to the next supported hidden size (padded units stay at state 0 and
-                                      feed zero weights; BiGRU.plan_hidden / _pad_map of the mirror).  Anything else returns
+                                      feed zero weights; BiGRU.plan_hidden / _Padding of the mirror).  Anything else returns
                                       BIGRU_ERR_UNSUPPORTED. */
 
 #define BIGRU_LOSS_CE   0          /* torch.nn.CrossEntropyLoss (BASELINE.json configs) */
@@ -98,16 +98,6 @@ int  bigru_backward(const bigru_plan* plan, const float* d_params, const float* 
                     float dropout_p, int spatial, int training, uint64_t seed,
                     const void* d_stash, void* d_scratch, const float* d_dlogits,
                     float* d_grads, float* d_dx, float* d_dh0, void* stream);
-
-/* The same backward pass in two (or more) calls, layers layer_from .. layer_to downwards (tensor-core precisions only): the call
- * that starts at the top layer also zeroes d_grads and forms the head's gradients.  After bigru_backward_layers(.., L-1, 1, ..) the
- * gradients of layers >= 1 and of the head are final, so a data-parallel caller can start their all-reduce while
- * bigru_backward_layers(.., 0, 0, ..) still runs (BiGRU.train_step with enable_data_parallel does exactly that; no reference
- * counterpart: /root/reference has no distributed code). */
-int  bigru_backward_layers(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
-                           float dropout_p, int spatial, int training, uint64_t seed,
-                           const void* d_stash, void* d_scratch, const float* d_dlogits,
-                           float* d_grads, float* d_dx, float* d_dh0, int layer_from, int layer_to, void* stream);
 
 /* --- losses (biGRU_model.py:202 `self.loss_fn(pred, target)`), fused value + d(loss)/d(logits).
  *  kind CE: d_target int64[B]; BCE/MLSM: d_target float[B,C]; d_weight/d_pos_weight nullable [C]

@@ -40,7 +40,7 @@ def test_library_exports_every_declared_symbol(pkg):
     assert lib.bigru_version() >= 100
 
 
-def test_plan_bookkeeping_without_gpu(pkg):
+def test_plan_bookkeeping_and_null_backward_input_without_gpu(pkg):
     """Plans are host objects: parameter layout and workspace sizes can be checked on CPU."""
     lib, C = pkg._lib.load(), pkg._lib.C
     h = C.c_void_p()
@@ -61,7 +61,6 @@ def test_plan_bookkeeping_without_gpu(pkg):
         assert lib.bigru_plan_create(32, 4, 8, 128, 1, 3, 1, pkg._lib.PREC_BF16X3, C.byref(h)) == 0
         dev = C.c_void_p(256)                                        # stands for a device pointer; never dereferenced
         assert lib.bigru_backward(h, dev, None, None, 0.0, 0, 0, 0, dev, dev, dev, dev, None, None, None) == pkg._lib.ERR_ARG
-        assert lib.bigru_backward_layers(h, dev, None, None, 0.0, 0, 0, 0, dev, dev, dev, dev, None, None, 0, 0, None) == pkg._lib.ERR_ARG
         assert b"null argument" in lib.bigru_last_error()
         lib.bigru_plan_destroy(h)
 
@@ -111,27 +110,8 @@ def test_model_surface_and_state_dict(pkg, golden_dir):
         pkg.BiGRU(8, 4, 2, 1, precision="fp64")
 
 
-def test_dp_split_offset_is_the_first_upper_layer_parameter(pkg, monkeypatch):
-    """BiGRU._dp_split (data-parallel overlap experiment): the flat-gradient offset where layer 1 starts equals the offset of
-    gru.weight_ih_l1 in the C-ABI parameter order; the split is off by default, for one layer, for fp32 and for padded hidden sizes."""
-    m = pkg.BiGRU(128, 24, 3, 2, precision="bf16x3")
-    m._dp_world = 2
-    names = [n for n, _ in m.named_parameters()]
-    off = {n: o for n, (o, _, _) in zip(names, m._views)}
-    assert m._dp_split({}) == 0                                         # opt-in only
-    monkeypatch.setenv("BIGRU_B200_DP_OVERLAP", "1")
-    assert m._dp_split({}) == off["gru.weight_ih_l1"] > 0
-    assert m._dp_split({"pflat": None}) == 0                            # hidden-size padding: gradients are gathered after the whole backward
-    one = pkg.BiGRU(128, 24, 3, 1, precision="bf16x3"); one._dp_world = 2
-    assert one._dp_split({}) == 0
-    f32 = pkg.BiGRU(128, 24, 3, 2, precision="fp32"); f32._dp_world = 2
-    assert f32._dp_split({}) == 0
-    m._dp_world = 1
-    assert m._dp_split({}) == 0
-
-
 def test_hidden_padding_index_map(pkg):
-    """BiGRU._pad_map (real parameter -> position in the zero-padded plan's flat vector) against an independent construction:
+    """BiGRU._plan_params / _plan_grads (real parameter -> position in the zero-padded plan's flat vector) against an independent construction:
     every weight tensor zero-padded by its own rule (gate rows g*H + j -> g*Hp + j, input columns of upper layers d*H + k ->
     d*Hp + k, head columns part*H + j -> part*Hp + j) and flattened in the C-ABI order."""
     import oracle_c
