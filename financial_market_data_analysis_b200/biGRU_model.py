@@ -503,13 +503,20 @@ class BiGRU(nn.Module):
                     and fn.ignore_index == -100:
                 return _lib.LOSS_CE, None, None
         elif isinstance(fn, nn.BCEWithLogitsLoss):
-            per_class = lambda w: w is None or w.numel() in (1, self.output_size)      # per-element weights: autograd path
-            if fn.reduction == "mean" and per_class(fn.weight) and per_class(fn.pos_weight):
+            if fn.reduction == "mean" and self._per_class(fn.weight) and self._per_class(fn.pos_weight):
                 return _lib.LOSS_BCE, fn.weight, fn.pos_weight
         elif isinstance(fn, nn.MultiLabelSoftMarginLoss):
             if fn.weight is None and fn.reduction == "mean":
                 return _lib.LOSS_MLSM, None, None
         return None
+
+    def _per_class(self, w):
+        """Whether a BCE weight broadcasts over [B, C] logits as one value per class: a single element, or C values along the
+        last dimension with every leading dimension 1.  Anything else ([C, 1], per-row, per-element) weighs rows, which the
+        fused loss cannot express, even when its element count happens to be C."""
+        if w is None or w.numel() == 1:
+            return True
+        return w.dim() >= 1 and w.shape[-1] == self.output_size and all(s == 1 for s in w.shape[:-1])
 
     def _adam_spec(self):
         opt = self.optimizer

@@ -17,7 +17,7 @@ void bigru_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* bigru_last_error(void) { return g_err; }
-extern "C" int bigru_version(void) { return 203; }
+extern "C" int bigru_version(void) { return 204; }
 
 extern "C" int bigru_device_check(int dev) {
     int n = 0;

@@ -286,16 +286,19 @@ __global__ void loss_kernel(int kind, const float* __restrict__ logits, const vo
     for (int b = threadIdx.x; b < B; b += blockDim.x) {
         const float* lg = logits + (int64_t)b * C;
         if (kind == BIGRU_LOSS_CE) {
+            // a target outside [0, C) (torch's ignore_index -100 included) is never read through: its row's loss and dlogits
+            // are NaN, so the mismatch with torch, which would skip the row, cannot pass unnoticed
             const long long tg = ((const long long*)target)[b];
+            const bool valid = tg >= 0 && tg < C;
             float m = lg[0];
             for (int c = 1; c < C; ++c) m = fmaxf(m, lg[c]);
             float s = 0.f;
             for (int c = 0; c < C; ++c) s += expf(lg[c] - m);
             const float lse = m + logf(s);
-            l += lse - lg[tg];
+            l += lse - (valid ? lg[tg] : nanf(""));
             if (dlogits)
                 for (int c = 0; c < C; ++c)
-                    dlogits[(int64_t)b * C + c] = (expf(lg[c] - lse) - (c == tg ? 1.f : 0.f)) * inv_denom;
+                    dlogits[(int64_t)b * C + c] = valid ? (expf(lg[c] - lse) - (c == tg ? 1.f : 0.f)) * inv_denom : nanf("");
         } else {
             const float* tg = (const float*)target + (int64_t)b * C;
             for (int c = 0; c < C; ++c) {
@@ -442,7 +445,9 @@ __global__ void multilabel_counts_kernel(const float* __restrict__ logits, const
     if (b >= B) return;
     int mism = 0;
     for (int c = 0; c < C; ++c) {
-        const bool pred = logits[(int64_t)b * C + c] > 0.f;          // sigmoid(x) > 0.5  <=>  x > 0
+        // fp32 sigmoid as torch.sigmoid evaluates it on the GPU: it rounds to exactly 0.5 for positive x below about 1e-7,
+        // so the test is not the same as x > 0
+        const bool pred = 1.f / (1.f + expf(-logits[(int64_t)b * C + c])) > 0.5f;
         const bool tru = target[(int64_t)b * C + c] > 0.5f;
         if (pred != tru) ++mism;
         if (pred && tru) atomicAdd(counts + 2 + 3 * c, 1ull);

@@ -102,7 +102,9 @@ int  bigru_backward(const bigru_plan* plan, const float* d_params, const float* 
 /* --- losses (biGRU_model.py:202 `self.loss_fn(pred, target)`), fused value + d(loss)/d(logits).
  *  kind CE: d_target int64[B]; BCE/MLSM: d_target float[B,C]; d_weight/d_pos_weight nullable [C]
  *  (BCE only).  Mean reduction over `denom` elements (B for CE, B*C otherwise; pass the GLOBAL
- *  count under data parallelism).  d_loss: one float, overwritten. */
+ *  count under data parallelism).  d_loss: one float, overwritten.  CE needs every target in [0, C): it does not
+ *  implement nn.CrossEntropyLoss's ignore_index, and a row whose target lies outside [0, C) (ignore_index = -100
+ *  included) is not read through but makes the loss and that row's dlogits NaN. */
 int  bigru_loss(int kind, const float* d_logits, const void* d_target, const float* d_weight,
                 const float* d_pos_weight, int B, int C, double denom, float* d_loss,
                 float* d_dlogits, void* stream);
@@ -156,7 +158,9 @@ int  bigru_window_features(const float* d_close, const float* d_high, const floa
 int  bigru_infer_window(const float* d_params, const float* d_x, const float* d_xmin, const float* d_xmax, int B, int T,
                         int F, int H, int L, int C, int bidirectional, float* d_logits, float* d_probs, void* stream);
 
-/* --- train_model/evaluate_model metrics (biGRU_model.py:213-221): pred = sigmoid(logit) > 0.5;
+/* --- train_model/evaluate_model metrics (biGRU_model.py:213-221): pred = sigmoid(logit) > 0.5 with the sigmoid
+ *  evaluated in fp32 as torch.sigmoid does (false for positive logits below about 1e-7, where it rounds to 0.5);
+ *  true = target > 0.5;
  *  d_counts[0] += #rows with all labels right; [1] += #label mismatches;
  *  [2+3c], [3+3c], [4+3c] += tp, fp, fn of class c.  int64 accumulators, caller zeroes. */
 int  bigru_multilabel_counts(const float* d_logits, const float* d_target, int B, int C,

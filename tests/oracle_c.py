@@ -138,7 +138,18 @@ def loss_bce(logits, target, weight=None, pos_weight=None, scale=None):
     return v, d
 
 
+def loss_mlsm(logits, target, scale=None):
+    B, C_ = logits.shape
+    lg = np.ascontiguousarray(logits, np.float32)
+    tg = np.ascontiguousarray(target, np.float32)
+    d = np.zeros_like(lg)
+    v = lib().bigru_ref_loss_mlsm(B, C_, _p(lg), _p(tg), _p(d), C.c_double(scale or 1.0 / (B * C_)))
+    return v, d
+
+
 def clip_adam(params, grads, m, v, clip, lr, b1, b2, eps, step):
+    """clip_grad_norm_ + one Adam step in fp64, on float32 arrays updated in place (grads become the clipped gradient).
+    Returns the norm of the unclipped gradient."""
     return lib().bigru_ref_clip_adam(C.c_int64(params.size), _p(params), _p(grads), _p(m), _p(v), C.c_double(clip),
                                      C.c_double(lr), C.c_double(b1), C.c_double(b2), C.c_double(eps), step)
 

@@ -110,6 +110,31 @@ def test_model_surface_and_state_dict(pkg, golden_dir):
         pkg.BiGRU(8, 4, 2, 1, precision="fp64")
 
 
+def test_bce_weight_fuses_only_when_it_broadcasts_per_class(pkg):
+    """The fused BCE applies weight[c] / pos_weight[c] to every row.  A weight of C elements that broadcasts over rows
+    instead ([C, 1] against logits [B, C] with B == C) must take the autograd path, or the fused step would compute a
+    different loss than torch."""
+    C = B = 4
+    m = pkg.BiGRU(8, 5, C, 1, 50, 0.0, False, True)
+    m.add_optimizer(torch.optim.Adam(m.parameters(), lr=1e-3))
+    g = torch.Generator().manual_seed(3)
+    logits, target = torch.randn(B, C, generator=g), (torch.rand(B, C, generator=g) < 0.5).float()
+    w = torch.rand(C, generator=g) + 0.5
+    # what torch computes with the [C, 1] weight is row-weighted: not the per-class loss the fused kernel would apply
+    row_w = nn.BCEWithLogitsLoss(weight=w.reshape(C, 1))(logits, target)
+    col_w = nn.BCEWithLogitsLoss(weight=w)(logits, target)
+    assert not torch.allclose(row_w, col_w)
+    for kw in ({"weight": w.reshape(C, 1)}, {"pos_weight": w.reshape(C, 1)}, {"weight": w.reshape(C, 1, 1)},
+               {"weight": torch.rand(B, C, generator=g)}, {"weight": w.reshape(2, 2)}):
+        m.add_loss_fn(nn.BCEWithLogitsLoss(**kw))
+        assert m._loss_spec() is None and not m.can_fuse_step(), kw
+    for kw in ({}, {"weight": w}, {"weight": w.reshape(1, C)}, {"weight": w.reshape(1, 1, C)}, {"pos_weight": w},
+               {"weight": torch.tensor(2.0)}, {"weight": torch.tensor([2.0])}, {"pos_weight": torch.ones(1, 1)},
+               {"weight": w.reshape(1, C), "pos_weight": w}):
+        m.add_loss_fn(nn.BCEWithLogitsLoss(**kw))
+        assert m._loss_spec() is not None and m.can_fuse_step(), kw
+
+
 def test_hidden_padding_index_map(pkg):
     """BiGRU._plan_params / _plan_grads (real parameter -> position in the zero-padded plan's flat vector) against an independent construction:
     every weight tensor zero-padded by its own rule (gate rows g*H + j -> g*Hp + j, input columns of upper layers d*H + k ->
