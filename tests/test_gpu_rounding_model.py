@@ -12,16 +12,15 @@ dh0 are compared, each on its own.  The oracle's backward routes the max-pool gr
 (bigru_stash_argmax_offset).
 Run on an H100:  python -m pytest tests/test_gpu_rounding_model.py -m gpu -q
 (BIGRU_ROUNDING_REPORT=path.json appends every measured distance to that file.)"""
-import ctypes as C
 import functools
 import json
 import os
 
 import numpy as np
 import pytest
-import torch
 
 import oracle_c
+from gru_driver import abi_names, dist as _dist, kernel, kernel_steps as _kernel_steps, stepwise as _stepwise, tensors as _tensors
 
 NSM = 132                  # SMs of an H100 SXM: what wg_splits (tc_hopper.cuh) aims its split-K at
 
@@ -100,7 +99,6 @@ TOL = {
                "logits": (2.8e-5, 3.7e-5), "y": (1.7e-5, 1.8e-5), "hn": (1.4e-5, 1.7e-5),
                "w": (3.8e-5, 4.7e-5), "b": (2.7e-5, 3e-5), "dx": (4.5e-5, 4.5e-5), "dh0": (1e-5, 1e-5)},
 }
-CODE = {"bf16": 1, "bf16x3": 2}
 
 
 def test_shapes_are_in_the_regimes_they_claim():
@@ -131,63 +129,6 @@ def _inputs(s):
     return flat, x, h0, dl
 
 
-def _param_names(plan, s):
-    """name -> (offset, size) of every parameter block, from bigru_param_offset."""
-    lib = _pkg()._lib.load()
-    out = {}
-    off, rows, cols = C.c_int64(), C.c_int64(), C.c_int64()
-    for l in range(s["L"] + 1):
-        for d in range(s["D"] if l < s["L"] else 1):
-            for which, nm in enumerate(("w_ih", "w_hh", "b_ih", "b_hh")):
-                if l == s["L"] and which in (1, 3):
-                    continue
-                assert lib.bigru_param_offset(plan, l, d, which, C.byref(off), C.byref(rows), C.byref(cols)) == 0
-                name = ("lin_w" if which == 0 else "lin_b") if l == s["L"] else f"l{l}d{d}.{nm}"
-                out[name] = (off.value, rows.value * cols.value)
-    return out
-
-
-def _kernel(s, prec, flat, x, h0, dl):
-    pkg = _pkg()
-    lib, L_ = pkg._lib.load(), pkg._lib
-    B, T, F, H, L, C_, D = (s[k] for k in "BTFHLCD")
-    plan = C.c_void_p()
-    L_.check(lib.bigru_plan_create(B, T, F, H, L, C_, int(D == 2), CODE[prec], C.byref(plan)), "plan_create")
-    try:
-        sb, cb = C.c_size_t(), C.c_size_t()
-        L_.check(lib.bigru_workspace_bytes(plan, C.byref(sb), C.byref(cb)), "workspace_bytes")
-        dev = torch.device("cuda")
-        stash = torch.zeros(sb.value // 4, dtype=torch.float32, device=dev)
-        scratch = torch.zeros(cb.value // 4, dtype=torch.float32, device=dev)
-        p, xd = torch.from_numpy(flat).to(dev), torch.from_numpy(x).to(dev)
-        h0d = None if h0 is None else torch.from_numpy(h0).to(dev)
-        logits = torch.zeros(B, C_, device=dev)
-        hn = torch.zeros(L * D, B, H, device=dev)
-        st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-        ptr = L_.ptr
-        L_.check(lib.bigru_forward(plan, ptr(p), ptr(xd), ptr(h0d), 0.0, 0, 0, 0, ptr(stash), ptr(scratch), ptr(logits), ptr(hn), st),
-                 "forward")
-        off = C.c_size_t()
-        ys = []
-        for l in range(L):
-            L_.check(lib.bigru_stash_output_offset(plan, l, C.byref(off)), "stash_output_offset")
-            ys.append(stash[off.value // 4: off.value // 4 + B * T * D * H].view(B, T, D * H).cpu().numpy().astype(np.float64))
-        L_.check(lib.bigru_stash_argmax_offset(plan, C.byref(off)), "stash_argmax_offset")
-        arg = stash.view(torch.int32)[off.value // 4: off.value // 4 + B * H].view(B, H).cpu().numpy().astype(np.int64)
-        grads = torch.zeros(flat.size, device=dev)
-        dx = torch.zeros(B, T, F, device=dev)
-        dh0 = torch.zeros(L * D, B, H, device=dev) if h0 is not None else None
-        dld = torch.from_numpy(dl).to(dev)                      # alive until the synchronize below: the backward reads it
-        L_.check(lib.bigru_backward(plan, ptr(p), ptr(xd), ptr(h0d), 0.0, 0, 0, 0, ptr(stash), ptr(scratch),
-                                    ptr(dld), ptr(grads), ptr(dx), ptr(dh0), st), "backward")
-        torch.cuda.synchronize()
-        names = _param_names(plan, s)
-    finally:
-        lib.bigru_plan_destroy(plan)
-    f64 = lambda t: None if t is None else t.cpu().numpy().astype(np.float64)   # noqa: E731
-    return dict(logits=f64(logits), hn=f64(hn), ys=ys, arg=arg, grads=f64(grads), dx=f64(dx), dh0=f64(dh0)), names
-
-
 @functools.lru_cache(maxsize=None)
 def _oracle_forward(name, prec):
     s = SHAPES[name]
@@ -211,72 +152,6 @@ def _oracle(name, prec, arg):
                 dh0=dh0.astype(np.float64) if h0 is not None else None)
 
 
-def _bf16(v32):
-    """Round float32 to the nearest bf16 (ties to even), returned as float32."""
-    u = np.ascontiguousarray(v32, np.float32).view(np.uint32)
-    u = (u + np.uint32(0x7FFF) + ((u >> np.uint32(16)) & np.uint32(1))) & np.uint32(0xFFFF0000)
-    return u.view(np.float32)
-
-
-def _mm(a, b, prec):
-    """a[M,K] b[N,K]^T in float64 with both operands rounded as the kernels store them (fp32, then bf16 or a bf16 pair):
-    ah bf + al bh = ah bh + ah bl + al bh, the rule of oracle/bigru_ref.c."""
-    if prec == "exact":
-        return a @ b.T
-    def split(v):
-        v32 = v.astype(np.float32)
-        hi = _bf16(v32)
-        lo = _bf16(v32 - hi) if prec == "bf16x3" else np.zeros_like(hi)
-        return hi.astype(np.float64) + lo, hi.astype(np.float64), lo.astype(np.float64)
-    _, ah, al = split(a)
-    bf, bh, _ = split(b)
-    return ah @ bf.T + al @ bh.T
-
-
-def _stepwise(s, prec, flat, x, h0, dl, got, names):
-    """The rounding model run one step at a time from the kernel's own state: every step of every layer starts from the
-    kernel's h_{t-1} (its Y, or h0) and the kernel's layer input (x, or the previous layer's Y), the head from the kernel's
-    top-layer Y.  Rounding flips cannot compound, so what is left of the kernel's distance is the fp32 arithmetic of one
-    step.  Returns (name, class) -> array like _tensors: Y per layer, direction and step, the logits and the lin_w gradient."""
-    B, T, H, L, C_, D = (s[k] for k in "BTHLCD")
-    out = {}
-    sig = lambda v: 1 / (1 + np.exp(-v))                        # noqa: E731
-    inp = x.astype(np.float64)
-    for l in range(L):
-        Y = got["ys"][l]
-        I = inp.shape[2]
-        for d in range(D):
-            o = names[f"l{l}d{d}.w_ih"][0]
-            w_ih = flat[o:o + 3 * H * I].reshape(3 * H, I).astype(np.float64); o += 3 * H * I
-            w_hh = flat[o:o + 3 * H * H].reshape(3 * H, H).astype(np.float64); o += 3 * H * H
-            b_ih, b_hh = flat[o:o + 3 * H].astype(np.float64), flat[o + 3 * H:o + 6 * H].astype(np.float64)
-            y = Y[:, :, d * H:(d + 1) * H]
-            start = np.zeros((B, H)) if h0 is None else h0[l * D + d].astype(np.float64)
-            if d == 0:
-                hp = np.concatenate([start[:, None], y[:, :-1]], 1)
-            else:
-                hp = np.concatenate([y[:, 1:], start[:, None]], 1)
-            gi = (_mm(inp.reshape(B * T, I), w_ih, prec) + b_ih).reshape(B, T, 3 * H)
-            gh = (_mm(hp.reshape(B * T, H), w_hh, prec) + b_hh).reshape(B, T, 3 * H)
-            r = sig(gi[..., :H] + gh[..., :H])
-            z = sig(gi[..., H:2 * H] + gh[..., H:2 * H])
-            n = np.tanh(gi[..., 2 * H:] + r * gh[..., 2 * H:])
-            h = (1 - z) * n + z * hp
-            for t in range(T):
-                out[(f"step:y[l{l}d{d},t{t}]", "y_step")] = h[:, t]
-        inp = Y
-    top = got["ys"][-1]
-    pooled = top[..., :H] + top[..., H:] if D == 2 else top
-    last = top[:, T - 1, :H] + (top[:, 0, H:] if D == 2 else 0)
-    cat = np.concatenate([last, pooled.max(1), pooled.sum(1) / T], 1)
-    o = names["lin_w"][0]
-    lin_w = flat[o:o + C_ * 3 * H].reshape(C_, 3 * H).astype(np.float64)
-    lin_b = flat[names["lin_b"][0]:names["lin_b"][0] + C_].astype(np.float64)
-    out[("step:logits", "logits_step")] = _mm(cat, lin_w, prec) + lin_b
-    out[("step:grad:lin_w", "w_step")] = _mm(dl.astype(np.float64).T, cat.T, prec).ravel()
-    return out
-
-
 @pytest.mark.parametrize("prec", ["bf16", "bf16x3"])
 def test_stepwise_model_reproduces_the_oracle(prec):
     """Fed the oracle's own state instead of the kernel's, the one-step model is the oracle's rounding model again."""
@@ -288,58 +163,11 @@ def test_stepwise_model_reproduces_the_oracle(prec):
     grads = oracle_c.backward(flat, x, stash, dl, H, L, C_, D, prec=oracle_c.PRECISION[prec])[0]
     own = dict(ys=[y.copy() for y in oracle_c.layer_outputs(stash, B, T, H, L, D)], logits=logits.astype(np.float64),
                grads=grads.astype(np.float64))
-    names = {}
-    o = 0
-    for l in range(L):
-        for d in range(D):
-            for nm, n in (("w_ih", 3 * H * (s["F"] if l == 0 else D * H)), ("w_hh", 3 * H * H), ("b_ih", 3 * H), ("b_hh", 3 * H)):
-                names[f"l{l}d{d}.{nm}"] = (o, n)
-                o += n
-    names["lin_w"], names["lin_b"] = (o, C_ * 3 * H), (o + C_ * 3 * H, C_)
+    names = abi_names(s)
     want, got = _kernel_steps(own, s, names), _stepwise(s, prec, flat, x, h0, dl, own, names)
     for key, v in want.items():
         tol = 1e-12 if key[1] == "y_step" else 2e-7             # logits and gradients come back from the oracle as float32
         assert np.abs(got[key] - v).max() <= tol * np.abs(v).max(), key
-
-
-def _kernel_steps(got, s, names):
-    """The kernel's side of _stepwise."""
-    H = s["H"]
-    out = {}
-    for l, y in enumerate(got["ys"]):
-        for d in range(s["D"]):
-            for t in range(s["T"]):
-                out[(f"step:y[l{l}d{d},t{t}]", "y_step")] = y[:, t, d * H:(d + 1) * H]
-    out[("step:logits", "logits_step")] = got["logits"]
-    o, k = names["lin_w"]
-    out[("step:grad:lin_w", "w_step")] = got["grads"][o:o + k]
-    return out
-
-
-def _tensors(r, s, names):
-    """(name, class) -> array of every compared tensor; y per layer and time step, hn and dh0 per layer and direction."""
-    out = {("logits", "logits"): r["logits"], ("dx", "dx"): r["dx"]}
-    H, T = s["H"], s["T"]
-    for l, y in enumerate(r["ys"]):
-        for d in range(s["D"]):
-            for t in range(T):
-                out[(f"y[l{l}d{d},t{t}]", "y")] = y[:, t, d * H:(d + 1) * H]
-    for i in range(s["L"] * s["D"]):
-        out[(f"hn[l{i // s['D']}d{i % s['D']}]", "hn")] = r["hn"][i]
-        if r["dh0"] is not None:
-            out[(f"dh0[l{i // s['D']}d{i % s['D']}]", "dh0")] = r["dh0"][i]
-    for n, (o, k) in names.items():
-        out[(f"grad:{n}", "b" if n.split(".")[-1] in ("b_ih", "b_hh", "lin_b") else "w")] = r["grads"][o:o + k]
-    return out
-
-
-def _dist(a, b):
-    """(rel-L2, max-abs / max |b|); a reference of zeros admits only zeros."""
-    nb, mb = np.linalg.norm(b), np.abs(b).max()
-    d = a - b
-    if mb == 0:
-        return (0.0, 0.0) if not d.any() else (np.inf, np.inf)
-    return float(np.linalg.norm(d) / nb), float(np.abs(d).max() / mb)
 
 
 CASES = [(n, p) for n, s in SHAPES.items() for p in s["precs"]]
@@ -354,7 +182,7 @@ def test_kernel_matches_its_rounding_model(name, prec):
     s = SHAPES[name]
     B, H, D = s["B"], s["H"], s["D"]
     flat, x, h0, dl = _inputs(s)
-    got, names = _kernel(s, prec, flat, x, h0, dl)
+    got, names = kernel(s, prec, flat, x, h0, dl)
 
     # max-pool routing: where the kernel picked another time step than the model, the two must tie to within the kernel's
     # own deviation from the model (if |s_k - s_m| <= e everywhere, the kernel's choice is at most 2e below the model's max)
