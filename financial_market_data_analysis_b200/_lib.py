@@ -33,6 +33,8 @@ SIGNATURES = {
     "bigru_stash_output_offset": (_i, [_vp, _i, C.POINTER(C.c_size_t)]),
     "bigru_forward": (_i, [_vp, _vp, _vp, _vp, _f, _i, _i, _u64, _vp, _vp, _vp, _vp, _vp]),
     "bigru_backward": (_i, [_vp, _vp, _vp, _vp, _f, _i, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "bigru_infer_workspace_bytes": (_i, [_vp, C.POINTER(C.c_size_t)]),
+    "bigru_infer": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_loss": (_i, [_i, _vp, _vp, _vp, _vp, _i, _i, _d, _vp, _vp, _vp]),
     "bigru_sqnorm": (_i, [_vp, _i64, _vp, _vp, _vp]),
     "bigru_adam_tick": (_i, [_vp, _vp, _vp]),

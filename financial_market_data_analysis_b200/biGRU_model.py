@@ -204,7 +204,8 @@ class _GRUWeights(nn.Module):
 
 
 class _Plan:
-    """A C plan plus its device workspaces for one (B, T) shape."""
+    """A C plan plus its device workspaces for one (B, T) shape.  Each workspace is allocated on first use: a plan that only
+    runs ``BiGRU.infer`` holds the inference workspace alone, not the stash and scratch of the training forward."""
 
     def __init__(self, model: "BiGRU", B: int, T: int, device):
         lib = _lib.load()
@@ -215,11 +216,23 @@ class _Plan:
                                          int(model.bidirectional), _PRECISIONS[model.resolved_precision(B)], _lib.C.byref(h)),
                    "bigru_plan_create")
         self.handle, self.B, self.T, self.device = h, B, T, device
-        a, b = _lib.C.c_size_t(), _lib.C.c_size_t()
+        a, b, c = _lib.C.c_size_t(), _lib.C.c_size_t(), _lib.C.c_size_t()
         _lib.check(lib.bigru_workspace_bytes(h, _lib.C.byref(a), _lib.C.byref(b)), "bigru_workspace_bytes")
-        self.stash_bytes, self.scratch_bytes = a.value, b.value
-        self.scratch = torch.empty(max(self.scratch_bytes, 16), dtype=torch.uint8, device=device)
+        _lib.check(lib.bigru_infer_workspace_bytes(h, _lib.C.byref(c)), "bigru_infer_workspace_bytes")
+        self.stash_bytes, self.scratch_bytes, self.infer_bytes = a.value, b.value, c.value
+        self._scratch = self._infer_ws = None
         self._free_stash = []
+
+    @property
+    def scratch(self):
+        if self._scratch is None:
+            self._scratch = torch.empty(max(self.scratch_bytes, 16), dtype=torch.uint8, device=self.device)
+        return self._scratch
+
+    def infer_workspace(self):
+        if self._infer_ws is None:
+            self._infer_ws = torch.empty(max(self.infer_bytes, 16), dtype=torch.uint8, device=self.device)
+        return self._infer_ws
 
     def acquire_stash(self):
         if self._free_stash:
@@ -477,6 +490,44 @@ class BiGRU(nn.Module):
         self.batch_size, self.input_length = x.size(0), x.size(1)          # as the reference sets (:82-85)
         return _BiGRUFunction.apply(self, x, h0, *self._ordered_params())
 
+    def infer(self, input_seq, hidden=None, max_batch: Optional[int] = None):
+        """Eval-mode logits [batch, output_size] (bigru_infer), bit-identical to ``self.eval()(input_seq, hidden)`` under
+        ``torch.no_grad()``: no dropout whatever ``self.training`` says, no autograd record, and nothing kept for a backward, so
+        the plan allocates only its inference workspace (about a sixth of the training forward's stash + scratch at
+        configs[1]).  ``max_batch`` runs the batch in slices of at most that many rows, all on one plan (the last slice
+        zero-padded), which bounds the memory whatever the batch size.  ``pooled_argmax()`` and the last hidden state stay
+        those of the last ``forward``."""
+        x, h0 = self._prepare_input(input_seq, hidden)
+        B = x.shape[0]
+        k = self._slice_rows(max_batch, B)
+        pflat = self._plan_params()
+        outs = [self._infer_slice(pflat, x[s:s + k], None if h0 is None else h0[:, s:s + k], self._pad.batch(k))
+                for s in range(0, B, k)]
+        return outs[0] if len(outs) == 1 else torch.cat(outs)
+
+    @staticmethod
+    def _slice_rows(max_batch, n):
+        """Rows per slice when `infer` splits n rows by max_batch."""
+        if max_batch is None:
+            return n
+        if int(max_batch) <= 0:
+            raise ValueError(f"max_batch must be positive, got {max_batch}")
+        return min(int(max_batch), n)
+
+    def _infer_slice(self, pflat, x, h0, Bp):
+        """Logits of the rows of x (at most Bp) through bigru_infer on the plan of Bp rows; pflat: _plan_params()."""
+        pad, B = self._pad, x.shape[0]
+        x = pad.pad(x, Bp)
+        h0 = pad.pad(h0, Bp, dim=1, units=True)
+        h0 = None if h0 is None else h0.contiguous()
+        plan = self._plan_for(x)
+        with torch.no_grad(), torch.cuda.device(x.device):    # the C ABI launches on the CURRENT device: make it the model's
+            logits = torch.empty(Bp, self.output_size, device=x.device, dtype=torch.float32)
+            _lib.check(_lib.load().bigru_infer(plan.handle, _lib.ptr(pflat), _lib.ptr(x), _lib.ptr(h0),
+                                               _lib.ptr(plan.infer_workspace()), _lib.ptr(logits), _stream_ptr(x.device)),
+                       "bigru_infer")
+        return pad.crop(logits, B)
+
     def add_loss_fn(self, loss_fn):
         self.loss_fn = loss_fn
 
@@ -733,6 +784,19 @@ class BiGRU(nn.Module):
         self._window_args(dataset, start, count)
         with torch.no_grad():
             return self.forward(dataset.collate(start, count)[0])
+
+    def infer_windows(self, dataset, start: int, count: int, max_batch: Optional[int] = None):
+        """``infer`` on windows start .. start+count-1 of a chunk-resident ``MySQLBatchLoader``: eval-mode logits, bit-identical
+        to ``forward_windows`` in eval mode.  The windows are collated one slice of at most ``max_batch`` at a time, so the
+        whole [count, window, F] input never exists at once."""
+        self._window_args(dataset, start, count)
+        k = self._slice_rows(max_batch, count)
+        pflat, Bp = self._plan_params(), self._pad.batch(k)
+        outs = []
+        for s in range(start, start + count, k):
+            x, _ = self._prepare_input(dataset.collate(s, min(k, start + count - s))[0], None)
+            outs.append(self._infer_slice(pflat, x, None, Bp))
+        return outs[0] if len(outs) == 1 else torch.cat(outs)
 
     def train_step_windows(self, dataset, start: int, count: int):
         """``train_step`` on windows of a chunk-resident dataset, inputs and targets collated on the device.

@@ -17,7 +17,7 @@ void bigru_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* bigru_last_error(void) { return g_err; }
-extern "C" int bigru_version(void) { return 204; }
+extern "C" int bigru_version(void) { return 205; }
 
 extern "C" int bigru_device_check(int dev) {
     int n = 0;
@@ -113,6 +113,38 @@ static ScratchF32 scratch_layout(const bigru_plan& p) {
     s.total = o;
     return s;
 }
+// Inference workspace (bigru_infer): what the next layer and the head read, nothing for a backward.  gi is reused by every
+// layer.  Tensor-core precisions: a lower layer writes only its Y planes (yp[l % 2]; none at L = 1, one buffer at L = 2,
+// ping-pong from L = 3), the top layer only its fp32 Y (y[0]), which the pooling head reads; tcw holds the packed W_ih and
+// head operands.  fp32: every layer writes fp32 Y into y[l % 2] (its per-step gh GEMM reads h_{t-1} from there) and gh is
+// the per-step gh buffer; no planes, no tcw.
+struct InferF32 {
+    int64_t gi, gh, y[2], cat, arg, xp, yp[2], tcw, total;
+};
+static InferF32 infer_layout(const bigru_plan& p) {
+    InferF32 s{};
+    int64_t o = 0;
+    const int64_t BT = (int64_t)p.B * p.T, DH = (int64_t)p.D * p.H;
+    const bool tc = p.prec != BIGRU_PREC_FP32;
+    s.gi = o; o += (int64_t)p.D * BT * 3 * p.H;
+    s.gh = o; if (!tc) o += (int64_t)p.D * p.B * 3 * p.H;
+    s.y[0] = o; o += BT * DH;
+    s.y[1] = o; if (!tc && p.L > 1) o += BT * DH;
+    s.cat = o; o += (int64_t)p.B * 3 * p.H;
+    s.arg = o; o += (int64_t)p.B * p.H;
+    o = rup(o, 64);
+    s.xp = o; o += plane_floats(p, BT * in_pitch(p, 0));
+    s.yp[0] = o; if (p.L > 1) o += plane_floats(p, BT * DH);
+    s.yp[1] = o; if (p.L > 2) o += plane_floats(p, BT * DH);
+    s.tcw = o;
+    if (tc) {
+        int64_t need = tc_gemm_ws_elems(p.B, p.C, 3LL * p.H, 1, p.prec);                       // head
+        for (int l = 0; l < p.L; ++l) need = std::max(need, tc_pack_elems(3LL * p.H, p.in_size(l), p.D, p.prec));   // W_ih
+        o += plane_floats(p, need);
+    }
+    s.total = o;
+    return s;
+}
 
 // Shapes the tensor-core scans take: 64-unit slices per CTA (clusters of H/64), 16-row batch tiles.  bf16x3 needs hi/lo
 // weight pairs, which fit the 227 KB of shared memory per block up to H = 256; bf16 goes to H = 512.  The batch multiples
@@ -131,10 +163,9 @@ static int tc_plan_check(const bigru_plan& p) {
     return BIGRU_OK;
 }
 
-// GEMMs of a plan: FFMA on the fp32 path, tensor cores (bf16 or split bf16x3 operands) on the others
-static int plan_gemm(const bigru_plan& p, const GemmArgs& g, int cls, float* scratch, cudaStream_t st) {
-    return p.prec == BIGRU_PREC_FP32 ? sgemm_launch(g, st)
-                                     : tc_gemm_launch(g, p.prec, cls, reinterpret_cast<htc::bf16_t*>(scratch + scratch_layout(p).tcw), st);
+// GEMMs of a plan: FFMA on the fp32 path, tensor cores (bf16 or split bf16x3 operands, packed into tcw) on the others
+static int plan_gemm(const bigru_plan& p, const GemmArgs& g, int cls, htc::bf16_t* tcw, cudaStream_t st) {
+    return p.prec == BIGRU_PREC_FP32 ? sgemm_launch(g, st) : tc_gemm_launch(g, p.prec, cls, tcw, st);
 }
 
 // planes [depth][rows][pitch] at float offset off of buf (lo follows hi at bf16x3)
@@ -143,12 +174,12 @@ static Planes plan_planes(const bigru_plan& p, const float* buf, int64_t off, in
     const htc::bf16_t* hi = reinterpret_cast<const htc::bf16_t*>(buf + off);
     return Planes{hi, p.prec == BIGRU_PREC_BF16X3 ? hi + depth * rows * pitch : nullptr, cols, rows, depth, pitch};
 }
-// the layer input's planes as the projection and dW_ih read them: its own (layer 0, dropout) or the previous layer's Y
-static Planes input_planes(const bigru_plan& p, const float* stash, int l, bool own) {
-    const StashF32 S = stash_layout(p);
+// the layer input's planes at `planes` as the projection and dW_ih read them: its own (layer 0, dropout) or the previous
+// layer's Y planes
+static Planes input_planes(const bigru_plan& p, const float* planes, int l, bool own) {
     const int64_t BT = (int64_t)p.B * p.T;
-    return own ? plan_planes(p, stash, S.XP[l], p.in_size(l), BT, 1, in_pitch(p, l))
-               : plan_planes(p, stash, S.YP[l - 1], (int64_t)p.D * p.H, BT, 1, (int64_t)p.D * p.H);
+    return own ? plan_planes(p, planes, 0, p.in_size(l), BT, 1, in_pitch(p, l))
+               : plan_planes(p, planes, 0, (int64_t)p.D * p.H, BT, 1, (int64_t)p.D * p.H);
 }
 static htc::bf16_t* mut(const Planes& q) { return const_cast<htc::bf16_t*>(q.hi); }
 static htc::bf16_t* mut_lo(const Planes& q) { return const_cast<htc::bf16_t*>(q.lo); }
@@ -228,15 +259,48 @@ static inline unsigned nblk(int64_t n, int bs) { return (unsigned)cdiv64(n, bs);
 // ------------------------------------------------------------------------------------------
 // forward (all precisions share the layout; the recurrence and the GEMMs run on tensor cores except at fp32)
 // ------------------------------------------------------------------------------------------
+// Where one forward reads and writes, per layer.  The training forward keeps everything in the stash for the backward
+// (train_bufs); inference keeps only what the next layer and the head read (infer_bufs).  A null Y, G or YP: that output is
+// not written.  X (dropped input) and XP (planes of a layer's own input) are read only where the forward writes them.
+struct FwdBufs {
+    float *gi, *gh, *cat, *arg;
+    htc::bf16_t* tcw;
+    float *X[16], *Y[16], *G[16], *XP[16], *YP[16];
+};
+static FwdBufs train_bufs(const bigru_plan& p, float* stash, float* scratch) {
+    const StashF32 S = stash_layout(p);
+    const ScratchF32 W = scratch_layout(p);
+    FwdBufs b{};
+    b.gi = scratch + W.gi; b.gh = scratch + W.gh; b.cat = stash + S.cat; b.arg = stash + S.arg;
+    b.tcw = reinterpret_cast<htc::bf16_t*>(scratch + W.tcw);
+    for (int l = 0; l < p.L; ++l) {
+        b.X[l] = stash + S.X[l]; b.Y[l] = stash + S.Y[l]; b.G[l] = stash + S.G[l];
+        b.XP[l] = stash + S.XP[l]; b.YP[l] = stash + S.YP[l];
+    }
+    return b;
+}
+static FwdBufs infer_bufs(const bigru_plan& p, float* ws) {
+    const InferF32 I = infer_layout(p);
+    const bool tc = p.prec != BIGRU_PREC_FP32;
+    FwdBufs b{};
+    b.gi = ws + I.gi; b.gh = ws + I.gh; b.cat = ws + I.cat; b.arg = ws + I.arg;
+    b.tcw = reinterpret_cast<htc::bf16_t*>(ws + I.tcw);
+    b.XP[0] = ws + I.xp;
+    for (int l = 0; l < p.L; ++l) {
+        const bool top = l == p.L - 1;
+        b.Y[l] = !tc ? ws + I.y[l % 2] : top ? ws + I.y[0] : nullptr;
+        b.YP[l] = tc && !top ? ws + I.yp[l % 2] : nullptr;
+    }
+    return b;
+}
+
 static int forward_plan(const bigru_plan& p, const float* params, const float* x, const float* h0, float drop,
-                        int spatial, int training, uint64_t seed, float* stash, float* scratch, float* logits,
-                        float* hn, cudaStream_t st) {
+                        int spatial, int training, uint64_t seed, const FwdBufs& buf, float* logits, float* hn,
+                        cudaStream_t st) {
     if (p.prec == BIGRU_PREC_BF16 && h0) {
         bigru_set_error("BIGRU_PREC_BF16: an initial hidden state is not supported; use BIGRU_PREC_FP32 or BIGRU_PREC_BF16X3");
         return BIGRU_ERR_UNSUPPORTED;
     }
-    const StashF32 S = stash_layout(p);
-    const ScratchF32 W = scratch_layout(p);
     const int B = p.B, T = p.T, H = p.H, D = p.D;
     const int64_t BT = (int64_t)B * T;
     const bool do_drop = training && drop > 0.f;
@@ -245,40 +309,43 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
         const int I = (int)p.in_size(l);
         if (do_drop && (l == 0 || p.L > 1)) {
             // l == 0: input dropout (elementwise or per-channel); l > 0: nn.GRU inter-layer dropout
-            float* xd = stash + S.X[l];
+            float* xd = buf.X[l];
             KLAUNCH(KC_MISC, 0.0, 0.0, st, dropout_kernel<<<132 * 8, 256, 0, st>>>(inp, xd, BT * I, T, I, l == 0 ? spatial : 0, drop, seed, (uint32_t)l));
             inp = xd;
         }
-        float* Y = stash + S.Y[l];
-        float* G = stash + S.G[l];
+        float* Y = buf.Y[l];
+        float* G = buf.G[l];
         const float* h0l = h0 ? h0 + (int64_t)l * D * B * H : nullptr;
         float* hnl = hn ? hn + (int64_t)l * D * B * H : nullptr;
         if (p.prec != BIGRU_PREC_FP32) {
             const bool own = l == 0 || do_drop;
-            const Planes xp = input_planes(p, stash, l, own);
+            const Planes xp = input_planes(p, own ? buf.XP[l] : buf.YP[l - 1], l, own);
             if (own)
                 KLAUNCH(KC_PACK, 0.0, 0.0, st, htc::to_planes_kernel<<<132 * 8, 256, 0, st>>>(inp, BT, I, (int)xp.pitch, mut(xp), mut_lo(xp)));
             // gi[d] = X W_ih[d]^T + b_ih[d]   for both directions
             Planes wp;
-            TRY(tc_pack(params + p.off_wih(l, 0), I, 1, p.ld_block(l), 3 * H, I, D, p.prec, reinterpret_cast<htc::bf16_t*>(scratch + W.tcw),
-                        &wp, st));
+            TRY(tc_pack(params + p.off_wih(l, 0), I, 1, p.ld_block(l), 3 * H, I, D, p.prec, buf.tcw, &wp, st));
             {
                 ProfScope ps(KC_TC_GEMM, 2.0 * BT * 3 * H * (double)I * D, 0.0, st);
-                htc::WgJob j = wg_job(scratch + W.gi, (int)BT, 3 * H, 3 * H, D, cdiv64(I, htc::WG_BK));
+                htc::WgJob j = wg_job(buf.gi, (int)BT, 3 * H, 3 * H, D, cdiv64(I, htc::WG_BK));
                 j.bias = params + p.off_bih(l, 0); j.zBias = p.ld_block(l); j.zC = BT * 3 * H;
                 j.b.zsel = 1;
                 TRY(wg_gemm(j, xp, false, wp, false, p.prec, st));
             }
-            const Planes yp = plan_planes(p, stash, S.YP[l], (int64_t)D * H, BT, 1, (int64_t)D * H);
-            TRY(tc_scan_fwd(p, l, scratch + W.gi, params + p.off_whh(l, 0), params + p.off_bhh(l, 0), h0l, Y, G, hnl, mut(yp), mut_lo(yp), st));
+            htc::bf16_t *yh = nullptr, *yl = nullptr;
+            if (buf.YP[l]) {
+                const Planes yp = plan_planes(p, buf.YP[l], 0, (int64_t)D * H, BT, 1, (int64_t)D * H);
+                yh = mut(yp); yl = mut_lo(yp);
+            }
+            TRY(tc_scan_fwd(p, l, buf.gi, params + p.off_whh(l, 0), params + p.off_bhh(l, 0), h0l, Y, G, hnl, yh, yl, st));
             inp = Y;
             continue;
         }
         // gi[d] = X W_ih[d]^T + b_ih[d]   for both directions
-        GemmArgs g = gemm_args(inp, params + p.off_wih(l, 0), scratch + W.gi, (int)BT, 3 * H, I, I, 1, I, 1, 3 * H);
+        GemmArgs g = gemm_args(inp, params + p.off_wih(l, 0), buf.gi, (int)BT, 3 * H, I, I, 1, I, 1, 3 * H);
         g.bias = params + p.off_bih(l, 0);
         g.batch = D; g.zA = 0; g.zB = p.ld_block(l); g.zBias = p.ld_block(l); g.zC = BT * 3 * H;
-        TRY(plan_gemm(p, g, KC_TC_GEMM, scratch, st));
+        TRY(plan_gemm(p, g, KC_TC_GEMM, buf.tcw, st));
         for (int s = 0; s < T; ++s) {
             // gh[d] = h_prev[d] W_hh[d]^T + b_hh[d];  h_prev rows live in Y (or h0 at s == 0)
             const float* hp; int64_t sam, zA;
@@ -289,7 +356,7 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
                 sam = (int64_t)T * D * H;
                 zA = D == 2 ? ((int64_t)(T - s) - (s - 1)) * D * H + H : 0;
             }
-            GemmArgs r = gemm_args(hp, params + p.off_whh(l, 0), scratch + W.gh, B, 3 * H, hp ? H : 0, sam, 1, H, 1, 3 * H);
+            GemmArgs r = gemm_args(hp, params + p.off_whh(l, 0), buf.gh, B, 3 * H, hp ? H : 0, sam, 1, H, 1, 3 * H);
             r.bias = params + p.off_bhh(l, 0);
             r.batch = D; r.zA = zA; r.zB = p.ld_block(l); r.zBias = p.ld_block(l); r.zC = (int64_t)B * 3 * H;
             if (hp) { TRY(sgemm_launch(r, st)); }
@@ -299,16 +366,15 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
                 r.mask_period = 1; r.mask_skip = 0;                           // every k masked -> pure bias
                 TRY(sgemm_launch(r, st));
             }
-            KLAUNCH(KC_GATES_FWD, 0.0, 0.0, st, gru_gates_fwd_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(scratch + W.gi, scratch + W.gh, h0l, Y, G,
+            KLAUNCH(KC_GATES_FWD, 0.0, 0.0, st, gru_gates_fwd_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(buf.gi, buf.gh, h0l, Y, G,
                                                                               hnl, B, T, H, D, s));
         }
         inp = Y;
     }
-    const float* Ytop = stash + S.Y[p.L - 1];
-    KLAUNCH(KC_HEAD, 0.0, 0.0, st, head_pool_kernel<<<nblk((int64_t)B * H, 128), 128, 0, st>>>(Ytop, stash + S.cat, (int*)(stash + S.arg), B, T, H, D));
-    GemmArgs lin = gemm_args(stash + S.cat, params + p.off_linw(), logits, B, p.C, 3 * H, 3 * H, 1, 3 * H, 1, p.C);
+    KLAUNCH(KC_HEAD, 0.0, 0.0, st, head_pool_kernel<<<nblk((int64_t)B * H, 128), 128, 0, st>>>(buf.Y[p.L - 1], buf.cat, (int*)buf.arg, B, T, H, D));
+    GemmArgs lin = gemm_args(buf.cat, params + p.off_linw(), logits, B, p.C, 3 * H, 3 * H, 1, 3 * H, 1, p.C);
     lin.bias = params + p.off_linb();
-    TRY(plan_gemm(p, lin, KC_HEAD, scratch, st));
+    TRY(plan_gemm(p, lin, KC_HEAD, buf.tcw, st));
     return BIGRU_OK;
 }
 
@@ -329,12 +395,13 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
     const bool do_drop = training && drop > 0.f;
     const bool tc = p.prec != BIGRU_PREC_FP32;
     float* dhc = scratch + W.dhc;
+    htc::bf16_t* tcw = reinterpret_cast<htc::bf16_t*>(scratch + W.tcw);
     CUDA_TRY(cudaMemsetAsync(grads, 0, sizeof(float) * p.nparams, st));
     // head: dcat = dlogits lin_w ; dlin_w = dlogits^T cat ; dlin_b = colsum(dlogits)
     GemmArgs a = gemm_args(dlogits, params + p.off_linw(), scratch + W.dcat, B, 3 * H, C, C, 1, 1, 3 * H, 3 * H);
-    TRY(plan_gemm(p, a, KC_HEAD, scratch, st));
+    TRY(plan_gemm(p, a, KC_HEAD, tcw, st));
     GemmArgs w = gemm_args(dlogits, stash + S.cat, grads + p.off_linw(), C, 3 * H, B, 1, C, 1, 3 * H, 3 * H);
-    TRY(plan_gemm(p, w, KC_HEAD, scratch, st));
+    TRY(plan_gemm(p, w, KC_HEAD, tcw, st));
     TRY(colsum_launch(dlogits, grads + p.off_linb(), B, C, C, 1, 0, 0, scratch + W.csum, st));
     KLAUNCH(KC_HEAD, 0.0, 0.0, st, head_bwd_dy_kernel<<<nblk(BT * H, 256), 256, 0, st>>>(scratch + W.dcat, (const int*)(stash + S.arg), scratch + W.dYa, dhc, B, T, H, D));
     for (int l = p.L - 1; l >= 0; --l) {
@@ -378,7 +445,8 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
                 htc::WgJob j = wg_job(grads + p.off_wih(l, 0), (int)H3, I, I, D, kb);
                 j.zC = p.ld_block(l); j.a.zsel = 1; j.part = part;
                 j.splits = wg_splits(cdiv64(H3, htc::WG_BM) * cdiv64(I, htc::WG_BN) * D, kb);
-                TRY(wg_gemm(j, gip, true, input_planes(p, stash, l, l == 0 || do_drop), true, p.prec, st));
+                const bool own = l == 0 || do_drop;
+                TRY(wg_gemm(j, gip, true, input_planes(p, stash + (own ? S.XP[l] : S.YP[l - 1]), l, own), true, p.prec, st));
             }
             // the dgh planes are zero at each sequence's first step, so the ±1-row shift needs no mask
             if (T > 1) {
@@ -417,7 +485,7 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
                 GemmArgs w0 = gemm_args(dgh_d + (int64_t)tf * 3 * H, h0l + (int64_t)d * B * H, grads + p.off_whh(l, d),
                                         3 * H, H, B, 1, (int64_t)T * 3 * H, 1, H, H);
                 w0.beta = 1;
-                TRY(plan_gemm(p, w0, KC_TC_GEMM_DWHH, scratch, st));
+                TRY(plan_gemm(p, w0, KC_TC_GEMM_DWHH, tcw, st));
             }
             TRY(colsum_launch(dgi_d, grads + p.off_bih(l, d), BT, 3 * H, 3 * H, 1, 0, 0, scratch + W.csum, st));
             TRY(colsum_launch(dgh_d, grads + p.off_bhh(l, d), BT, 3 * H, 3 * H, 1, 0, 0, scratch + W.csum, st));
@@ -428,8 +496,7 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
         if (tc) {
             // one K loop over direction 0, then direction 1
             Planes wp;
-            TRY(tc_pack(params + p.off_wih(l, 0), 1, I, p.ld_block(l), I, 3 * H, D, p.prec, reinterpret_cast<htc::bf16_t*>(scratch + W.tcw),
-                        &wp, st));
+            TRY(tc_pack(params + p.off_wih(l, 0), 1, I, p.ld_block(l), I, 3 * H, D, p.prec, tcw, &wp, st));
             ProfScope ps(KC_TC_GEMM_DX, 2.0 * BT * I * (double)H3 * D, 0.0, st);
             htc::WgJob j = wg_job(dxo, (int)BT, I, I, 1, D * (H3 / htc::WG_BK));
             j.kbd = (int)(H3 / htc::WG_BK); j.kcat = 1; j.a.zsel = 1; j.b.zsel = 1;
@@ -460,8 +527,25 @@ extern "C" int bigru_forward(const bigru_plan* plan, const float* d_params, cons
         return BIGRU_ERR_ARG;
     }
     if (dropout_p < 0.f || dropout_p >= 1.f) { bigru_set_error("forward: dropout_p must be in [0,1)"); return BIGRU_ERR_ARG; }
-    return forward_plan(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, (float*)d_stash,
-                        (float*)d_scratch, d_logits, d_hn, (cudaStream_t)stream);
+    return forward_plan(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed,
+                        train_bufs(*plan, (float*)d_stash, (float*)d_scratch), d_logits, d_hn, (cudaStream_t)stream);
+}
+
+extern "C" int bigru_infer_workspace_bytes(const bigru_plan* p, size_t* bytes) {
+    if (!p || !bytes) { bigru_set_error("infer_workspace_bytes: null argument"); return BIGRU_ERR_ARG; }
+    *bytes = (size_t)infer_layout(*p).total * sizeof(float);
+    return BIGRU_OK;
+}
+
+// the eval-mode forward through the same launch sequence as bigru_forward, with the outputs placed by infer_layout
+extern "C" int bigru_infer(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
+                           void* d_workspace, float* d_logits, void* stream) {
+    if (!plan || !d_params || !d_x || !d_workspace || !d_logits) {
+        bigru_set_error("infer: null argument");
+        return BIGRU_ERR_ARG;
+    }
+    return forward_plan(*plan, d_params, d_x, d_h0, 0.f, 0, 0, 0, infer_bufs(*plan, (float*)d_workspace), d_logits, nullptr,
+                        (cudaStream_t)stream);
 }
 
 extern "C" int bigru_backward(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,

@@ -170,7 +170,7 @@ static int colsum_launch(const float* A, float* out, int64_t rows, int cols, int
 // ------------------------------------------------------------------------------------------
 // GRU pointwise: forward gates for one time step of both directions.
 //   gi [D][B*T][3H] (input projection + b_ih), gh [D][B][3H] (h_prev W_hh^T + b_hh)
-//   Y [B][T][D*H] layer output; G [D][B*T][4H] stash of (r, z, n, gh_n)
+//   Y [B][T][D*H] layer output; G [D][B*T][4H] stash of (r, z, n, gh_n), null when no backward follows (inference)
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.f / (1.f + expf(-x)); }
 
@@ -196,8 +196,10 @@ __global__ void gru_gates_fwd_kernel(const float* __restrict__ gi, const float* 
     const float n = tanhf(gir[2 * H + j] + r * hn);
     const float h = (1.f - z) * n + z * hp;
     Y[row * D * H + d * H + j] = h;
-    float* g = G + ((int64_t)d * B * T + row) * 4 * H;
-    g[j] = r; g[H + j] = z; g[2 * H + j] = n; g[3 * H + j] = hn;
+    if (G) {
+        float* g = G + ((int64_t)d * B * T + row) * 4 * H;
+        g[j] = r; g[H + j] = z; g[2 * H + j] = n; g[3 * H + j] = hn;
+    }
     if (hn_out && s == T - 1) hn_out[((int64_t)d * B + b) * H + j] = h;
 }
 

@@ -341,8 +341,13 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ part, int splits,
 // read them.
 // Grid (CS, B/16, D), cluster (CS, 1, 1), 256 threads.  Warp w owns units 16*(w/2) .. +16 of the CTA's slice and batch
 // columns 8*(w%2) .. +8: its r, z and n accumulators hold the same (unit, column) pairs, so the gate math needs no exchange.
+// OUT selects at compile time which of Y, G and the Y planes are written (hn_out is written whenever it is non-null): the
+// training forward keeps all three for the backward; inference writes the planes of a lower layer (the next projection reads
+// them) and the fp32 Y of the top layer (the pooling head reads it).  The h arithmetic is the same in every instantiation.
 // ------------------------------------------------------------------------------------------------------
 constexpr int SCAN_U = 64, SCAN_NB = 16, SCAN_THREADS = 256;
+constexpr int SCAN_Y = 1, SCAN_G = 2, SCAN_PLANES = 4;
+constexpr int SCAN_TRAIN = SCAN_Y | SCAN_G | SCAN_PLANES, SCAN_INFER_LOWER = SCAN_PLANES, SCAN_INFER_TOP = SCAN_Y;
 
 template <int H, int NS>
 struct FwdSmem {
@@ -353,7 +358,7 @@ struct FwdSmem {
     static constexpr int TOTAL = NH * WBYTES + 2 * NH * HBYTES;
 };
 
-template <int H, int NS>
+template <int H, int NS, int OUT>
 __global__ void __launch_bounds__(SCAN_THREADS, 1)
 gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh, const float* __restrict__ bhh, int64_t zW,
                     const float* __restrict__ h0, float* __restrict__ Y, float* __restrict__ G, float* __restrict__ hn_out,
@@ -452,9 +457,11 @@ gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh,
             const float h = (1.f - z) * n + z * hp[e];
             hp[e] = h;
             const int64_t row = (int64_t)b * T + t;
-            Y[row * DH + d * H + j] = h;
-            float* gs = G + ((int64_t)d * B * T + row) * 4 * H + j;
-            gs[0] = r; gs[H] = z; gs[2 * H] = n; gs[3 * H] = hnv;
+            if (OUT & SCAN_Y) Y[row * DH + d * H + j] = h;
+            if (OUT & SCAN_G) {
+                float* gs = G + ((int64_t)d * B * T + row) * 4 * H + j;
+                gs[0] = r; gs[H] = z; gs[2 * H] = n; gs[3 * H] = hnv;
+            }
             if (hn_out && s == T - 1) hn_out[((int64_t)d * B + b) * H + j] = h;
             bf16_t hi, lo;
             split_bf16(h, hi, lo);
@@ -470,10 +477,12 @@ gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh,
         cluster_wait();
         // the Y planes of this CTA's units: h_t is now in the h tile (hi / lo, every unit), so copy the own slice out with
         // 16-byte stores.  Nobody writes this buffer again before the next step's barrier.
-        for (int i = tid; i < NH * SCAN_NB * (U / 8); i += SCAN_THREADS) {
-            const int h = i / (SCAN_NB * U / 8), r = (i / (U / 8)) % SCAN_NB, k = c * U + (i % (U / 8)) * 8;
-            const uint4 v = *reinterpret_cast<const uint4*>(Hsm + (nbuf * NH + h) * S::HBYTES + swz<H * 2>(r, k));
-            *reinterpret_cast<uint4*>((h ? yl : yh) + ((int64_t)(bt0 + r) * T + t) * DH + d * H + k) = v;
+        if (OUT & SCAN_PLANES) {
+            for (int i = tid; i < NH * SCAN_NB * (U / 8); i += SCAN_THREADS) {
+                const int h = i / (SCAN_NB * U / 8), r = (i / (U / 8)) % SCAN_NB, k = c * U + (i % (U / 8)) * 8;
+                const uint4 v = *reinterpret_cast<const uint4*>(Hsm + (nbuf * NH + h) * S::HBYTES + swz<H * 2>(r, k));
+                *reinterpret_cast<uint4*>((h ? yl : yh) + ((int64_t)(bt0 + r) * T + t) * DH + d * H + k) = v;
+            }
         }
     }
 }
@@ -819,13 +828,31 @@ static int launch_cluster(void (*kernel)(KArgs...), int cs, int ntiles, int D, i
     return BIGRU_OK;
 }
 
-// one layer's forward recurrence; shapes were validated by the plan (H in {128, 256, 512}, B % 16 == 0)
+template <int HH, int NS>
+static int scan_fwd_launch(int out, int cs, int nt, int D, cudaStream_t st, const float* gi, const float* Whh, const float* bhh,
+                           int64_t zW, const float* h0, float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, int B, int T) {
+    constexpr int smem = htc::FwdSmem<HH, NS>::TOTAL;
+    switch (out) {
+        case htc::SCAN_TRAIN:
+            return launch_cluster(htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_TRAIN>, cs, nt, D, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D);
+        case htc::SCAN_INFER_LOWER:
+            return launch_cluster(htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_INFER_LOWER>, cs, nt, D, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D);
+        case htc::SCAN_INFER_TOP:
+            return launch_cluster(htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_INFER_TOP>, cs, nt, D, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D);
+    }
+    bigru_set_error("tc_scan_fwd: no kernel writes this set of outputs (Y %d, G %d, planes %d)", Y != nullptr, G != nullptr, yh != nullptr);
+    return BIGRU_ERR_ARG;
+}
+
+// one layer's forward recurrence; shapes were validated by the plan (H in {128, 256, 512}, B % 16 == 0).  A null Y, G or yh:
+// that output is not written (the instantiations: all three, planes only, Y only)
 static int tc_scan_fwd(const bigru_plan& p, int l, const float* gi, const float* Whh, const float* bhh, const float* h0,
                        float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, cudaStream_t st) {
     const int H = p.H, D = p.D, B = p.B, T = p.T, cs = H / htc::SCAN_U, nt = B / htc::SCAN_NB;
     const int64_t zW = p.ld_block(l);
+    const int out = (Y ? htc::SCAN_Y : 0) | (G ? htc::SCAN_G : 0) | (yh ? htc::SCAN_PLANES : 0);
     ProfScope ps(KC_TC_SCAN_FWD, 2.0 * D * B * (double)T * 3 * H * H, 0.0, st);
-#define FWD(HH, NS) return launch_cluster(htc::gru_scan_fwd_kernel<HH, NS>, cs, nt, D, htc::FwdSmem<HH, NS>::TOTAL, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D)
+#define FWD(HH, NS) return scan_fwd_launch<HH, NS>(out, cs, nt, D, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T)
     if (p.prec == BIGRU_PREC_BF16X3) {
         if (H == 128) FWD(128, 3);
         if (H == 256) FWD(256, 3);

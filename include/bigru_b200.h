@@ -91,6 +91,16 @@ int  bigru_forward(const bigru_plan* plan, const float* d_params, const float* d
                    float dropout_p, int spatial, int training, uint64_t seed,
                    void* d_stash, void* d_scratch, float* d_logits, float* d_hn, void* stream);
 
+/* --- eval-mode BiGRU.forward (no dropout, nothing kept for a backward): logits of the plan's batch (evaluate_model,
+ *  biGRU_model.py:227-286).  Same plans, precisions, shape rules and d_h0 rules as bigru_forward (d_h0 at BIGRU_PREC_BF16:
+ *  BIGRU_ERR_UNSUPPORTED), and bit-identical logits: the same launch sequence and kernels, with the scans writing only what
+ *  the next layer and the head read.  d_workspace: bigru_infer_workspace_bytes(plan) bytes; neither the stash nor the
+ *  scratch of bigru_forward is used.  At configs[1] bf16x3 (B512 T128 F64 H256 L2) that is about 0.69 GB against
+ *  1915 + 2329 MB of stash + scratch. */
+int  bigru_infer_workspace_bytes(const bigru_plan* plan, size_t* bytes);
+int  bigru_infer(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
+                 void* d_workspace, float* d_logits, void* stream);
+
 /* --- loss.backward() through the model (biGRU_model.py:204): every parameter gradient into
  *  d_grads (flat, overwritten), optional d_dx[B,T,F] and d_dh0[L*D,B,H].  d_x (required) is the
  *  input the forward read.  Must follow bigru_forward on the same plan/stash with the same dropout arguments. */
