@@ -4,6 +4,7 @@ The reference builds its technical-indicator columns and the four target labels 
 joined table (``create_database.py:76-190``) and joins them back in a fixed column order (``create_database.py:239-256``).
 ``window_features`` computes the same columns from device tensors with one row-parallel CUDA kernel
 (``bigru_window_features``), for bulk back-fills where the table already lives on the GPU.  SQL ``NULL`` is ``NaN``.
+A NULL inside an input column differs from SQL: AVG skips it, while the kernel's NaN propagates into every frame holding it.
 Argument names follow ``config.py:40-49`` of the reference.  There is no CPU fallback."""
 from __future__ import annotations
 

@@ -154,7 +154,8 @@ int  bigru_chunk_minmax(const float* d_table, int64_t N, int F, int64_t row_lo, 
  *  [stoch] (15-row MIN / MAX of close; NaN = SQL NULL when max == min), ATR (15-row AVG(high - low)), price_change
  *  (close - LAG(close, 1); NaN on the first row) -> d_out[n][n_out]; and the four targets up1, up2, down1, down2
  *  (create_database.py:163-185: LEAD(close, 8 / 15) against close +- n1 / n2 * ATR, 0 where the lead is NULL)
- *  -> d_targets[n][4] (nullable).  At most 8 periods per list.  Returns n_out through *n_out (pass d_out = NULL to query). */
+ *  -> d_targets[n][4] (nullable), decided as the SQL decides them in double, ties included.  n1 and n2 are fp32: the
+ *  reference's 1.5 and 3 are exact, other factors are rounded to fp32 first.  At most 8 periods per list.  Returns n_out through *n_out (pass d_out = NULL to query). */
 int  bigru_window_features(const float* d_close, const float* d_high, const float* d_low, const float* d_volume,
                            const float* d_delta, int64_t n, const int* vol_periods, int n_vol, const int* price_periods,
                            int n_price, const int* delta_periods, int n_delta, int bb_period, float bb_std,

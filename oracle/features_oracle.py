@@ -13,10 +13,19 @@ PINNED to the reference's own SQL: tests/golden/make_features_golden.py imports 
 `mysql.connector` stub that forwards its statements to sqlite3 (window functions; MariaDB's STD registered as a window
 aggregate), fills the table with a seed-fixed synthetic market and stores what the reference's views return in
 tests/golden/features.npz; tests/test_oracle_cpu.py checks this restatement against it (exact) and, independently,
-against pandas.rolling and hand-computed rows."""
+against pandas.rolling and hand-computed rows.  tests/golden/features_ties.npz is the same check on a quarter-point tick
+grid, where the move to row i + 8 / i + 15 often equals n1 / n2 * ATR exactly.
+
+Exactness: every frame is summed on its own with math.fsum (the correctly rounded sum; a running cumsum loses its low bits
+on long tables) and then divided by the row count, as SQL's AVG does.  The targets compare close[i + h] with
+close[i] +- n * ATR in double, in the SQL's order of operations.  So on a tick grid, where the sums are exact, the labels
+equal the SQL's at ties as well."""
 from __future__ import annotations
 
+import math
+
 import numpy as np
+from numpy.lib.stride_tricks import sliding_window_view
 
 
 def _frames(n, w):
@@ -24,28 +33,56 @@ def _frames(n, w):
     return np.maximum(0, i - w + 1), i
 
 
-def rolling_mean(x, w):
+def _head_and_body(x, w):
+    """The clipped frames of the first min(w - 1, n) rows as lists, and the full frames after them as a [n - w + 1, w] view."""
     x = np.asarray(x, dtype=np.float64)
-    cs = np.concatenate([[0.0], np.cumsum(x)])
+    h = min(w - 1, len(x))
+    head = [x[:i + 1] for i in range(h)]
+    body = sliding_window_view(x, w) if len(x) >= w else np.zeros((0, w))
+    return head, body
+
+
+def _chunks(body, elems=1 << 20):
+    """(first row, rows) of the [n - w + 1, w] frame view in pieces of about `elems` values, so that no list or
+    temporary of the whole view is built (w = 4096 over 20,000 rows would be 65M values)."""
+    step = max(1, elems // max(1, body.shape[1]))
+    for r in range(0, len(body), step):
+        yield r, body[r:r + step]
+
+
+def rolling_sum(x, w):
+    """Correctly rounded sum of every frame [max(0, i - w + 1), i]."""
+    head, body = _head_and_body(x, w)
+    out = [math.fsum(f.tolist()) for f in head]
+    for _, rows in _chunks(body):
+        out += [math.fsum(f) for f in rows.tolist()]
+    return np.array(out, dtype=np.float64)
+
+
+def rolling_mean(x, w):
     lo, hi = _frames(len(x), w)
-    return (cs[hi + 1] - cs[lo]) / (hi - lo + 1)
+    return rolling_sum(x, w) / (hi - lo + 1)
 
 
 def rolling_std_pop(x, w):
+    """Population standard deviation of every frame, two-pass around the frame's exact mean: no cancellation."""
     x = np.asarray(x, dtype=np.float64)
+    m = rolling_mean(x, w)
+    head, body = _head_and_body(x, w)
     out = np.empty(len(x))
-    for i in range(len(x)):                      # two-pass per frame: no cancellation
-        f = x[max(0, i - w + 1): i + 1]
-        out[i] = np.sqrt(np.mean((f - f.mean()) ** 2))
+    for i, f in enumerate(head):
+        out[i] = np.sqrt(np.mean((f - m[i]) ** 2))
+    for r, rows in _chunks(body):
+        i = len(head) + r
+        out[i:i + len(rows)] = np.sqrt(np.mean((rows - m[i:i + len(rows), None]) ** 2, axis=1))
     return out
 
 
 def rolling_minmax(x, w):
     x = np.asarray(x, dtype=np.float64)
-    mn, mx = np.empty(len(x)), np.empty(len(x))
-    for i in range(len(x)):
-        f = x[max(0, i - w + 1): i + 1]
-        mn[i], mx[i] = f.min(), f.max()
+    head, body = _head_and_body(x, w)
+    mn = np.array([f.min() for f in head] + [v for _, rows in _chunks(body) for v in rows.min(axis=1)], dtype=np.float64)
+    mx = np.array([f.max() for f in head] + [v for _, rows in _chunks(body) for v in rows.max(axis=1)], dtype=np.float64)
     return mn, mx
 
 
@@ -74,11 +111,10 @@ def window_features(close, high, low, volume=None, delta=None, volume_MA_periods
     cols.append(pc)
     feats = np.stack(cols, axis=1) if n else np.zeros((0, len(cols)))
     tgt = np.zeros((n, 4))
-    for i in range(n):
-        if i + 8 < n:
-            tgt[i, 0] = close[i + 8] >= close[i] + n1 * atr[i]
-            tgt[i, 2] = close[i + 8] <= close[i] - n1 * atr[i]
-        if i + 15 < n:
-            tgt[i, 1] = close[i + 15] >= close[i] + n2 * atr[i]
-            tgt[i, 3] = close[i + 15] <= close[i] - n2 * atr[i]
+    n1, n2 = float(n1), float(n2)
+    for h, n_atr, up, down in ((8, n1, 0, 2), (15, n2, 1, 3)):       # p_h >= p0 + (n * ATR), p_h <= p0 - (n * ATR); NULL -> 0
+        if n > h:
+            p0, ph, a = close[:-h], close[h:], n_atr * atr[:-h]
+            tgt[:-h, up] = ph >= p0 + a
+            tgt[:-h, down] = ph <= p0 - a
     return feats, tgt

@@ -8,8 +8,13 @@ script imports the UNMODIFIED module with
     a digit get quoted, DESCRIBE -> PRAGMA table_info, a bare `Timestamp` in the window order of the two-table `target` view
     is qualified, and MariaDB's STD() = population standard deviation is registered as a sqlite window aggregate),
   * a stub `pytz` (config.py imports it; nothing on this path uses it),
-fills `stock_data_joined` with a seed-fixed synthetic market table (values exactly representable in the FLOAT(6,2) / INT
-columns the reference declares) and selects every view plus the `target` view.  Output: tests/golden/features.npz.
+fills `stock_data_joined` with a seed-fixed synthetic market table and selects every view plus the `target` view.  It does
+this for two tables and writes two files:
+  * tests/golden/features.npz: 400 rows on a cent grid near 300 (values exactly representable in the FLOAT(6,2) / INT
+    columns the reference declares);
+  * tests/golden/features_ties.npz: 8,000 rows on a quarter-point grid near 3000 (an index future's tick), every price
+    exact in fp32.  On this grid sqlite's window AVG is exact, and the move to row i + 8 / i + 15 often equals
+    n1 / n2 * ATR exactly, so the file pins the labels the reference's double arithmetic gives at exact ties.
 
 Run in the build container:  python tests/golden/make_features_golden.py
 """
@@ -23,7 +28,7 @@ import types
 import numpy as np
 
 REF = "/root/reference"
-OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "features.npz")
+HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 class _Std:
@@ -113,21 +118,32 @@ def synthetic_table(n, seed=7):
     return f32(close), f32(high), f32(low), f32(volume), f32(delta)
 
 
-def main():
-    db = sqlite3.connect(":memory:")
-    db.create_window_function("STD", 1, _Std)
-    cur = _install_stubs(db)
-    sys.path.insert(0, REF)
-    import create_database as ref                                   # the UNMODIFIED reference module: creates table + views
-    import config
-    table = config.mysql_table_name
-    n = 400
-    close, high, low, volume, delta = synthetic_table(n)
+def tick_table(n, seed=11, tick=0.25):
+    """Quarter-point steps of round(N(0, 3)) ticks from 3000, high / low 1-5 ticks either side, and a flat stretch."""
+    rng = np.random.default_rng(seed)
+    close = 3000 + tick * np.cumsum(np.round(rng.normal(0, 3, n)))
+    close[500:530] = close[500]                                    # stochastic max == min -> NULL
+    high = close + tick * rng.integers(1, 6, n)
+    low = close - tick * rng.integers(1, 6, n)
+    volume = rng.integers(1, 5000, n)
+    delta = rng.integers(-2000, 2000, n)
+    f32 = lambda a: np.asarray(a, np.float32)
+    cols = f32(close), f32(high), f32(low), f32(volume), f32(delta)
+    assert all(np.array_equal(c.astype(np.float64), a) for c, a in zip(cols, (close, high, low, volume, delta)))
+    return cols
+
+
+
+def reference_views(db, config, table, cols):
+    """Replaces the rows of `table` with `cols` and returns (features, targets) as the reference's views select them."""
+    close, high, low, volume, delta = cols
+    n = len(close)
+    db.execute(f"DELETE FROM {table}")
     names = [r[1] for r in db.execute(f"PRAGMA table_info({table})")]
     special = {"4_close": close, "2_high": high, "3_low": low, "5_volume": volume, "delta": delta}
     rows = []
     for i in range(n):
-        ts = "2020-01-{:02d} {:02d}:{:02d}:00".format(2 + i // 200, 9 + (i % 200) * 2 // 60, (i % 200) * 2 % 60)
+        ts = "2020-{:02d}-{:02d} {:02d}:{:02d}:00".format(1 + i // 6000, 2 + i % 6000 // 200, 9 + (i % 200) * 2 // 60, (i % 200) * 2 % 60)
         row = []
         for c in names:
             if c == "ID":
@@ -151,13 +167,28 @@ def main():
     feats += [col("delta_MA", f"delta_MA{p}") for p in config.delta_MA_periods]
     feats += [col("stochastic_oscillator", "stoch"), col("ATR", "ATR"), col("price_change", "price_change")]
     tgt = np.stack([col("target", f) for f in ("up1", "up2", "down1", "down2")], axis=1)
+    return np.stack(feats, axis=1), tgt
+
+
+def main():
+    db = sqlite3.connect(":memory:")
+    db.create_window_function("STD", 1, _Std)
+    cur = _install_stubs(db)
+    sys.path.insert(0, REF)
+    import create_database as ref                                   # the UNMODIFIED reference module: creates table + views
+    import config
+    table = config.mysql_table_name
     views = [s for s in cur.log if "CREATE OR REPLACE VIEW" in s]
-    np.savez_compressed(OUT, close=close, high=high, low=low, volume=volume, delta=delta, features=np.stack(feats, axis=1),
-                        targets=tgt, volume_MA_periods=np.array(config.volume_MA_periods), price_MA_periods=np.array(config.price_MA_periods),
-                        delta_MA_periods=np.array(config.delta_MA_periods), bollinger_bands_period=config.bollinger_bands_period,
-                        bollinger_bands_std=config.bollinger_bands_std, n_views=len(views), join_statement=str(ref.join_statement))
-    print(f"{OUT}: {n} rows, {len(feats)} feature columns, {len(views)} reference views executed; "
-          f"NULLs: stoch {int(np.isnan(feats[-3]).sum())}, price_change {int(np.isnan(feats[-1]).sum())}")
+    for name, cols in (("features.npz", synthetic_table(400)), ("features_ties.npz", tick_table(8000))):
+        feats, tgt = reference_views(db, config, table, cols)
+        close, high, low, volume, delta = cols
+        out = os.path.join(HERE, name)
+        np.savez_compressed(out, close=close, high=high, low=low, volume=volume, delta=delta, features=feats, targets=tgt,
+                            volume_MA_periods=np.array(config.volume_MA_periods), price_MA_periods=np.array(config.price_MA_periods),
+                            delta_MA_periods=np.array(config.delta_MA_periods), bollinger_bands_period=config.bollinger_bands_period,
+                            bollinger_bands_std=config.bollinger_bands_std, n_views=len(views), join_statement=str(ref.join_statement))
+        print(f"{out}: {len(close)} rows, {feats.shape[1]} feature columns, {len(views)} reference views executed; "
+              f"NULLs: stoch {int(np.isnan(feats[:, -3]).sum())}, price_change {int(np.isnan(feats[:, -1]).sum())}")
 
 
 if __name__ == "__main__":

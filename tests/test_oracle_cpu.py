@@ -226,6 +226,22 @@ def test_features_oracle_against_reference_sql(golden_dir):
     assert np.array_equal(t, z["targets"])
 
 
+def test_features_oracle_against_reference_sql_at_ties(golden_dir):
+    """The same pin on tests/golden/features_ties.npz: 8,000 quarter-point rows where the move to row i + 8 / i + 15
+    often equals n1 / n2 * ATR exactly.  The labels must be the SQL's at those ties (the GPU tests use this oracle as
+    the reference for longer tick-grid tables), and every feature within 1e-12."""
+    from oracle import features_oracle as fo
+    z = np.load(os.path.join(golden_dir, "features_ties.npz"))
+    cols = [z[k].astype(np.float64) for k in ("close", "high", "low", "volume", "delta")]
+    f, t = fo.window_features(*cols, volume_MA_periods=list(z["volume_MA_periods"]), price_MA_periods=list(z["price_MA_periods"]),
+                              delta_MA_periods=list(z["delta_MA_periods"]), bollinger_bands_period=int(z["bollinger_bands_period"]),
+                              bollinger_bands_std=float(z["bollinger_bands_std"]), stochastic_oscillator=True)
+    assert int(z["n_views"]) == 8 and f.shape == z["features"].shape == (8000, 9)
+    assert np.array_equal(np.isnan(f), np.isnan(z["features"])) and np.isnan(z["features"][:, 6]).any()
+    np.testing.assert_allclose(np.nan_to_num(f), np.nan_to_num(z["features"]), rtol=0, atol=1e-12)
+    assert np.array_equal(t, z["targets"])
+
+
 # ---- rounding model of the tensor-core precisions (oracle/bigru_ref.c, prec / mask) ------------------------------------
 def _rand_case(B, T, F, H, L, C, D, use_h0, seed):
     rng = np.random.default_rng(seed)
