@@ -17,7 +17,7 @@ void bigru_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* bigru_last_error(void) { return g_err; }
-extern "C" int bigru_version(void) { return 206; }
+extern "C" int bigru_version(void) { return 207; }
 
 extern "C" int bigru_device_check(int dev) {
     int n = 0;
@@ -251,6 +251,53 @@ extern "C" int bigru_stash_argmax_offset(const bigru_plan* p, size_t* byte_offse
 extern "C" int bigru_stash_output_offset(const bigru_plan* p, int layer, size_t* byte_offset) {
     if (!p || !byte_offset || layer < 0 || layer >= p->L) { bigru_set_error("stash_output_offset: bad argument"); return BIGRU_ERR_ARG; }
     *byte_offset = (size_t)stash_layout(*p).Y[layer] * sizeof(float);
+    return BIGRU_OK;
+}
+
+// where a forward or backward intermediate lives inside the stash or the scratch (test support; see the header for the
+// regions and when each is valid)
+extern "C" int bigru_workspace_region(const bigru_plan* p, int which, int layer, int* in_scratch, size_t* byte_offset,
+                                      size_t* lo_byte_offset, int64_t* pitch) {
+    if (!p || !in_scratch || !byte_offset || !lo_byte_offset || !pitch) {
+        bigru_set_error("workspace_region: null argument");
+        return BIGRU_ERR_ARG;
+    }
+    const bool planes = which == BIGRU_WS_Y_PLANES || which == BIGRU_WS_IN_PLANES || which == BIGRU_WS_DGI_PLANES ||
+                        which == BIGRU_WS_DGH_PLANES;
+    const bool stashed = which == BIGRU_WS_GATES || which == BIGRU_WS_Y_PLANES || which == BIGRU_WS_IN_PLANES;
+    // stash regions exist for every layer; the scratch keeps layer 0's recurrence gradients, the upstream gradients of layers
+    // 0 and 1 and the head's dcat (layer L, as in bigru_param_offset)
+    const bool layer_ok = stashed ? layer >= 0 && layer < p->L
+                        : which == BIGRU_WS_DY ? layer >= 0 && layer < p->L && layer < 2
+                        : which == BIGRU_WS_DCAT ? layer == p->L : layer == 0;
+    if (which < 0 || which >= BIGRU_WS_COUNT || !layer_ok) {
+        bigru_set_error("workspace_region: bad region %d or layer %d", which, layer);
+        return BIGRU_ERR_ARG;
+    }
+    if (planes && p->prec == BIGRU_PREC_FP32) {
+        bigru_set_error("workspace_region: BIGRU_PREC_FP32 keeps no bf16 planes");
+        return BIGRU_ERR_UNSUPPORTED;
+    }
+    const StashF32 S = stash_layout(*p);
+    const ScratchF32 W = scratch_layout(*p);
+    const int64_t BT = (int64_t)p->B * p->T, H3 = 3LL * p->H, DH = (int64_t)p->D * p->H;
+    int64_t off = 0, pt = 0, depth_rows = 0;          // float offset, row pitch (elements), depth x rows of a plane
+    switch (which) {
+        case BIGRU_WS_GATES:      off = S.G[layer]; pt = 4LL * p->H; break;
+        case BIGRU_WS_Y_PLANES:   off = S.YP[layer]; pt = DH; depth_rows = BT; break;
+        case BIGRU_WS_IN_PLANES:  off = S.XP[layer]; pt = in_pitch(*p, layer); depth_rows = BT; break;
+        case BIGRU_WS_DGI:        off = W.dgi; pt = H3; break;
+        case BIGRU_WS_DGH:        off = W.dgh; pt = H3; break;
+        case BIGRU_WS_DGI_PLANES: off = W.dgiP; pt = H3; depth_rows = p->D * BT; break;
+        case BIGRU_WS_DGH_PLANES: off = W.dghP; pt = H3; depth_rows = p->D * BT; break;
+        case BIGRU_WS_DY:         off = (p->L - 1 - layer) % 2 == 0 ? W.dYa : W.dYb; pt = DH; break;
+        case BIGRU_WS_DHC:        off = W.dhc; pt = p->H; break;
+        default:                  off = W.dcat; pt = H3; break;
+    }
+    *in_scratch = stashed ? 0 : 1;
+    *byte_offset = (size_t)off * sizeof(float);
+    *lo_byte_offset = planes && p->prec == BIGRU_PREC_BF16X3 ? *byte_offset + (size_t)(depth_rows * pt) * 2 : SIZE_MAX;
+    *pitch = pt;
     return BIGRU_OK;
 }
 

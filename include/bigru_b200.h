@@ -82,6 +82,35 @@ int  bigru_stash_argmax_offset(const bigru_plan* plan, size_t* byte_offset);
 /* byte offset, inside the same stash, of layer `layer`'s fp32 output Y[B][T][D*H] (the nn.GRU output of that layer, direction
  * d in columns [d*H, d*H+H)); lets tests compare every layer at every time step. */
 int  bigru_stash_output_offset(const bigru_plan* plan, int layer, size_t* byte_offset);
+/* Test support, like the two offsets above: where an intermediate of the tensor-core forward or backward lives, so that
+ * tests can recompute each step and each GEMM from the kernels' own operands.  *in_scratch: 0 stash, 1 scratch;
+ * *byte_offset: start of the region (of the hi plane for planes); *lo_byte_offset: the lo plane at BIGRU_PREC_BF16X3,
+ * SIZE_MAX otherwise; *pitch: elements per row.  Planes are bf16 in the layout of their fp32 producer.  Rows are b*T + t.
+ *   which                   buffer   layer      contents; valid after
+ *   BIGRU_WS_GATES          stash    0..L-1     G [D][B*T][4H] fp32: r, z, n, W_hn h_{t-1} + b_hn; bigru_forward
+ *   BIGRU_WS_Y_PLANES       stash    0..L-1     planes of Y [B*T][D*H]; bigru_forward
+ *   BIGRU_WS_IN_PLANES      stash    0..L-1     planes of the layer's own input [B*T][rup(I_l, 8)], zero-padded columns;
+ *                                               bigru_forward, layer 0 always, layers above only in training with dropout
+ *   BIGRU_WS_DGI, _DGH      scratch  0          dgi, dgh [D][B*T][3H] fp32 of layer 0; bigru_backward (each layer reuses them)
+ *   BIGRU_WS_DGI_PLANES,    scratch  0          their planes; dgi's n-gate rows hold dan, the dgh rows are zero at each
+ *   BIGRU_WS_DGH_PLANES                         sequence's first step (t = 0 forward, t = T-1 reverse); bigru_backward
+ *   BIGRU_WS_DY             scratch  0, 1       upstream gradient of the layer's output [B*T][D*H]; bigru_backward
+ *   BIGRU_WS_DHC            scratch  0          dh_{-1} of layer 0 [D][B][H]; bigru_backward
+ *   BIGRU_WS_DCAT           scratch  L (head)   d cat [B][3H] (last | max | mean); bigru_backward
+ * Planes at BIGRU_PREC_FP32: BIGRU_ERR_UNSUPPORTED.  Another layer or an unknown `which`: BIGRU_ERR_ARG. */
+#define BIGRU_WS_GATES       0
+#define BIGRU_WS_Y_PLANES    1
+#define BIGRU_WS_IN_PLANES   2
+#define BIGRU_WS_DGI         3
+#define BIGRU_WS_DGH         4
+#define BIGRU_WS_DGI_PLANES  5
+#define BIGRU_WS_DGH_PLANES  6
+#define BIGRU_WS_DY          7
+#define BIGRU_WS_DHC         8
+#define BIGRU_WS_DCAT        9
+#define BIGRU_WS_COUNT      10
+int  bigru_workspace_region(const bigru_plan* plan, int which, int layer, int* in_scratch, size_t* byte_offset,
+                            size_t* lo_byte_offset, int64_t* pitch);
 
 /* --- BiGRU.forward (biGRU_model.py:63-138): dropout :87-94, nn.GRU :102, head :111-137.
  *  d_x[B,T,F]; d_h0 nullable [L*D,B,H] (the `hidden` argument); d_logits[B,C];

@@ -1,10 +1,13 @@
 """Drives the library's C ABI on one plan and takes the result apart tensor by tensor.  Test infrastructure, shared by
-test_gpu_rounding_model.py and test_gpu_fp32_path.py.
+test_gpu_rounding_model.py, test_gpu_fp32_path.py and test_gpu_tc_steps.py.
 
 A shape is a dict with B, T, F, H, L, C, D (1 or 2) and h0 (bool).  `kernel` runs bigru_forward and bigru_backward at a
 precision ("fp32", "bf16" or "bf16x3"), optionally with dropout, and returns every layer's output, hn, the max-pool
-routing, the flat gradient, dx and dh0 in float64.  `tensors` / `kernel_steps` split such a result into the per-tensor
-comparisons, `stepwise` recomputes one step from the kernel's own state, `dist` measures two tensors."""
+routing, the flat gradient, dx and dh0 in float64 (with regions=True also the backward's intermediates, read through
+bigru_workspace_region).  `tensors` / `kernel_steps` split such a result into the per-tensor comparisons, `stepwise`
+recomputes one forward step from the kernel's own state, `backward_steps` / `gemm_steps` each backward step of layer 0
+and each backward GEMM from the kernel's own operands, `plane_checks` the bf16 planes bit for bit, `dist` measures two
+tensors."""
 import ctypes as C
 
 import numpy as np
@@ -68,8 +71,57 @@ def abi_names(s):
     return names
 
 
-def kernel(s, prec, flat, x, h0, dl, p=0.0, spatial=False, seed=0):
-    """bigru_forward + bigru_backward of shape s at precision prec; dropout p (training mode) when p > 0."""
+# BIGRU_WS_* of include/bigru_b200.h
+WS = dict(GATES=0, Y_PLANES=1, IN_PLANES=2, DGI=3, DGH=4, DGI_PLANES=5, DGH_PLANES=6, DY=7, DHC=8, DCAT=9)
+PLANE_REGIONS = ("Y_PLANES", "IN_PLANES", "DGI_PLANES", "DGH_PLANES")
+
+
+def region(plan, which, layer):
+    """bigru_workspace_region: (rc, in_scratch, byte offset, lo byte offset, pitch)."""
+    lib = _pkg()._lib.load()
+    sc, off, lo, pitch = C.c_int(), C.c_size_t(), C.c_size_t(), C.c_int64()
+    rc = lib.bigru_workspace_region(plan, WS[which], layer, C.byref(sc), C.byref(off), C.byref(lo), C.byref(pitch))
+    return rc, sc.value, off.value, lo.value, pitch.value
+
+
+def _bits_to_f32(u16):
+    """bf16 bit patterns -> the float32 values they stand for."""
+    return (u16.astype(np.uint32) << np.uint32(16)).view(np.float32)
+
+
+def _workspace(plan, s, prec, stash, scratch):
+    """The backward's operands and intermediates (bigru_workspace_region) as host arrays: fp32 regions as float32, planes
+    as (hi, lo) pairs of bf16 bit patterns (uint16; lo None at bf16).  Rows are split into [B, T] (and a leading D where
+    there is one)."""
+    B, T, F, H, L, D = (s[k] for k in "BTFHLD")
+    bufs = (stash, scratch)
+
+    def f32(which, layer, shape):
+        _, sc, off, _, _ = region(plan, which, layer)
+        n = int(np.prod(shape))
+        return bufs[sc][off // 4: off // 4 + n].view(*shape).cpu().numpy()
+
+    def planes(which, layer, shape):
+        _, sc, off, lo, _ = region(plan, which, layer)
+        n = int(np.prod(shape))
+        v = bufs[sc].view(torch.int16)
+        get = lambda o: v[o // 2: o // 2 + n].view(*shape).cpu().numpy().view(np.uint16)   # noqa: E731
+        return get(off), (get(lo) if prec == "bf16x3" else None)
+
+    pitch0 = region(plan, "IN_PLANES", 0)[4]
+    ws = dict(G=[f32("GATES", l, (D, B, T, 4 * H)) for l in range(L)],
+              YP=[planes("Y_PLANES", l, (B, T, D * H)) for l in range(L)],
+              XP=planes("IN_PLANES", 0, (B, T, pitch0)),
+              DGI=f32("DGI", 0, (D, B, T, 3 * H)), DGH=f32("DGH", 0, (D, B, T, 3 * H)),
+              DGIP=planes("DGI_PLANES", 0, (D, B, T, 3 * H)), DGHP=planes("DGH_PLANES", 0, (D, B, T, 3 * H)),
+              DY=[f32("DY", l, (B, T, D * H)) for l in range(min(L, 2))],
+              DHC=f32("DHC", 0, (D, B, H)), DCAT=f32("DCAT", L, (B, 3 * H)))
+    return ws
+
+
+def kernel(s, prec, flat, x, h0, dl, p=0.0, spatial=False, seed=0, regions=False):
+    """bigru_forward + bigru_backward of shape s at precision prec; dropout p (training mode) when p > 0.  regions: the
+    result also holds "ws", the intermediates of _workspace (tensor-core precisions)."""
     pkg = _pkg()
     lib, L_ = pkg._lib.load(), pkg._lib
     B, T, F, H, L, C_, D = (s[k] for k in "BTFHLCD")
@@ -105,10 +157,15 @@ def kernel(s, prec, flat, x, h0, dl, p=0.0, spatial=False, seed=0):
                                     ptr(dld), ptr(grads), ptr(dx), ptr(dh0), st), "backward")
         torch.cuda.synchronize()
         names = param_names(plan, s)
+        ws = _workspace(plan, s, prec, stash, scratch) if regions else None
+        del stash, scratch
     finally:
         lib.bigru_plan_destroy(plan)
     f64 = lambda t: None if t is None else t.cpu().numpy().astype(np.float64)   # noqa: E731
-    return dict(logits=f64(logits), hn=f64(hn), ys=ys, arg=arg, grads=f64(grads), dx=f64(dx), dh0=f64(dh0)), names
+    out = dict(logits=f64(logits), hn=f64(hn), ys=ys, arg=arg, grads=f64(grads), dx=f64(dx), dh0=f64(dh0))
+    if regions:
+        out["ws"] = ws
+    return out, names
 
 
 def bf16(v32):
@@ -136,20 +193,60 @@ def mm(a, b, prec):
     return ah @ bf.T + al @ bh.T
 
 
-def stepwise(s, prec, flat, x, h0, dl, got, names):
+def split(v, prec):
+    """An operand as the tensor-core kernels read it, as a (hi, lo) pair of float64 arrays: exact -> (v, None); bf16 ->
+    (rn_bf16(fp32 v), None); bf16x3 -> split_bf16 of tc_hopper.cuh, hi = rn_bf16(v), lo = rn_bf16(v - hi), from fp32 v."""
+    if prec == "exact":
+        return np.asarray(v, np.float64), None
+    v32 = np.asarray(v, np.float32)
+    hi = bf16(v32)
+    return hi.astype(np.float64), (bf16(v32 - hi).astype(np.float64) if prec == "bf16x3" else None)
+
+
+def pmm(a, b):
+    """a @ b of split operands (hi, lo) in float64: ah bh + ah bl + al bh (lo None: absent), the products the bf16x3
+    kernels issue; the dropped lo*lo is what split_bf16's model drops too."""
+    out = a[0] @ b[0]
+    if b[1] is not None:
+        out += a[0] @ b[1]
+    if a[1] is not None:
+        out += a[1] @ b[0]
+    return out
+
+
+def tr(p):
+    """Transpose of a split operand."""
+    return p[0].T, (None if p[1] is None else p[1].T)
+
+
+def f64(a):
+    """float64 values of an operand array: bf16 bit patterns (uint16, a kernel's plane) or floating-point values."""
+    return _bits_to_f32(a).astype(np.float64) if a.dtype == np.uint16 else np.asarray(a, np.float64)
+
+
+def rows64(p, sl, cols=slice(None)):
+    """Rows `sl` (and columns `cols`) of a (hi, lo) operand pair as a float64 split operand."""
+    return f64(p[0][sl, cols]), (None if p[1] is None else f64(p[1][sl, cols]))
+
+
+def stepwise(s, prec, flat, x, h0, dl, got, names, rows=None, gates=False):
     """The model at `prec` (mm's) run one step at a time from the kernel's own state: every step of every layer starts
     from the kernel's h_{t-1} (its Y, or h0) and the kernel's layer input (x, or the previous layer's Y), the head from
     the kernel's top-layer Y.  Rounding flips cannot compound, so what is left of the kernel's distance is the arithmetic
     of one step.  At "fp32" every operation is float32.  Returns (name, class) -> array like `tensors`: Y per layer,
-    direction and step, the logits and the lin_w gradient."""
+    direction and step, the logits and the lin_w gradient.  rows: the batch rows the layers are stepped for (all when
+    None; the head always takes all).  gates: also G per layer, direction and step (class g_step), the model's r, z, n and
+    W_hn h_{t-1} + b_hn, which the forward scan stashes for the backward."""
     B, T, H, L, C_, D = (s[k] for k in "BTHLCD")
+    rows = np.arange(B) if rows is None else np.asarray(rows)
+    B = len(rows)
     dt = np.float32 if prec == "fp32" else np.float64
     one = dt(1)
     out = {}
     sig = lambda v: one / (one + np.exp(-v))                    # noqa: E731
-    inp = x.astype(dt)
+    inp = x[rows].astype(dt)
     for l in range(L):
-        Y = got["ys"][l].astype(dt)
+        Y = got["ys"][l][rows].astype(dt)
         I = inp.shape[2]
         for d in range(D):
             o = names[f"l{l}d{d}.w_ih"][0]
@@ -157,7 +254,7 @@ def stepwise(s, prec, flat, x, h0, dl, got, names):
             w_hh = flat[o:o + 3 * H * H].reshape(3 * H, H).astype(dt); o += 3 * H * H
             b_ih, b_hh = flat[o:o + 3 * H].astype(dt), flat[o + 3 * H:o + 6 * H].astype(dt)
             y = Y[:, :, d * H:(d + 1) * H]
-            start = np.zeros((B, H), dt) if h0 is None else h0[l * D + d].astype(dt)
+            start = np.zeros((B, H), dt) if h0 is None else h0[l * D + d][rows].astype(dt)
             if d == 0:
                 hp = np.concatenate([start[:, None], y[:, :-1]], 1)
             else:
@@ -170,6 +267,9 @@ def stepwise(s, prec, flat, x, h0, dl, got, names):
             h = (one - z) * n + z * hp
             for t in range(T):
                 out[(f"step:y[l{l}d{d},t{t}]", "y_step")] = h[:, t].astype(np.float64)
+                if gates:
+                    out[(f"step:g[l{l}d{d},t{t}]", "g_step")] = np.concatenate(
+                        [r[:, t], z[:, t], n[:, t], gh[:, t, 2 * H:]], 1).astype(np.float64)
         inp = Y
     top = got["ys"][-1].astype(dt)
     pooled = top[..., :H] + top[..., H:] if D == 2 else top
@@ -183,17 +283,170 @@ def stepwise(s, prec, flat, x, h0, dl, got, names):
     return out
 
 
-def kernel_steps(got, s, names):
+def kernel_steps(got, s, names, rows=None, gates=False):
     """The kernel's side of stepwise."""
     H = s["H"]
+    rows = np.arange(s["B"]) if rows is None else np.asarray(rows)
     out = {}
     for l, y in enumerate(got["ys"]):
         for d in range(s["D"]):
             for t in range(s["T"]):
-                out[(f"step:y[l{l}d{d},t{t}]", "y_step")] = y[:, t, d * H:(d + 1) * H]
+                out[(f"step:y[l{l}d{d},t{t}]", "y_step")] = y[rows, t, d * H:(d + 1) * H]
+                if gates:
+                    out[(f"step:g[l{l}d{d},t{t}]", "g_step")] = got["ws"]["G"][l][d][rows, t].astype(np.float64)
     out[("step:logits", "logits_step")] = got["logits"]
     o, k = names["lin_w"]
     out[("step:grad:lin_w", "w_step")] = got["grads"][o:o + k]
+    return out
+
+
+def _block(flat, names, name, shape):
+    o = names[name][0]
+    return flat[o:o + int(np.prod(shape))].reshape(shape)
+
+
+def head_dcat(s, prec, flat, dl, names):
+    """d cat [B, 3H] = dlogits lin_w, operands split as tc_pack_kernel splits them."""
+    return pmm(split(dl, prec), split(_block(flat, names, "lin_w", (s["C"], 3 * s["H"])), prec))
+
+
+def head_dy(s, dcat, arg):
+    """The top layer's upstream gradient [B, T, D*H] from d cat and the max-pool routing, as head_bwd_dy_kernel routes it:
+    the mean's share at every step plus the max's at the arg-max step, the same for both directions.  (The `last` share
+    is the carry into the layer's last step, dcat[:, :H].)"""
+    B, T, H, D = (s[k] for k in "BTHD")
+    v = np.broadcast_to(dcat[:, None, 2 * H:] / T, (B, T, H)).copy()
+    v += np.where(arg[:, None, :] == np.arange(T)[None, :, None], dcat[:, None, H:2 * H], 0.0)
+    return np.concatenate([v] * D, 2)
+
+
+def backward_steps(s, prec, flat, h0, ws, ys, names, own=False):
+    """Layer 0's backward recurrence one step at a time in float64, following gru_scan_bwd_kernel (tc_hopper.cuh), per
+    direction in the kernel's step order.  Each step takes the kernel's own operands: its dY (ws["DY"][0]), its gates
+    (ws["G"][0]) and its h_{t-1} (ys[0], or h0), and
+        dh_t = dY_t + dh_{t+1} z_{t+1} + P_{t+1},   P_{t+1} = dgh_{t+1} W_hh  with both operands split at `prec`,
+    where dgh_{t+1} is the kernel's fp32 dgh (ws["DGH"]; not its planes, which are zero at the first step, where the
+    recurrence still reads the real tile).  The carry dh itself stays float64: no rounding separates it from the kernel's,
+    so rounding flips cannot compound.  It starts from the head's `last` share of the kernel's dcat when layer 0 is the
+    top layer, else from zero.  own: P takes the model's own dgh instead, which makes this the oracle's free-running
+    backward again.  Yields ("dg", d, t, dgi, dgh) per step ([B, 3H] each: dgi's n gate is dan, dgh's is dan r) and
+    ("dh0", d, None, dh_{-1}, None) after each direction's last step."""
+    B, T, H, L, D = (s[k] for k in "BTHLD")
+    for d in range(D):
+        w = split(_block(flat, names, f"l0d{d}.w_hh", (3 * H, H)), prec)        # P[b, k] = sum_q dgh[b, q] W[q, k]
+        G, y, dY = ws["G"][0][d], ys[0][:, :, d * H:(d + 1) * H], ws["DY"][0][:, :, d * H:(d + 1) * H]
+        carry = ws["DCAT"][:, :H].astype(np.float64) if L == 1 else np.zeros((B, H))
+        start = np.zeros((B, H)) if h0 is None else h0[d].astype(np.float64)
+        for st in range(T):
+            t = T - 1 - st if d == 0 else st
+            first = t == (0 if d == 0 else T - 1)
+            g = G[:, t].astype(np.float64)
+            r, z, n, hnv = g[:, :H], g[:, H:2 * H], g[:, 2 * H:3 * H], g[:, 3 * H:]
+            hp = start if first else y[:, t - 1 if d == 0 else t + 1].astype(np.float64)
+            dh = carry + dY[:, t]
+            dan = dh * (1 - z) * (1 - n * n)
+            dar = dan * hnv * r * (1 - r)
+            daz = dh * (hp - n) * z * (1 - z)
+            dgh = np.concatenate([dar, daz, dan * r], 1)
+            yield "dg", d, t, np.concatenate([dar, daz, dan], 1), dgh
+            carry = dh * z + pmm(split(dgh if own else ws["DGH"][d][:, t], prec), w)
+        yield "dh0", d, None, carry, None
+
+
+def gemm_steps(s, prec, flat, dl, h0, ops, names, arg):
+    """Every backward GEMM of layer 0 and of the head in float64, from the operands the kernels read: `ops` holds the dgi
+    and dgh planes (DGIP, DGHP: (hi, lo) [D, B, T, 3H]), the layer input's planes (XP [B, T, pitch]), the Y planes of layer
+    0 (YP [B, T, D*H]), fp32 dgi and dgh (DGI, DGH [D, B, T, 3H]) and the kernel's dcat.  Returns (name, "gemm_step") ->
+      grad:l0d{d}.w_ih   dgi planes^T input planes;
+      grad:l0d{d}.w_hh   dgh planes^T Y planes shifted by one row against the step order, plus the w0 term from fp32 dgh
+                         at each sequence's first step and h0 (both split as tc_pack_kernel splits them);
+      grad:l0d{d}.b_ih, .b_hh   column sums of fp32 dgi, dgh;
+      dx                 sum over d of dgi planes W_ih[d] (the kcat GEMM);
+      dcat               dlogits lin_w;
+      dy[l{L-1}]         the top layer's upstream gradient from the kernel's dcat and `arg` (when it survives the backward:
+                         layers 0 and 1)."""
+    B, T, F, H, L, D = (s[k] for k in "BTFHLD")
+    BT = B * T
+    flat2 = lambda p, d=None: tuple(None if a is None else (a if d is None else a[d]).reshape(BT, -1) for a in p)   # noqa: E731
+    xp, yp = flat2(ops["XP"]), flat2(ops["YP"])
+    t_of = np.arange(BT) % T
+    dx = np.zeros((BT, F))
+    out = {}
+    for d in range(D):
+        gi, gh = flat2(ops["DGIP"], d), flat2(ops["DGHP"], d)
+        w_ih = split(_block(flat, names, f"l0d{d}.w_ih", (3 * H, F)), prec)
+        dwih, dwhh = np.zeros((3 * H, F)), np.zeros((3 * H, H))
+        # K = B*T in chunks of rows, so that no float64 copy of a whole plane is made
+        for r0 in range(0, BT, 8192):
+            sl = slice(r0, min(BT, r0 + 8192))
+            a, c = rows64(gi, sl), rows64(gh, sl)
+            dwih += pmm(tr(a), rows64(xp, sl, slice(0, F)))
+            # H_prev(b, t) = Y(b, t - 1) forward, Y(b, t + 1) reverse: rows shifted by one; where that leaves the sequence
+            # the dgh planes are zero (and so is H_prev here)
+            src = np.arange(sl.start, sl.stop) + (-1 if d == 0 else 1)
+            keep = (t_of[sl] != (0 if d == 0 else T - 1))[:, None]
+            hp = rows64(yp, np.clip(src, 0, BT - 1), slice(d * H, (d + 1) * H))
+            dwhh += pmm(tr(c), tuple(None if v is None else v * keep for v in hp))
+            dx[sl] += pmm(a, w_ih)
+        if h0 is not None:
+            tf = 0 if d == 0 else T - 1
+            dwhh += pmm(tr(split(ops["DGH"][d][:, tf], prec)), split(h0[d], prec))
+        out[(f"gemm:grad:l0d{d}.w_ih", "gemm_step")] = dwih.ravel()
+        out[(f"gemm:grad:l0d{d}.w_hh", "gemm_step")] = dwhh.ravel()
+        out[(f"gemm:grad:l0d{d}.b_ih", "gemm_step")] = ops["DGI"][d].reshape(BT, 3 * H).astype(np.float64).sum(0)
+        out[(f"gemm:grad:l0d{d}.b_hh", "gemm_step")] = ops["DGH"][d].reshape(BT, 3 * H).astype(np.float64).sum(0)
+    out[("gemm:dx", "gemm_step")] = dx.reshape(B, T, F)
+    out[("gemm:dcat", "gemm_step")] = head_dcat(s, prec, flat, dl, names)
+    if L <= 2:
+        out[(f"gemm:dy[l{L - 1}]", "gemm_step")] = head_dy(s, ops["DCAT"].astype(np.float64), arg)
+    return out
+
+
+def kernel_gemm_steps(got, s, names):
+    """The kernel's side of gemm_steps."""
+    out = {}
+    for d in range(s["D"]):
+        for nm in ("w_ih", "w_hh", "b_ih", "b_hh"):
+            o, k = names[f"l0d{d}.{nm}"]
+            out[(f"gemm:grad:l0d{d}.{nm}", "gemm_step")] = got["grads"][o:o + k]
+    out[("gemm:dx", "gemm_step")] = got["dx"]
+    out[("gemm:dcat", "gemm_step")] = got["ws"]["DCAT"].astype(np.float64)
+    if s["L"] <= 2:
+        out[(f"gemm:dy[l{s['L'] - 1}]", "gemm_step")] = got["ws"]["DY"][s["L"] - 1].astype(np.float64)
+    return out
+
+
+def _split_bits(v32, prec):
+    """split_bf16 of float32 values as bf16 bit patterns (uint16): hi, and lo at bf16x3."""
+    bits = lambda v: (v.view(np.uint32) >> np.uint32(16)).astype(np.uint16)     # noqa: E731
+    hi = bf16(v32)
+    return bits(hi), (bits(bf16(v32 - hi)) if prec == "bf16x3" else None)
+
+
+def plane_checks(got, s, prec, x):
+    """Elements (hi and lo together) where a plane the kernels wrote differs bitwise from split_bf16 of its fp32 source:
+    the Y planes of every layer; layer 0's input planes (x, zero-padded to the pitch); the dgi planes; the dgh planes, zero
+    at each sequence's first step.  name -> count; all must be 0."""
+    ws, T, F = got["ws"], s["T"], s["F"]
+    bad = lambda a, b: int((a != b).sum())                                       # noqa: E731
+
+    def cmp(pl, want):
+        n = bad(pl[0], want[0])
+        return n + (bad(pl[1], want[1]) if prec == "bf16x3" else 0)
+
+    out = {f"Y_PLANES[l{l}]": cmp(ws["YP"][l], _split_bits(y.astype(np.float32), prec)) for l, y in enumerate(got["ys"])}
+    xw = np.zeros(ws["XP"][0].shape, np.float32)
+    xw[..., :F] = x
+    hi, lo = _split_bits(xw, prec)
+    out["IN_PLANES[l0]"] = cmp(ws["XP"], (hi, lo))
+    out["DGI_PLANES"] = cmp(ws["DGIP"], _split_bits(ws["DGI"], prec))
+    want = [p.copy() if p is not None else None for p in _split_bits(ws["DGH"], prec)]
+    for p in want:
+        if p is not None:
+            p[0, :, 0] = 0
+            if s["D"] == 2:
+                p[1, :, T - 1] = 0
+    out["DGH_PLANES"] = cmp(ws["DGHP"], want)
     return out
 
 

@@ -61,6 +61,9 @@ REGIMES = {
     "h0": lambda s: s["h0"],
     # split-K on every weight-gradient GEMM, and more units than SMs: CTAs run several units, the producer runs ahead
     "splitk_persistent": lambda s: all(sp > 1 and units > NSM for sp, units in dw_gemms(s)),
+    # bidirectional H = 512 (8-CTA clusters, both directions: bf16's largest backward shared-memory footprint), and an odd
+    # number of 16-row batch tiles
+    "cluster8_d2": lambda s: s["H"] == 512 and s["D"] == 2, "odd_tiles": lambda s: (s["B"] // 16) % 2 == 1 and s["B"] > 16,
 }
 
 SHAPES = {
@@ -78,6 +81,10 @@ SHAPES = {
                          regimes=("cluster4", "F_wide_ragged", "h0", "T_odd")),
     "h256_splitk": dict(B=32, T=128, F=136, H=256, L=2, C=3, D=2, h0=False, precs=("bf16", "bf16x3"),
                         regimes=("cluster4", "many_tiles", "splitk_persistent")),
+    "h512_d2": dict(B=32, T=6, F=40, H=512, L=2, C=3, D=2, h0=False, precs=("bf16",),
+                    regimes=("cluster8", "cluster8_d2", "many_tiles", "D2")),
+    "h256_b48": dict(B=48, T=5, F=20, H=256, L=1, C=3, D=2, h0=False, precs=("bf16",),
+                     regimes=("cluster4", "odd_tiles", "many_tiles", "D2", "T_odd")),
 }
 
 # Kernel-vs-model tolerances (rel-L2, max-abs over max |model|) per tensor class: about 4x the worst value measured on an
