@@ -36,6 +36,9 @@ SIGNATURES = {
     "bigru_backward": (_i, [_vp, _vp, _vp, _vp, _f, _i, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_infer_workspace_bytes": (_i, [_vp, C.POINTER(C.c_size_t)]),
     "bigru_infer": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "bigru_forward_lengths": (_i, [_vp, _vp, _vp, _vp, _f, _i, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "bigru_backward_lengths": (_i, [_vp, _vp, _vp, _vp, _f, _i, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "bigru_infer_lengths": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_loss": (_i, [_i, _vp, _vp, _vp, _vp, _i, _i, _d, _vp, _vp, _vp]),
     "bigru_sqnorm": (_i, [_vp, _i64, _vp, _vp, _vp]),
     "bigru_adam_tick": (_i, [_vp, _vp, _vp]),

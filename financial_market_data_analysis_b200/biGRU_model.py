@@ -81,6 +81,14 @@ class _Padding:
         out[tuple(slice(0, n) for n in t.shape)] = t
         return out
 
+    def lengths(self, lens, Bp, T):
+        """Per-row lengths [Bp] of a plan: `lens` (None stays None) with the appended zero rows T steps long."""
+        if lens is None or lens.shape[0] == Bp:
+            return lens
+        out = lens.new_full((Bp,), T)
+        out[:lens.shape[0]] = lens
+        return out
+
     def crop(self, t, B, dim=0, units=False):
         """The first B rows along `dim` of a plan-sized tensor and, when `units`, its real hidden units."""
         if t is None:
@@ -164,12 +172,14 @@ class _AdamState:
 
 
 class _StepBuffers:
-    """What one fused train step reads and writes: the plan and a stash of its pool, the padded inputs, the targets of the
-    real rows, the loss arguments, logits / dlogits of the padded batch and the dropout arguments of the C calls."""
+    """What one fused train step reads and writes: the plan and a stash of its pool, the padded inputs and per-row lengths
+    (None: every row T steps), the targets of the real rows, the loss arguments, logits / dlogits of the padded batch and the
+    dropout arguments of the C calls."""
 
-    def __init__(self, plan, x, h0, tgt, loss, C, drop):
+    def __init__(self, plan, x, h0, tgt, loss, C, drop, lengths=None):
         Bp = x.shape[0]
         self.plan, self.stash, self.x, self.h0, self.tgt, self.loss, self.drop = plan, plan.acquire_stash(), x, h0, tgt, loss, drop
+        self.lengths = lengths
         self.logits = torch.empty(Bp, C, device=x.device, dtype=torch.float32)
         # the loss writes dlogits of the real rows only: the padded rows stay zero
         self.dlogits = (torch.zeros if Bp != tgt.shape[0] else torch.empty)(Bp, C, device=x.device, dtype=torch.float32)
@@ -255,12 +265,13 @@ class _BiGRUFunction(torch.autograd.Function):
     """autograd boundary: forward/backward are single calls into the C ABI."""
 
     @staticmethod
-    def forward(ctx, model, x, h0, *params):
+    def forward(ctx, model, x, h0, lengths, *params):
         lib = _lib.load()
         pad = model._pad
         B = x.shape[0]
         Bp = model._padded_batch(B)
         x, h0 = pad.pad(x, Bp), pad.pad(h0, Bp, dim=1, units=True)
+        lengths = pad.lengths(lengths, Bp, x.shape[1])
         plan = model._plan_for(x)
         with torch.cuda.device(x.device):                 # the C ABI launches on the CURRENT device: make it the model's
             pflat = model._plan_params()
@@ -271,15 +282,15 @@ class _BiGRUFunction(torch.autograd.Function):
             training = bool(model.training and model.dropout_p > 0)
             seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if training else 0
             model._last_seed = seed                       # the dropout masks are a pure function of (seed, element index)
-            _lib.check(lib.bigru_forward(plan.handle, _lib.ptr(pflat), _lib.ptr(x), _lib.ptr(h0),
-                                         float(model.dropout_p), int(bool(model.spatial_dropout)), int(training), seed,
-                                         _lib.ptr(stash), _lib.ptr(plan.scratch), _lib.ptr(logits), _lib.ptr(hn),
-                                         _stream_ptr(x.device)), "bigru_forward")
+            _lib.check(lib.bigru_forward_lengths(plan.handle, _lib.ptr(pflat), _lib.ptr(x), _lib.ptr(h0),
+                                                 float(model.dropout_p), int(bool(model.spatial_dropout)), int(training), seed,
+                                                 _lib.ptr(stash), _lib.ptr(plan.scratch), _lib.ptr(logits), _lib.ptr(hn),
+                                                 _lib.ptr(lengths), _stream_ptr(x.device)), "bigru_forward_lengths")
             model._last_hidden = pad.crop(hn, B, dim=1, units=True)
             model._last_forward = (plan, stash, B)
             if need_grad:
                 ctx.model, ctx.pad, ctx.plan, ctx.stash, ctx.seed, ctx.training = model, pad, plan, stash, seed, training
-                ctx.pflat, ctx.real_batch, ctx.has_h0 = pflat, B, h0 is not None
+                ctx.pflat, ctx.real_batch, ctx.has_h0, ctx.lengths = pflat, B, h0 is not None, lengths
                 ctx.save_for_backward(x, h0 if h0 is not None else torch.empty(0, device=x.device))
             else:
                 plan.release_stash(stash)
@@ -297,15 +308,16 @@ class _BiGRUFunction(torch.autograd.Function):
         dx = torch.empty_like(x) if ctx.needs_input_grad[1] else None
         dh0 = torch.empty_like(h0) if (h0 is not None and ctx.needs_input_grad[2]) else None
         with torch.cuda.device(x.device):
-            _lib.check(lib.bigru_backward(plan.handle, _lib.ptr(ctx.pflat), _lib.ptr(x), _lib.ptr(h0),
-                                          float(model.dropout_p), int(bool(model.spatial_dropout)), int(ctx.training),
-                                          ctx.seed, _lib.ptr(ctx.stash), _lib.ptr(plan.scratch), _lib.ptr(dlogits),
-                                          _lib.ptr(grads), _lib.ptr(dx), _lib.ptr(dh0), _stream_ptr(x.device)), "bigru_backward")
+            _lib.check(lib.bigru_backward_lengths(plan.handle, _lib.ptr(ctx.pflat), _lib.ptr(x), _lib.ptr(h0),
+                                                  float(model.dropout_p), int(bool(model.spatial_dropout)), int(ctx.training),
+                                                  ctx.seed, _lib.ptr(ctx.stash), _lib.ptr(plan.scratch), _lib.ptr(dlogits),
+                                                  _lib.ptr(grads), _lib.ptr(dx), _lib.ptr(dh0), _lib.ptr(ctx.lengths),
+                                                  _stream_ptr(x.device)), "bigru_backward_lengths")
         plan.release_stash(ctx.stash)
-        ctx.stash = ctx.pflat = None
+        ctx.stash = ctx.pflat = ctx.lengths = None
         grads = model._plan_grads(grads)                  # drop the padded hidden units' entries
         pg = tuple(grads[o:o + n].view(shape) for (o, n, shape) in model._views)
-        return (None, pad.crop(dx, B), pad.crop(dh0, B, dim=1, units=True)) + pg
+        return (None, pad.crop(dx, B), pad.crop(dh0, B, dim=1, units=True), None) + pg
 
 
 class BiGRU(nn.Module):
@@ -473,6 +485,25 @@ class BiGRU(nn.Module):
             h0 = hidden.to(device=dev, dtype=torch.float32).contiguous()
         return x, h0
 
+    @staticmethod
+    def _prepare_lengths(lengths, x, hidden):
+        """`lengths` (a list, a CPU or a CUDA tensor of integers) as an int32 tensor [B] on x's device, checked on the host:
+        shape [B], every value in [1, T], and no initial state with it.  None stays None (every row T steps long)."""
+        if lengths is None:
+            return None
+        if hidden is not None:
+            raise ValueError("lengths together with an initial hidden state (hidden) are not supported")
+        B, T = int(x.shape[0]), int(x.shape[1])
+        host = lengths.detach().cpu() if isinstance(lengths, torch.Tensor) else torch.as_tensor(lengths)
+        if host.dtype.is_floating_point or host.dtype.is_complex or host.dtype == torch.bool:
+            raise ValueError(f"lengths must hold integers, got {host.dtype}")
+        if tuple(host.shape) != (B,):
+            raise ValueError(f"lengths must have shape [{B}] (one per batch row), got {tuple(host.shape)}")
+        if B and (int(host.min()) < 1 or int(host.max()) > T):
+            raise ValueError(f"every length must lie in [1, {T}], got values from {int(host.min())} to {int(host.max())}")
+        # from pinned memory, so that the copy does not wait for the work already queued on the stream
+        return host.to(torch.int32).pin_memory().to(x.device, non_blocking=True)
+
     def pooled_argmax(self) -> torch.Tensor:
         """argmax_t of the max-pooled direction sum [batch, hidden] as taken by the last ``forward`` (the routing of the
         max-pool gradient, biGRU_model.py:125).  Valid until the next forward of the same shape."""
@@ -484,24 +515,33 @@ class BiGRU(nn.Module):
         return self._pad.crop(arg, B, units=True).clone()
 
     # ------------------------------------------------------------------ reference surface
-    def forward(self, input_seq, hidden=None):
-        """Logits [batch, output_size] (biGRU_model.py:63-138)."""
-        x, h0 = self._prepare_input(input_seq, hidden)
-        self.batch_size, self.input_length = x.size(0), x.size(1)          # as the reference sets (:82-85)
-        return _BiGRUFunction.apply(self, x, h0, *self._ordered_params())
+    def forward(self, input_seq, hidden=None, lengths=None):
+        """Logits [batch, output_size] (biGRU_model.py:63-138).
 
-    def infer(self, input_seq, hidden=None, max_batch: Optional[int] = None):
+        ``lengths`` ([batch] integers, each in [1, seq_len]; a list, a CPU or a CUDA tensor): row b is ``lengths[b]`` steps
+        long and its inputs at later steps are ignored.  Each GRU layer then runs as ``nn.GRU`` on
+        ``pack_padded_sequence(input_seq, lengths, batch_first=True, enforce_sorted=False)``, the head pools over the valid
+        steps only (``last`` at t = lengths[b] - 1 forward, t = 0 reverse) and the input gradient is 0 at padded steps.
+        Not with ``hidden`` (ValueError)."""
+        x, h0 = self._prepare_input(input_seq, hidden)
+        lens = self._prepare_lengths(lengths, x, hidden)
+        self.batch_size, self.input_length = x.size(0), x.size(1)          # as the reference sets (:82-85)
+        return _BiGRUFunction.apply(self, x, h0, lens, *self._ordered_params())
+
+    def infer(self, input_seq, hidden=None, max_batch: Optional[int] = None, lengths=None):
         """Eval-mode logits [batch, output_size] (bigru_infer), bit-identical to ``self.eval()(input_seq, hidden)`` under
         ``torch.no_grad()``: no dropout whatever ``self.training`` says, no autograd record, and nothing kept for a backward, so
         the plan allocates only its inference workspace (about a sixth of the training forward's stash + scratch at
         configs[1]).  ``max_batch`` runs the batch in slices of at most that many rows, all on one plan (the last slice
         zero-padded), which bounds the memory whatever the batch size.  ``pooled_argmax()`` and the last hidden state stay
-        those of the last ``forward``."""
+        those of the last ``forward``.  ``lengths``: per-row lengths as in ``forward``."""
         x, h0 = self._prepare_input(input_seq, hidden)
+        lens = self._prepare_lengths(lengths, x, hidden)
         B = x.shape[0]
         k = self._slice_rows(max_batch, B)
         pflat = self._plan_params()
-        outs = [self._infer_slice(pflat, x[s:s + k], None if h0 is None else h0[:, s:s + k], self._pad.batch(k))
+        outs = [self._infer_slice(pflat, x[s:s + k], None if h0 is None else h0[:, s:s + k], self._pad.batch(k),
+                                  None if lens is None else lens[s:s + k])
                 for s in range(0, B, k)]
         return outs[0] if len(outs) == 1 else torch.cat(outs)
 
@@ -514,18 +554,19 @@ class BiGRU(nn.Module):
             raise ValueError(f"max_batch must be positive, got {max_batch}")
         return min(int(max_batch), n)
 
-    def _infer_slice(self, pflat, x, h0, Bp):
+    def _infer_slice(self, pflat, x, h0, Bp, lengths=None):
         """Logits of the rows of x (at most Bp) through bigru_infer on the plan of Bp rows; pflat: _plan_params()."""
         pad, B = self._pad, x.shape[0]
         x = pad.pad(x, Bp)
+        lengths = pad.lengths(lengths, Bp, x.shape[1])
         h0 = pad.pad(h0, Bp, dim=1, units=True)
         h0 = None if h0 is None else h0.contiguous()
         plan = self._plan_for(x)
         with torch.no_grad(), torch.cuda.device(x.device):    # the C ABI launches on the CURRENT device: make it the model's
             logits = torch.empty(Bp, self.output_size, device=x.device, dtype=torch.float32)
-            _lib.check(_lib.load().bigru_infer(plan.handle, _lib.ptr(pflat), _lib.ptr(x), _lib.ptr(h0),
-                                               _lib.ptr(plan.infer_workspace()), _lib.ptr(logits), _stream_ptr(x.device)),
-                       "bigru_infer")
+            _lib.check(_lib.load().bigru_infer_lengths(plan.handle, _lib.ptr(pflat), _lib.ptr(x), _lib.ptr(h0),
+                                                       _lib.ptr(plan.infer_workspace()), _lib.ptr(logits), _lib.ptr(lengths),
+                                                       _stream_ptr(x.device)), "bigru_infer_lengths")
         return pad.crop(logits, B)
 
     def add_loss_fn(self, loss_fn):
@@ -650,13 +691,14 @@ class BiGRU(nn.Module):
         pflat = self._plan_params(st.pflat)
         # the loss sees the real batch rows (tgt's); logits / dlogits may carry zero-padded rows behind them
         B, C = buf.tgt.shape[0], buf.logits.shape[1]
-        _lib.check(lib.bigru_forward(plan.handle, _lib.ptr(pflat), _lib.ptr(buf.x), _lib.ptr(buf.h0), *buf.drop,
-                                     _lib.ptr(buf.stash), _lib.ptr(plan.scratch), _lib.ptr(buf.logits), None, s), "bigru_forward")
+        _lib.check(lib.bigru_forward_lengths(plan.handle, _lib.ptr(pflat), _lib.ptr(buf.x), _lib.ptr(buf.h0), *buf.drop,
+                                             _lib.ptr(buf.stash), _lib.ptr(plan.scratch), _lib.ptr(buf.logits), None,
+                                             _lib.ptr(buf.lengths), s), "bigru_forward_lengths")
         _lib.check(lib.bigru_loss(kind, _lib.ptr(buf.logits), _lib.ptr(buf.tgt), _lib.ptr(wv), _lib.ptr(pwv), B, C, denom,
                                   _lib.ptr(st.loss), _lib.ptr(buf.dlogits), s), "bigru_loss")
-        _lib.check(lib.bigru_backward(plan.handle, _lib.ptr(pflat), _lib.ptr(buf.x), _lib.ptr(buf.h0), *buf.drop,
-                                      _lib.ptr(buf.stash), _lib.ptr(plan.scratch), _lib.ptr(buf.dlogits), _lib.ptr(st.pgrad),
-                                      None, None, s), "bigru_backward")
+        _lib.check(lib.bigru_backward_lengths(plan.handle, _lib.ptr(pflat), _lib.ptr(buf.x), _lib.ptr(buf.h0), *buf.drop,
+                                              _lib.ptr(buf.stash), _lib.ptr(plan.scratch), _lib.ptr(buf.dlogits),
+                                              _lib.ptr(st.pgrad), None, None, _lib.ptr(buf.lengths), s), "bigru_backward_lengths")
         self._plan_grads(st.pgrad, st.grad)
 
     def _launch_update(self, g, st, s):
@@ -705,17 +747,20 @@ class BiGRU(nn.Module):
             self._graphs.clear()
         self._graphs[key] = (buf, ga, gb, launches)
 
-    def train_step(self, input_seq, target, hidden=None):
+    def train_step(self, input_seq, target, hidden=None, lengths=None):
         """One optimisation step = the body of the reference loop (biGRU_model.py:198-210):
         zero_grad, forward, loss, backward, clip_grad_norm_(clip), Adam step - C-ABI calls with no autograd graph, replayed
-        from a captured CUDA graph when the step is replayable (no dropout noise to draw, no initial state).
-        Returns (loss, logits) as device tensors (no host sync)."""
+        from a captured CUDA graph when the step is replayable (no dropout noise to draw, no initial state).  ``lengths``:
+        per-row lengths as in ``forward``.
+        Returns (loss, logits) as device tensors (no host sync, except that lengths given as a CUDA tensor are copied back to
+        be checked on the host)."""
         spec, g = self._loss_spec(), self._adam_spec()
         if spec is None or g is None:
             raise RuntimeError("train_step needs add_loss_fn(CrossEntropyLoss | BCEWithLogitsLoss | "
                                "MultiLabelSoftMarginLoss, mean reduction) and add_optimizer(torch.optim.Adam(model.parameters()))")
         lib = _lib.load()
         x, h0 = self._prepare_input(input_seq, hidden)
+        lens = self._prepare_lengths(lengths, x, hidden)
         dev = x.device
         kind, w, pw = spec
         B, C = x.shape[0], self.output_size
@@ -738,12 +783,14 @@ class BiGRU(nn.Module):
             key = ent = None
             if graphed:
                 key = (B, int(x.shape[1]), self.precision, kind, id(wv), id(pwv), denom, float(g["lr"]), tuple(g["betas"]),
-                       float(g["eps"]), float(self.clip), self._dp_world, dev.index)
+                       float(g["eps"]), float(self.clip), self._dp_world, dev.index, lens is not None)
                 ent = self._graphs.get(key)
             if ent is not None:
                 buf, ga, gb, launches = ent
                 buf.x[:B].copy_(x, non_blocking=True)      # rows >= B of the static buffer stay zero
                 buf.tgt.copy_(tgt, non_blocking=True)
+                if lens is not None:
+                    buf.lengths[:B].copy_(lens, non_blocking=True)   # rows >= B stay T steps long
                 compute, update = ga.replay, (gb.replay if gb is not None else lambda: None)
                 lib.bigru_launch_count_add(launches)
             else:
@@ -751,10 +798,12 @@ class BiGRU(nn.Module):
                 self._last_seed = seed
                 Bp = self._padded_batch(B)
                 x, h0 = self._pad.pad(x, Bp), self._pad.pad(h0, Bp, dim=1, units=True)
+                lens = self._pad.lengths(lens, Bp, int(x.shape[1]))
                 if graphed:                               # a new graph key: this step runs on the graph's static buffers
                     x, tgt = x.clone(), tgt.clone()
+                    lens = None if lens is None else lens.clone()
                 buf = _StepBuffers(self._plan_for(x), x, h0, tgt, (kind, wv, pwv, denom), C,
-                                   (float(self.dropout_p), int(bool(self.spatial_dropout)), int(training), seed))
+                                   (float(self.dropout_p), int(bool(self.spatial_dropout)), int(training), seed), lens)
                 compute, update = (lambda: self._launch_compute(buf, st, s)), (lambda: self._launch_update(g, st, s))
             compute()
             if self._dp_world > 1:

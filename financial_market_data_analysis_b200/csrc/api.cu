@@ -341,9 +341,14 @@ static FwdBufs infer_bufs(const bigru_plan& p, float* ws) {
     return b;
 }
 
-static int forward_plan(const bigru_plan& p, const float* params, const float* x, const float* h0, float drop,
+// len: per-row lengths [B] (device, 1 <= len <= T; the caller validates them) or null for T everywhere
+static int forward_plan(const bigru_plan& p, const float* params, const float* x, const float* h0, const int* len, float drop,
                         int spatial, int training, uint64_t seed, const FwdBufs& buf, float* logits, float* hn,
                         cudaStream_t st) {
+    if (len && h0) {
+        bigru_set_error("forward: lengths together with an initial hidden state are not supported");
+        return BIGRU_ERR_UNSUPPORTED;
+    }
     if (p.prec == BIGRU_PREC_BF16 && h0) {
         bigru_set_error("BIGRU_PREC_BF16: an initial hidden state is not supported; use BIGRU_PREC_FP32 or BIGRU_PREC_BF16X3");
         return BIGRU_ERR_UNSUPPORTED;
@@ -384,7 +389,7 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
                 const Planes yp = plan_planes(p, buf.YP[l], 0, (int64_t)D * H, BT, 1, (int64_t)D * H);
                 yh = mut(yp); yl = mut_lo(yp);
             }
-            TRY(tc_scan_fwd(p, l, buf.gi, params + p.off_whh(l, 0), params + p.off_bhh(l, 0), h0l, Y, G, hnl, yh, yl, st));
+            TRY(tc_scan_fwd(p, l, buf.gi, params + p.off_whh(l, 0), params + p.off_bhh(l, 0), h0l, Y, G, hnl, yh, yl, len, st));
             inp = Y;
             continue;
         }
@@ -414,11 +419,11 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
                 TRY(sgemm_launch(r, st));
             }
             KLAUNCH(KC_GATES_FWD, 0.0, 0.0, st, gru_gates_fwd_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(buf.gi, buf.gh, h0l, Y, G,
-                                                                              hnl, B, T, H, D, s));
+                                                                              hnl, B, T, H, D, s, len));
         }
         inp = Y;
     }
-    KLAUNCH(KC_HEAD, 0.0, 0.0, st, head_pool_kernel<<<nblk((int64_t)B * H, 128), 128, 0, st>>>(buf.Y[p.L - 1], buf.cat, (int*)buf.arg, B, T, H, D));
+    KLAUNCH(KC_HEAD, 0.0, 0.0, st, head_pool_kernel<<<nblk((int64_t)B * H, 128), 128, 0, st>>>(buf.Y[p.L - 1], buf.cat, (int*)buf.arg, B, T, H, D, len));
     GemmArgs lin = gemm_args(buf.cat, params + p.off_linw(), logits, B, p.C, 3 * H, 3 * H, 1, 3 * H, 1, p.C);
     lin.bias = params + p.off_linb();
     TRY(plan_gemm(p, lin, KC_HEAD, buf.tcw, st));
@@ -428,9 +433,13 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
 // ------------------------------------------------------------------------------------------
 // backward: the head, then layers L-1 .. 0.  The upstream gradient of layer l lives in dYa when L-1-l is even, else in dYb.
 // ------------------------------------------------------------------------------------------
-static int backward_plan(const bigru_plan& p, const float* params, const float* x, const float* h0, float drop,
+static int backward_plan(const bigru_plan& p, const float* params, const float* x, const float* h0, const int* len, float drop,
                          int spatial, int training, uint64_t seed, const float* stash, float* scratch,
                          const float* dlogits, float* grads, float* dx, float* dh0, cudaStream_t st) {
+    if (len && (h0 || dh0)) {
+        bigru_set_error("backward: lengths together with an initial hidden state or its gradient are not supported");
+        return BIGRU_ERR_UNSUPPORTED;
+    }
     if (p.prec == BIGRU_PREC_BF16 && (h0 || dh0)) {
         bigru_set_error("BIGRU_PREC_BF16: initial hidden state / its gradient are not supported");
         return BIGRU_ERR_UNSUPPORTED;
@@ -450,7 +459,7 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
     GemmArgs w = gemm_args(dlogits, stash + S.cat, grads + p.off_linw(), C, 3 * H, B, 1, C, 1, 3 * H, 3 * H);
     TRY(plan_gemm(p, w, KC_HEAD, tcw, st));
     TRY(colsum_launch(dlogits, grads + p.off_linb(), B, C, C, 1, 0, 0, scratch + W.csum, st));
-    KLAUNCH(KC_HEAD, 0.0, 0.0, st, head_bwd_dy_kernel<<<nblk(BT * H, 256), 256, 0, st>>>(scratch + W.dcat, (const int*)(stash + S.arg), scratch + W.dYa, dhc, B, T, H, D));
+    KLAUNCH(KC_HEAD, 0.0, 0.0, st, head_bwd_dy_kernel<<<nblk(BT * H, 256), 256, 0, st>>>(scratch + W.dcat, (const int*)(stash + S.arg), scratch + W.dYa, dhc, B, T, H, D, len));
     for (int l = p.L - 1; l >= 0; --l) {
         const int I = (int)p.in_size(l);
         const bool even = (p.L - 1 - l) % 2 == 0;
@@ -467,10 +476,10 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
         const Planes ghp = plan_planes(p, scratch, W.dghP, H3, BT, D, H3);
         // recurrence: dgi, dgh [D][B*T][3H] and dh0 in dhc
         if (tc) {
-            TRY(tc_scan_bwd(p, l, G, Y, h0l, dY, dhc, dgi, dgh, params + p.off_whh(l, 0), mut(gip), mut_lo(gip), mut(ghp), mut_lo(ghp), st));
+            TRY(tc_scan_bwd(p, l, G, Y, h0l, dY, dhc, dgi, dgh, params + p.off_whh(l, 0), mut(gip), mut_lo(gip), mut(ghp), mut_lo(ghp), len, st));
         } else {
             for (int s = 0; s < T; ++s) {
-                KLAUNCH(KC_GATES_BWD, 0.0, 0.0, st, gru_gates_bwd_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(G, Y, h0l, dY, dhc, dgi, dgh, B, T, H, D, s));
+                KLAUNCH(KC_GATES_BWD, 0.0, 0.0, st, gru_gates_bwd_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(G, Y, h0l, dY, dhc, dgi, dgh, B, T, H, D, s, len));
                 // dhc[d] += dgh_t[d] W_hh[d]   (rows t: dir0 -> T-1-s, dir1 -> s)
                 const int t0 = T - 1 - s, t1 = s;
                 GemmArgs r = gemm_args(dgh + (int64_t)t0 * 3 * H, params + p.off_whh(l, 0), dhc, B, H, 3 * H,
@@ -495,7 +504,8 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
                 const bool own = l == 0 || do_drop;
                 TRY(wg_gemm(j, gip, true, input_planes(p, stash + (own ? S.XP[l] : S.YP[l - 1]), l, own), true, p.prec, st));
             }
-            // the dgh planes are zero at each sequence's first step, so the ±1-row shift needs no mask
+            // the dgh planes are zero at each sequence's first step, so the ±1-row shift needs no mask.  With lengths they are
+            // zero at padded steps too, and the reverse direction's first step t = len - 1 meets the zero Y plane row of t = len
             if (T > 1) {
                 ProfScope ps(KC_TC_GEMM_DWHH, 2.0 * H3 * H * (double)BT * D, 0.0, st);
                 htc::WgJob j = wg_job(grads + p.off_whh(l, 0), (int)H3, H, H, D, kb);
@@ -569,12 +579,19 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
 extern "C" int bigru_forward(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
                              float dropout_p, int spatial, int training, uint64_t seed, void* d_stash,
                              void* d_scratch, float* d_logits, float* d_hn, void* stream) {
+    return bigru_forward_lengths(plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, d_stash, d_scratch, d_logits,
+                                 d_hn, nullptr, stream);
+}
+
+extern "C" int bigru_forward_lengths(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
+                                     float dropout_p, int spatial, int training, uint64_t seed, void* d_stash,
+                                     void* d_scratch, float* d_logits, float* d_hn, const int32_t* d_lengths, void* stream) {
     if (!plan || !d_params || !d_x || !d_stash || !d_scratch || !d_logits) {
         bigru_set_error("forward: null argument");
         return BIGRU_ERR_ARG;
     }
     if (dropout_p < 0.f || dropout_p >= 1.f) { bigru_set_error("forward: dropout_p must be in [0,1)"); return BIGRU_ERR_ARG; }
-    return forward_plan(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed,
+    return forward_plan(*plan, d_params, d_x, d_h0, d_lengths, dropout_p, spatial, training, seed,
                         train_bufs(*plan, (float*)d_stash, (float*)d_scratch), d_logits, d_hn, (cudaStream_t)stream);
 }
 
@@ -587,23 +604,36 @@ extern "C" int bigru_infer_workspace_bytes(const bigru_plan* p, size_t* bytes) {
 // the eval-mode forward through the same launch sequence as bigru_forward, with the outputs placed by infer_layout
 extern "C" int bigru_infer(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
                            void* d_workspace, float* d_logits, void* stream) {
+    return bigru_infer_lengths(plan, d_params, d_x, d_h0, d_workspace, d_logits, nullptr, stream);
+}
+
+extern "C" int bigru_infer_lengths(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
+                                   void* d_workspace, float* d_logits, const int32_t* d_lengths, void* stream) {
     if (!plan || !d_params || !d_x || !d_workspace || !d_logits) {
         bigru_set_error("infer: null argument");
         return BIGRU_ERR_ARG;
     }
-    return forward_plan(*plan, d_params, d_x, d_h0, 0.f, 0, 0, 0, infer_bufs(*plan, (float*)d_workspace), d_logits, nullptr,
-                        (cudaStream_t)stream);
+    return forward_plan(*plan, d_params, d_x, d_h0, d_lengths, 0.f, 0, 0, 0, infer_bufs(*plan, (float*)d_workspace), d_logits,
+                        nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int bigru_backward(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
                               float dropout_p, int spatial, int training, uint64_t seed, const void* d_stash,
                               void* d_scratch, const float* d_dlogits, float* d_grads, float* d_dx, float* d_dh0,
                               void* stream) {
+    return bigru_backward_lengths(plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, d_stash, d_scratch, d_dlogits,
+                                  d_grads, d_dx, d_dh0, nullptr, stream);
+}
+
+extern "C" int bigru_backward_lengths(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
+                                      float dropout_p, int spatial, int training, uint64_t seed, const void* d_stash,
+                                      void* d_scratch, const float* d_dlogits, float* d_grads, float* d_dx, float* d_dh0,
+                                      const int32_t* d_lengths, void* stream) {
     if (!plan || !d_params || !d_x || !d_stash || !d_scratch || !d_dlogits || !d_grads) {
         bigru_set_error("backward: null argument");
         return BIGRU_ERR_ARG;
     }
-    return backward_plan(*plan, d_params, d_x, d_h0, dropout_p, spatial, training, seed, (const float*)d_stash,
+    return backward_plan(*plan, d_params, d_x, d_h0, d_lengths, dropout_p, spatial, training, seed, (const float*)d_stash,
                          (float*)d_scratch, d_dlogits, d_grads, d_dx, d_dh0, (cudaStream_t)stream);
 }
 

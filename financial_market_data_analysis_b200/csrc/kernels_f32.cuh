@@ -171,12 +171,15 @@ static int colsum_launch(const float* A, float* out, int64_t rows, int cols, int
 // GRU pointwise: forward gates for one time step of both directions.
 //   gi [D][B*T][3H] (input projection + b_ih), gh [D][B][3H] (h_prev W_hh^T + b_hh)
 //   Y [B][T][D*H] layer output; G [D][B*T][4H] stash of (r, z, n, gh_n), null when no backward follows (inference)
+//   len: per-row lengths [B] or null.  A padded (row, t >= len) writes Y = 0 and no G; hn is the state at the row's last
+//   valid step.  The reverse direction reads h_prev = Y(len) = 0 at t = len - 1: the zero initial state.
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.f / (1.f + expf(-x)); }
 
 __global__ void gru_gates_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ gh,
                                      const float* __restrict__ h0, float* __restrict__ Y, float* __restrict__ G,
-                                     float* __restrict__ hn_out, int B, int T, int H, int D, int s) {
+                                     float* __restrict__ hn_out, int B, int T, int H, int D, int s,
+                                     const int* __restrict__ len) {
     const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t total = (int64_t)D * B * H;
     if (idx >= total) return;
@@ -195,19 +198,25 @@ __global__ void gru_gates_fwd_kernel(const float* __restrict__ gi, const float* 
     const float hn = ghr[2 * H + j];
     const float n = tanhf(gir[2 * H + j] + r * hn);
     const float h = (1.f - z) * n + z * hp;
+    const int n_b = len ? len[b] : T;
+    if (t >= n_b) {
+        Y[row * D * H + d * H + j] = 0.f;
+        return;
+    }
     Y[row * D * H + d * H + j] = h;
     if (G) {
         float* g = G + ((int64_t)d * B * T + row) * 4 * H;
         g[j] = r; g[H + j] = z; g[2 * H + j] = n; g[3 * H + j] = hn;
     }
-    if (hn_out && s == T - 1) hn_out[((int64_t)d * B + b) * H + j] = h;
+    if (hn_out && (d == 0 ? t == n_b - 1 : s == T - 1)) hn_out[((int64_t)d * B + b) * H + j] = h;
 }
 
-// backward gates for one step: consumes dh carry + dY_t, emits dgi/dgh rows and dh*z
+// backward gates for one step: consumes dh carry + dY_t, emits dgi/dgh rows and dh*z.  At a padded (row, t >= len[b]):
+// dgi = dgh = 0 and the carry passes through unchanged
 __global__ void gru_gates_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y,
                                      const float* __restrict__ h0, const float* __restrict__ dY,
                                      float* __restrict__ dhc, float* __restrict__ dgi, float* __restrict__ dgh,
-                                     int B, int T, int H, int D, int s) {
+                                     int B, int T, int H, int D, int s, const int* __restrict__ len) {
     const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t total = (int64_t)D * B * H;
     if (idx >= total) return;
@@ -216,6 +225,13 @@ __global__ void gru_gates_bwd_kernel(const float* __restrict__ G, const float* _
     const int d = idx / ((int64_t)H * B);
     const int t = d == 0 ? T - 1 - s : s;
     const int64_t row = (int64_t)b * T + t;
+    if (len && t >= len[b]) {
+        float* a = dgi + ((int64_t)d * B * T + row) * 3 * H;
+        float* c = dgh + ((int64_t)d * B * T + row) * 3 * H;
+        a[j] = a[H + j] = a[2 * H + j] = 0.f;
+        c[j] = c[H + j] = c[2 * H + j] = 0.f;
+        return;
+    }
     const float* g = G + ((int64_t)d * B * T + row) * 4 * H;
     const float r = g[j], z = g[H + j], n = g[2 * H + j], hn = g[3 * H + j];
     const bool first = d == 0 ? t == 0 : t == T - 1;
@@ -235,39 +251,45 @@ __global__ void gru_gates_bwd_kernel(const float* __restrict__ G, const float* _
 }
 
 // ------------------------------------------------------------------------------------------
-// Head (biGRU_model.py:111-133): direction sum, last hidden, max / mean pooling over T.
+// Head (biGRU_model.py:111-133): direction sum, last hidden, max / mean pooling over T.  len: per-row lengths [B] or
+// null; row b pools over its valid steps t < len[b] and its forward direction's last hidden is at t = len[b] - 1.
 // ------------------------------------------------------------------------------------------
 __global__ void head_pool_kernel(const float* __restrict__ Y, float* __restrict__ cat, int* __restrict__ arg,
-                                 int B, int T, int H, int D) {
+                                 int B, int T, int H, int D, const int* __restrict__ len) {
     const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= (int64_t)B * H) return;
     const int j = idx % H, b = idx / H;
     const float* y = Y + (int64_t)b * T * D * H;
-    float last = y[(int64_t)(T - 1) * D * H + j];
+    const int n_b = len ? len[b] : T;
+    float last = y[(int64_t)(n_b - 1) * D * H + j];
     if (D == 2) last += y[H + j];
     float mx = -INFINITY, sum = 0.f;
     int am = 0;
-    for (int t = 0; t < T; ++t) {
+    for (int t = 0; t < n_b; ++t) {
         float s = y[(int64_t)t * D * H + j];
         if (D == 2) s += y[(int64_t)t * D * H + H + j];
         if (s > mx) { mx = s; am = t; }
         sum += s;
     }
     float* c = cat + (int64_t)b * 3 * H;
-    c[j] = last; c[H + j] = mx; c[2 * H + j] = sum / (float)T;
+    c[j] = last; c[H + j] = mx; c[2 * H + j] = sum / (float)n_b;
     arg[idx] = am;
 }
 
-// dY of the top layer from d(concat): mean + routed max;  dhc (carry) = d(last_hidden) for both dirs
+// dY of the top layer from d(concat): mean + routed max;  dhc (carry) = d(last_hidden) for both dirs.  With lengths, dY is 0
+// at padded steps; the forward direction's carry passes through them unchanged (the scans' padded steps) and so enters at
+// t = len - 1, where its `last` was taken.
 __global__ void head_bwd_dy_kernel(const float* __restrict__ dcat, const int* __restrict__ arg,
-                                   float* __restrict__ dY, float* __restrict__ dhc, int B, int T, int H, int D) {
+                                   float* __restrict__ dY, float* __restrict__ dhc, int B, int T, int H, int D,
+                                   const int* __restrict__ len) {
     const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= (int64_t)B * T * H) return;
     const int j = idx % H;
     const int t = (idx / H) % T;
     const int b = idx / ((int64_t)H * T);
     const float* dc = dcat + (int64_t)b * 3 * H;
-    const float v = dc[2 * H + j] / (float)T + (arg[(int64_t)b * H + j] == t ? dc[H + j] : 0.f);
+    const int n_b = len ? len[b] : T;
+    const float v = t >= n_b ? 0.f : dc[2 * H + j] / (float)n_b + (arg[(int64_t)b * H + j] == t ? dc[H + j] : 0.f);
     float* o = dY + ((int64_t)b * T + t) * D * H;
     o[j] = v;
     if (D == 2) o[H + j] = v;

@@ -344,6 +344,9 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ part, int splits,
 // OUT selects at compile time which of Y, G and the Y planes are written (hn_out is written whenever it is non-null): the
 // training forward keeps all three for the backward; inference writes the planes of a lower layer (the next projection reads
 // them) and the fp32 Y of the top layer (the pooling head reads it).  The h arithmetic is the same in every instantiation.
+// LEN: per-sequence lengths (lens [B], 1 <= len <= T).  A padded (row, t >= len) keeps its state (hp and the h tile) and skips
+// G; its Y row and Y plane rows are 0, so the reverse direction stays at the zero state until t = len - 1 and hn is the state
+// after the row's last valid step.  Without LEN the kernel is the one without lengths, instruction for instruction.
 // ------------------------------------------------------------------------------------------------------
 constexpr int SCAN_U = 64, SCAN_NB = 16, SCAN_THREADS = 256;
 constexpr int SCAN_Y = 1, SCAN_G = 2, SCAN_PLANES = 4;
@@ -358,13 +361,14 @@ struct FwdSmem {
     static constexpr int TOTAL = NH * WBYTES + 2 * NH * HBYTES;
 };
 
-template <int H, int NS, int OUT>
+template <int H, int NS, int OUT, bool LEN>
 __global__ void __launch_bounds__(SCAN_THREADS, 1)
 gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh, const float* __restrict__ bhh, int64_t zW,
                     const float* __restrict__ h0, float* __restrict__ Y, float* __restrict__ G, float* __restrict__ hn_out,
-                    bf16_t* __restrict__ yh, bf16_t* __restrict__ yl, int B, int T, int D) {
+                    bf16_t* __restrict__ yh, bf16_t* __restrict__ yl, int B, int T, int D, const int* __restrict__ lens) {
     using S = FwdSmem<H, NS>;
     constexpr int U = SCAN_U, CS = H / U, NH = S::NH;
+    static_assert(SCAN_THREADS % (SCAN_NB * (U / 8)) == 0, "a thread copies the same Y plane row in every pass");
     extern __shared__ __align__(128) uint8_t smem[];
     uint8_t* Wsm = smem;                                     // [NH][3U rows][H]
     uint8_t* Hsm = smem + NH * S::WBYTES;                    // [2 buffers][NH][NB rows][H]
@@ -403,6 +407,13 @@ gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh,
     for (int e = 0; e < 4; ++e) {
         const int b = bt0 + bcol[e & 1], j = c * U + unit[e >> 1];
         hp[e] = h0 ? h0[((int64_t)d * B + b) * H + j] : 0.f;
+    }
+    // lengths of this thread's two batch columns, and of the row it copies to the Y planes (the same row in every pass of
+    // the copy loop: SCAN_THREADS is a multiple of SCAN_NB * U / 8)
+    int len[2] = {T, T}, rlen = T;
+    if (LEN) {
+        len[0] = lens[bt0 + bcol[0]]; len[1] = lens[bt0 + bcol[1]];
+        rlen = lens[bt0 + (tid / (U / 8)) % SCAN_NB];
     }
     // every CTA of the cluster has started and staged its tiles before any distributed-shared-memory store
     cluster_arrive();
@@ -454,11 +465,12 @@ gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh,
             const float z = sigmoid_f(giv[1][e] + acc[1][e] + bias[1][e >> 1]);
             const float hnv = acc[2][e] + bias[2][e >> 1];
             const float n = tanhf(giv[2][e] + r * hnv);
-            const float h = (1.f - z) * n + z * hp[e];
+            const bool pad = LEN && t >= len[e & 1];
+            const float h = pad ? hp[e] : (1.f - z) * n + z * hp[e];
             hp[e] = h;
             const int64_t row = (int64_t)b * T + t;
-            if (OUT & SCAN_Y) Y[row * DH + d * H + j] = h;
-            if (OUT & SCAN_G) {
+            if (OUT & SCAN_Y) Y[row * DH + d * H + j] = pad ? 0.f : h;
+            if ((OUT & SCAN_G) && !pad) {
                 float* gs = G + ((int64_t)d * B * T + row) * 4 * H + j;
                 gs[0] = r; gs[H] = z; gs[2 * H] = n; gs[3 * H] = hnv;
             }
@@ -476,11 +488,13 @@ gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh,
         cluster_arrive();
         cluster_wait();
         // the Y planes of this CTA's units: h_t is now in the h tile (hi / lo, every unit), so copy the own slice out with
-        // 16-byte stores.  Nobody writes this buffer again before the next step's barrier.
+        // 16-byte stores.  Nobody writes this buffer again before the next step's barrier.  A padded row's tile holds the
+        // carried state: its plane rows are zeros.
         if (OUT & SCAN_PLANES) {
             for (int i = tid; i < NH * SCAN_NB * (U / 8); i += SCAN_THREADS) {
                 const int h = i / (SCAN_NB * U / 8), r = (i / (U / 8)) % SCAN_NB, k = c * U + (i % (U / 8)) * 8;
-                const uint4 v = *reinterpret_cast<const uint4*>(Hsm + (nbuf * NH + h) * S::HBYTES + swz<H * 2>(r, k));
+                uint4 v = *reinterpret_cast<const uint4*>(Hsm + (nbuf * NH + h) * S::HBYTES + swz<H * 2>(r, k));
+                if (LEN && t >= rlen) v = make_uint4(0u, 0u, 0u, 0u);
                 *reinterpret_cast<uint4*>((h ? yl : yh) + ((int64_t)(bt0 + r) * T + t) * DH + d * H + k) = v;
             }
         }
@@ -496,6 +510,8 @@ gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh,
 // peers' partial sums [CS-1][16][64] fp32 (this CTA's own partial goes into the dgh tile's space, which is free by then).
 // Cluster barrier phases per step: (1) partials of the step have landed; (2) every CTA has read its receive slots, so
 // the next step's partials may be written.
+// LEN: at a padded (row, t >= lens[b]) dgi and dgh are 0 (fp32 and planes) and dh passes through unchanged: its dgh row
+// adds exact zeros to the partial sums.  The barriers and the exchange are those of every step.
 // ------------------------------------------------------------------------------------------------------
 template <int H, int NS>
 struct BwdSmem {
@@ -509,12 +525,12 @@ struct BwdSmem {
     static_assert(NH * DBYTES >= SLOT, "own partial sums alias the dgh tile");
 };
 
-template <int H, int NS>
+template <int H, int NS, bool LEN>
 __global__ void __launch_bounds__(SCAN_THREADS, 1)
 gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, const float* __restrict__ h0,
                     const float* __restrict__ dY, float* __restrict__ dhc, float* __restrict__ dgi, float* __restrict__ dgh,
                     const float* __restrict__ Whh, int64_t zW, bf16_t* __restrict__ gih, bf16_t* __restrict__ gil,
-                    bf16_t* __restrict__ ghh, bf16_t* __restrict__ ghl, int B, int T, int D) {
+                    bf16_t* __restrict__ ghh, bf16_t* __restrict__ ghl, int B, int T, int D, const int* __restrict__ lens) {
     using S = BwdSmem<H, NS>;
     constexpr int U = SCAN_U, CS = H / U, NH = S::NH, Q = S::Q, NB = SCAN_NB;
     constexpr int MT = H / 16 / 8;                           // m-tiles (16 rows of W^T) per warp
@@ -539,11 +555,13 @@ gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, co
         if (NH == 2) *reinterpret_cast<bf16_t*>(Wsm + S::WBYTES + swz<S::WP>(k, q)) = lo;
     }
     float dhr[PAIRS], dhz[PAIRS];
+    int plen[PAIRS];
 #pragma unroll
     for (int i = 0; i < PAIRS; ++i) {
         const int p = tid + i * SCAN_THREADS, u = p % U, b = p / U;
         dhr[i] = dhc[((int64_t)d * B + bt0 + b) * H + c * U + u];
         dhz[i] = 0.f;
+        plen[i] = LEN ? lens[bt0 + b] : T;
     }
     cluster_arrive();
     cluster_wait();
@@ -574,15 +592,17 @@ gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, co
             if (first) hpv = h0 ? h0[((int64_t)d * B + b) * H + j] : 0.f;
             else hpv = Y[((int64_t)b * T + (d == 0 ? t - 1 : t + 1)) * DH + d * H + j];
             const float dh = dhr[i] + dY[row * DH + d * H + j];
-            const float dan = dh * (1.f - z) * (1.f - n * n);
-            const float dar = dan * hnv * r * (1.f - r);
-            const float daz = dh * (hpv - n) * z * (1.f - z);
-            const float dgn = dan * r;
+            float dan = dh * (1.f - z) * (1.f - n * n);
+            float dar = dan * hnv * r * (1.f - r);
+            float daz = dh * (hpv - n) * z * (1.f - z);
+            float dgn = dan * r;
+            const bool pad = LEN && t >= plen[i];
+            if (pad) dan = dar = daz = dgn = 0.f;
             float* a = dgi + ((int64_t)d * B * T + row) * 3 * H + j;
             float* cg = dgh + ((int64_t)d * B * T + row) * 3 * H + j;
             a[0] = dar; a[H] = daz; a[2 * H] = dan;
             cg[0] = dar; cg[H] = daz; cg[2 * H] = dgn;
-            dhz[i] = dh * z;
+            dhz[i] = pad ? dhr[i] : dh * z;
             const float gv[3] = {dar, daz, dgn};
 #pragma unroll
             for (int gte = 0; gte < 3; ++gte) {
@@ -828,31 +848,33 @@ static int launch_cluster(void (*kernel)(KArgs...), int cs, int ntiles, int D, i
     return BIGRU_OK;
 }
 
-template <int HH, int NS>
+template <int HH, int NS, bool LEN>
 static int scan_fwd_launch(int out, int cs, int nt, int D, cudaStream_t st, const float* gi, const float* Whh, const float* bhh,
-                           int64_t zW, const float* h0, float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, int B, int T) {
+                           int64_t zW, const float* h0, float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, int B, int T,
+                           const int* len) {
     constexpr int smem = htc::FwdSmem<HH, NS>::TOTAL;
     switch (out) {
         case htc::SCAN_TRAIN:
-            return launch_cluster(htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_TRAIN>, cs, nt, D, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D);
+            return launch_cluster(htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_TRAIN, LEN>, cs, nt, D, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D, len);
         case htc::SCAN_INFER_LOWER:
-            return launch_cluster(htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_INFER_LOWER>, cs, nt, D, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D);
+            return launch_cluster(htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_INFER_LOWER, LEN>, cs, nt, D, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D, len);
         case htc::SCAN_INFER_TOP:
-            return launch_cluster(htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_INFER_TOP>, cs, nt, D, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D);
+            return launch_cluster(htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_INFER_TOP, LEN>, cs, nt, D, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D, len);
     }
     bigru_set_error("tc_scan_fwd: no kernel writes this set of outputs (Y %d, G %d, planes %d)", Y != nullptr, G != nullptr, yh != nullptr);
     return BIGRU_ERR_ARG;
 }
 
 // one layer's forward recurrence; shapes were validated by the plan (H in {128, 256, 512}, B % 16 == 0).  A null Y, G or yh:
-// that output is not written (the instantiations: all three, planes only, Y only)
+// that output is not written (the instantiations: all three, planes only, Y only).  len: per-row lengths [B] or null
 static int tc_scan_fwd(const bigru_plan& p, int l, const float* gi, const float* Whh, const float* bhh, const float* h0,
-                       float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, cudaStream_t st) {
+                       float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, const int* len, cudaStream_t st) {
     const int H = p.H, D = p.D, B = p.B, T = p.T, cs = H / htc::SCAN_U, nt = B / htc::SCAN_NB;
     const int64_t zW = p.ld_block(l);
     const int out = (Y ? htc::SCAN_Y : 0) | (G ? htc::SCAN_G : 0) | (yh ? htc::SCAN_PLANES : 0);
     ProfScope ps(KC_TC_SCAN_FWD, 2.0 * D * B * (double)T * 3 * H * H, 0.0, st);
-#define FWD(HH, NS) return scan_fwd_launch<HH, NS>(out, cs, nt, D, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T)
+#define FWD(HH, NS) return len ? scan_fwd_launch<HH, NS, true>(out, cs, nt, D, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, len) \
+                               : scan_fwd_launch<HH, NS, false>(out, cs, nt, D, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, len)
     if (p.prec == BIGRU_PREC_BF16X3) {
         if (H == 128) FWD(128, 3);
         if (H == 256) FWD(256, 3);
@@ -868,11 +890,12 @@ static int tc_scan_fwd(const bigru_plan& p, int l, const float* gi, const float*
 
 static int tc_scan_bwd(const bigru_plan& p, int l, const float* G, const float* Y, const float* h0, const float* dY, float* dhc,
                        float* dgi, float* dgh, const float* Whh, htc::bf16_t* gih, htc::bf16_t* gil, htc::bf16_t* ghh,
-                       htc::bf16_t* ghl, cudaStream_t st) {
+                       htc::bf16_t* ghl, const int* len, cudaStream_t st) {
     const int H = p.H, D = p.D, B = p.B, T = p.T, cs = H / htc::SCAN_U, nt = B / htc::SCAN_NB;
     const int64_t zW = p.ld_block(l);
     ProfScope ps(KC_TC_SCAN_BWD, 2.0 * D * B * (double)T * 3 * H * H, 0.0, st);
-#define BWD(HH, NS) return launch_cluster(htc::gru_scan_bwd_kernel<HH, NS>, cs, nt, D, htc::BwdSmem<HH, NS>::TOTAL, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D)
+#define BWD(HH, NS) return len ? launch_cluster(htc::gru_scan_bwd_kernel<HH, NS, true>, cs, nt, D, htc::BwdSmem<HH, NS>::TOTAL, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, len) \
+                           : launch_cluster(htc::gru_scan_bwd_kernel<HH, NS, false>, cs, nt, D, htc::BwdSmem<HH, NS>::TOTAL, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, len)
     if (p.prec == BIGRU_PREC_BF16X3) {
         if (H == 128) BWD(128, 3);
         if (H == 256) BWD(256, 3);

@@ -93,7 +93,8 @@ int  bigru_stash_output_offset(const bigru_plan* plan, int layer, size_t* byte_o
  *                                               bigru_forward, layer 0 always, layers above only in training with dropout
  *   BIGRU_WS_DGI, _DGH      scratch  0          dgi, dgh [D][B*T][3H] fp32 of layer 0; bigru_backward (each layer reuses them)
  *   BIGRU_WS_DGI_PLANES,    scratch  0          their planes; dgi's n-gate rows hold dan, the dgh rows are zero at each
- *   BIGRU_WS_DGH_PLANES                         sequence's first step (t = 0 forward, t = T-1 reverse); bigru_backward
+ *   BIGRU_WS_DGH_PLANES                         sequence's first step (t = 0 forward, t = T-1 reverse); bigru_backward.
+ *                                               With lengths, these and the Y planes are zero at padded steps
  *   BIGRU_WS_DY             scratch  0, 1       upstream gradient of the layer's output [B*T][D*H]; bigru_backward
  *   BIGRU_WS_DHC            scratch  0          dh_{-1} of layer 0 [D][B][H]; bigru_backward
  *   BIGRU_WS_DCAT           scratch  L (head)   d cat [B][3H] (last | max | mean); bigru_backward
@@ -129,6 +130,26 @@ int  bigru_forward(const bigru_plan* plan, const float* d_params, const float* d
 int  bigru_infer_workspace_bytes(const bigru_plan* plan, size_t* bytes);
 int  bigru_infer(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
                  void* d_workspace, float* d_logits, void* stream);
+
+/* --- per-sequence lengths (torch.nn.utils.rnn.pack_padded_sequence semantics) for bigru_forward, bigru_infer and
+ *  bigru_backward: the same arguments plus d_lengths, a DEVICE int32 [B] or NULL (every row T steps long; then each call is
+ *  exactly its twin without lengths).  Row b's valid steps are t < d_lengths[b], with 1 <= d_lengths[b] <= T; its inputs at
+ *  t >= d_lengths[b] are ignored (any finite values).  Every layer runs as nn.GRU on the packed sequence: layer outputs are
+ *  0 at padded steps, the reverse direction starts from the zero state at t = len - 1, d_hn holds the state after each
+ *  direction's last valid step; the head takes `last` at t = len - 1 (forward direction) and t = 0 (reverse), and max- and
+ *  mean-pools over t < len.  The backward is the gradient of that function: d_dx is 0 at padded steps.  A backward must get
+ *  the d_lengths of its forward.  The library does not read d_lengths on the host: the caller guarantees the range (the
+ *  Python mirror checks it).  d_lengths together with d_h0 or d_dh0: BIGRU_ERR_UNSUPPORTED. */
+int  bigru_forward_lengths(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
+                           float dropout_p, int spatial, int training, uint64_t seed,
+                           void* d_stash, void* d_scratch, float* d_logits, float* d_hn, const int32_t* d_lengths,
+                           void* stream);
+int  bigru_infer_lengths(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
+                         void* d_workspace, float* d_logits, const int32_t* d_lengths, void* stream);
+int  bigru_backward_lengths(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
+                            float dropout_p, int spatial, int training, uint64_t seed,
+                            const void* d_stash, void* d_scratch, const float* d_dlogits,
+                            float* d_grads, float* d_dx, float* d_dh0, const int32_t* d_lengths, void* stream);
 
 /* --- loss.backward() through the model (biGRU_model.py:204): every parameter gradient into
  *  d_grads (flat, overwritten), optional d_dx[B,T,F] and d_dh0[L*D,B,H].  d_x (required) is the
