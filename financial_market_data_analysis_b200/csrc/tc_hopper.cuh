@@ -8,8 +8,9 @@
 //   * gru_scan_fwd_kernel - one layer's whole forward recurrence in one launch: a thread-block cluster per (direction,
 //                           16-row batch tile); CTA c of the cluster owns hidden units [64c, 64c+64) and keeps their W_hh
 //                           rows (3 gates x 64 units x H) resident in shared memory for all T steps.  Each step it multiplies
-//                           them with h_{t-1} of the tile, runs the gate math in registers and writes its slice of h_t into
-//                           the shared memory of every CTA of the cluster (distributed shared memory), then a cluster barrier.
+//                           them with h_{t-1} of the tile, runs the gate math in registers and bulk-copies its slice of h_t
+//                           into the shared memory of every CTA of the cluster (distributed shared memory), where an
+//                           mbarrier counts the bytes in.
 //   * gru_scan_bwd_kernel - the backward recurrence, reduction-partitioned: CTA c keeps W_hh^T restricted to its own units'
 //                           gate rows (H x 192), multiplies it with its local dgh tile and sends each peer the fp32 partial
 //                           sums of dh_{t-1} for the peer's units; the owner adds them up.
@@ -64,11 +65,8 @@ __device__ __forceinline__ uint32_t mapa(uint32_t local_addr, uint32_t cta) {
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(cta));
     return r;
 }
-__device__ __forceinline__ void st_cluster_b16(uint32_t addr, bf16_t v) {
-    asm volatile("st.shared::cluster.b16 [%0], %1;" ::"r"(addr), "h"(__bfloat16_as_ushort(v)) : "memory");
-}
-__device__ __forceinline__ void st_cluster_f32(uint32_t addr, float v) {
-    asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
+__device__ __forceinline__ void st_cluster_v2_f32(uint32_t addr, float2 v) {
+    asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(v.x), "f"(v.y) : "memory");
 }
 __device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release;" ::: "memory"); }
 __device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire;" ::: "memory"); }
@@ -147,19 +145,35 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
         "selp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
     return ok != 0;
 }
+// the same with acquire at cluster scope: the phase's bytes were written by peer CTAs' bulk copies
+__device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
+    uint32_t ok;
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
+    return ok != 0;
+}
 // a wait that has not completed after 5 s of wall clock means the pipeline protocol is broken: stop the kernel (the launch
 // reports an error) rather than occupy the GPU
+template <bool CLUSTER = false>
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    if (mbar_try_wait(bar, parity)) return;
+    auto ready = [&] { return CLUSTER ? mbar_try_wait_cluster(bar, parity) : mbar_try_wait(bar, parity); };
+    if (ready()) return;
     uint64_t t0, t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
     for (uint32_t i = 0;; ++i) {
-        if (mbar_try_wait(bar, parity)) return;
+        if (ready()) return;
         if ((i & 1023u) == 1023u) {
             asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
             if (t - t0 > 5000000000ull) __trap();
         }
     }
+}
+// bytes from this CTA's shared memory to CTA `cta` of the cluster, at the same offsets; completes on that CTA's mbarrier
+__device__ __forceinline__ void bulk_copy_to_peer(uint32_t src, uint32_t bytes, uint64_t* bar, uint32_t cta) {
+    asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 ::"r"(mapa(src, cta)), "r"(src), "r"(bytes), "r"(mapa(smem_u32(bar), cta)) : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
@@ -341,6 +355,10 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ part, int splits,
 // read them.
 // Grid (CS, B/16, D), cluster (CS, 1, 1), 256 threads.  Warp w owns units 16*(w/2) .. +16 of the CTA's slice and batch
 // columns 8*(w%2) .. +8: its r, z and n accumulators hold the same (unit, column) pairs, so the gate math needs no exchange.
+// The h tile is double-buffered and laid out [buf][NH][CS][16 rows][64 units]: CTA c's part of a plane is one 2 KB block at
+// the same offset in every CTA.  Each step a CTA writes its h_t into its own block of the next buffer, and one thread sends
+// that block to every peer with a bulk copy, which completes on the peer's per-buffer "full" mbarrier.  Before its next
+// multiply a CTA waits on that barrier for the (CS - 1) blocks of its peers; there is no cluster barrier per step.
 // OUT selects at compile time which of Y, G and the Y planes are written (hn_out is written whenever it is non-null): the
 // training forward keeps all three for the backward; inference writes the planes of a lower layer (the next projection reads
 // them) and the fp32 Y of the top layer (the pooling head reads it).  The h arithmetic is the same in every instantiation.
@@ -358,8 +376,15 @@ struct FwdSmem {
     static constexpr int WP = H * 2;                        // W row pitch (bytes): K = H
     static constexpr int WBYTES = 3 * SCAN_U * WP;          // one of hi / lo
     static constexpr int HBYTES = SCAN_NB * H * 2;          // h tile, one of hi / lo
-    static constexpr int TOTAL = NH * WBYTES + 2 * NH * HBYTES;
+    static constexpr int SLICE = SCAN_NB * SCAN_U * 2;      // one CTA's units of one h plane: 16 rows x 128 B
+    static constexpr int TOTAL = NH * WBYTES + 2 * NH * HBYTES + 2 * 8;   // + the two buffers' full barriers
 };
+
+// byte offset of h element (row b, unit k) in one buffer plane of the forward h tile: 128-byte rows within the 2 KB block
+// of the units' CTA, chunks XOR-swizzled as in swz
+__device__ __forceinline__ uint32_t hsw(int b, int k) {
+    return (uint32_t)((k / SCAN_U) * (SCAN_NB * SCAN_U * 2)) + swz<SCAN_U * 2>(b, k % SCAN_U);
+}
 
 template <int H, int NS, int OUT, bool LEN>
 __global__ void __launch_bounds__(SCAN_THREADS, 1)
@@ -371,7 +396,8 @@ gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh,
     static_assert(SCAN_THREADS % (SCAN_NB * (U / 8)) == 0, "a thread copies the same Y plane row in every pass");
     extern __shared__ __align__(128) uint8_t smem[];
     uint8_t* Wsm = smem;                                     // [NH][3U rows][H]
-    uint8_t* Hsm = smem + NH * S::WBYTES;                    // [2 buffers][NH][NB rows][H]
+    uint8_t* Hsm = smem + NH * S::WBYTES;                    // [2 buffers][NH][CS][NB rows][U]
+    uint64_t* full = reinterpret_cast<uint64_t*>(Hsm + 2 * NH * S::HBYTES);   // [2 buffers]
     const int c = (int)cluster_rank(), tile = blockIdx.y, d = blockIdx.z;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int bt0 = tile * SCAN_NB;
@@ -390,8 +416,13 @@ gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh,
         const float v = h0 ? h0[((int64_t)d * B + bt0 + b) * H + k] : 0.f;
         bf16_t hi, lo;
         split_bf16(v, hi, lo);
-        *reinterpret_cast<bf16_t*>(Hsm + swz<H * 2>(b, k)) = hi;
-        if (NH == 2) *reinterpret_cast<bf16_t*>(Hsm + S::HBYTES + swz<H * 2>(b, k)) = lo;
+        *reinterpret_cast<bf16_t*>(Hsm + hsw(b, k)) = hi;
+        if (NH == 2) *reinterpret_cast<bf16_t*>(Hsm + S::HBYTES + hsw(b, k)) = lo;
+    }
+    if (tid == 0) {
+        mbar_init(full, 1);
+        mbar_init(full + 1, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
 
     const int ug = warp >> 1, nt = warp & 1;
@@ -415,14 +446,27 @@ gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh,
         len[0] = lens[bt0 + bcol[0]]; len[1] = lens[bt0 + bcol[1]];
         rlen = lens[bt0 + (tid / (U / 8)) % SCAN_NB];
     }
-    // every CTA of the cluster has started and staged its tiles before any distributed-shared-memory store
+    // every CTA of the cluster has started, staged its tiles and initialised its barriers before any bulk copy
     cluster_arrive();
     cluster_wait();
 
+    // Step s multiplies with buffer buf = s & 1 (h_{s-1}; h0 at s = 0) and produces h_s in buffer nbuf = buf ^ 1.  Each
+    // buffer's full barrier completes every other step, so the wait at step s >= 1 is for phase (s - 1) / 2 of full[buf].
+    // The last step sends nothing: only its own block is read (Y planes).
+    // Write after read on the double buffer: a peer sends its h_{s+1} into this CTA's buffer buf (the one step s reads)
+    // only after its own full barrier for h_s has completed, which needs this CTA's h_s, which this CTA sends only after the
+    // __syncthreads that follows its step-s multiply.  So every read of buffer buf is ordered before the copy that
+    // overwrites it (the copy's complete_tx releases at cluster scope, the peer's wait acquires at cluster scope).
+    // Likewise the own block of a buffer is rewritten at step s + 2 only after this CTA's full barrier for h_{s+1}
+    // completed, which needs every peer's h_{s+1}, which each peer computed after receiving all of this CTA's step-s copy:
+    // the bulk copies that read it are done.
     const int DH = D * H;
     for (int s = 0; s < T; ++s) {
         const int t = d == 0 ? s : T - 1 - s;
         const int buf = s & 1;
+        // the peers' blocks of h_{s-1} have landed; and the barrier of the buffer this step fills expects theirs of h_s
+        if (s > 0) mbar_wait<true>(full + buf, ((s - 1) >> 1) & 1);
+        if (tid == 0 && s + 1 < T) mbar_arrive_expect_tx(full + (buf ^ 1), (CS - 1) * NH * S::SLICE);
         float giv[3][4];
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
@@ -443,7 +487,7 @@ gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh,
             uint32_t bh[NH][2];
             const int brow = nt * 8 + (lane & 7), bk = ks * 16 + ((lane >> 3) & 1) * 8;
 #pragma unroll
-            for (int h = 0; h < NH; ++h) ldsm_x2(hbase + h * S::HBYTES + swz<H * 2>(brow, bk), bh[h]);
+            for (int h = 0; h < NH; ++h) ldsm_x2(hbase + h * S::HBYTES + hsw(brow, bk), bh[h]);
 #pragma unroll
             for (int gte = 0; gte < 3; ++gte) {
                 const int arow = gte * U + ug * 16 + (lane & 15), ak = ks * 16 + (lane >> 4) * 8;
@@ -477,28 +521,37 @@ gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh,
             if (hn_out && s == T - 1) hn_out[((int64_t)d * B + b) * H + j] = h;
             bf16_t hi, lo;
             split_bf16(h, hi, lo);
-            const uint32_t off = swz<H * 2>(bcol[e & 1], j);
-            const uint32_t la = smem_u32(Hsm + nbuf * NH * S::HBYTES) + off;
+            uint8_t* la = Hsm + nbuf * NH * S::HBYTES + hsw(bcol[e & 1], j);
+            *reinterpret_cast<bf16_t*>(la) = hi;
+            if (NH == 2) *reinterpret_cast<bf16_t*>(la + S::HBYTES) = lo;
+        }
+        // the own block of h_s is complete; make it visible to the bulk copies (async proxy), then send it to every peer
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        __syncthreads();
+        const uint32_t own = smem_u32(Hsm + nbuf * NH * S::HBYTES + c * S::SLICE);
+        if (tid == 0 && s + 1 < T) {
 #pragma unroll
-            for (int p = 0; p < CS; ++p) {
-                st_cluster_b16(mapa(la, p), hi);
-                if (NH == 2) st_cluster_b16(mapa(la + S::HBYTES, p), lo);
+            for (int p = 1; p < CS; ++p) {
+                const uint32_t dst = (c + p) % CS;
+#pragma unroll
+                for (int h = 0; h < NH; ++h) bulk_copy_to_peer(own + h * S::HBYTES, S::SLICE, full + nbuf, dst);
             }
         }
-        cluster_arrive();
-        cluster_wait();
-        // the Y planes of this CTA's units: h_t is now in the h tile (hi / lo, every unit), so copy the own slice out with
-        // 16-byte stores.  Nobody writes this buffer again before the next step's barrier.  A padded row's tile holds the
-        // carried state: its plane rows are zeros.
+        // the Y planes of this CTA's units from its own block, 16-byte stores, while the copies are in flight.  The block
+        // is rewritten two steps later (see above).  A padded row's tile holds the carried state: its plane rows are zeros.
         if (OUT & SCAN_PLANES) {
             for (int i = tid; i < NH * SCAN_NB * (U / 8); i += SCAN_THREADS) {
-                const int h = i / (SCAN_NB * U / 8), r = (i / (U / 8)) % SCAN_NB, k = c * U + (i % (U / 8)) * 8;
-                uint4 v = *reinterpret_cast<const uint4*>(Hsm + (nbuf * NH + h) * S::HBYTES + swz<H * 2>(r, k));
+                const int h = i / (SCAN_NB * U / 8), r = (i / (U / 8)) % SCAN_NB, kl = (i % (U / 8)) * 8;
+                uint4 v = *reinterpret_cast<const uint4*>(Hsm + nbuf * NH * S::HBYTES + h * S::HBYTES + c * S::SLICE +
+                                                          swz<U * 2>(r, kl));
                 if (LEN && t >= rlen) v = make_uint4(0u, 0u, 0u, 0u);
-                *reinterpret_cast<uint4*>((h ? yl : yh) + ((int64_t)(bt0 + r) * T + t) * DH + d * H + k) = v;
+                *reinterpret_cast<uint4*>((h ? yl : yh) + ((int64_t)(bt0 + r) * T + t) * DH + d * H + c * U + kl) = v;
             }
         }
     }
+    // no CTA leaves while a bulk copy into or out of its shared memory may be in flight
+    cluster_arrive();
+    cluster_wait();
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -507,7 +560,7 @@ gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh,
 // dgi, dgh [D][B*T][3H], and their bf16 planes gih/gil, ghh/ghl in the same layout for the GEMMs.  The dgh planes hold
 // zeros at each sequence's first step (t = 0 for d = 0, t = T-1 for d = 1): that row pairs with h0 (covered from fp32 dgh),
 // so dW_hh = dgh^T H_prev needs no row mask.  Shared memory: W^T rows (H) x own gate rows (192) | dgh tile [16][192] | receive slots of the
-// peers' partial sums [CS-1][16][64] fp32 (this CTA's own partial goes into the dgh tile's space, which is free by then).
+// peers' partial sums [CS-1][64][16] fp32 (k-major, xslot; this CTA's own partial goes into the dgh tile's space, which is free by then).
 // Cluster barrier phases per step: (1) partials of the step have landed; (2) every CTA has read its receive slots, so
 // the next step's partials may be written.
 // LEN: at a padded (row, t >= lens[b]) dgi and dgh are 0 (fp32 and planes) and dh passes through unchanged: its dgh row
@@ -525,6 +578,16 @@ struct BwdSmem {
     static_assert(NH * DBYTES >= SLOT, "own partial sums alias the dgh tile");
 };
 
+// float index of the partial sum for (unit kl, batch column b) in a receive slot: k-major [U][NB], so a thread's two
+// accumulators of adjacent columns (b even, b + 1) are one 8-byte store.  The column pair is XORed with a function of kl
+// that keeps each half-warp's 8-byte stores conflict-free and leaves the owner's reads (32 consecutive units, one column)
+// at two lanes per bank.
+__device__ __forceinline__ int xslot(int kl, int b) {
+    static_assert(SCAN_NB == 16, "eight column pairs per unit");
+    const int g = ((kl >> 1) & 1) * 4 + ((kl >> 2) & 3);
+    return kl * SCAN_NB + (((b >> 1) ^ g) << 1) + (b & 1);
+}
+
 template <int H, int NS, bool LEN>
 __global__ void __launch_bounds__(SCAN_THREADS, 1)
 gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, const float* __restrict__ h0,
@@ -537,8 +600,8 @@ gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, co
     constexpr int PAIRS = NB * U / SCAN_THREADS;             // (unit, column) pairs per thread in the gate math
     extern __shared__ __align__(128) uint8_t smem[];
     uint8_t* Wsm = smem;                                     // [NH][H rows][Q]
-    uint8_t* Dsm = smem + NH * S::WBYTES;                    // [NH][NB rows][Q]; also this CTA's own partial [NB][U] fp32
-    float* recv = reinterpret_cast<float*>(Dsm + NH * S::DBYTES);   // [CS-1][NB][U]
+    uint8_t* Dsm = smem + NH * S::WBYTES;                    // [NH][NB rows][Q]; also this CTA's own partial [U][NB] fp32
+    float* recv = reinterpret_cast<float*>(Dsm + NH * S::DBYTES);   // [CS-1][U][NB] (xslot)
     const int c = (int)cluster_rank(), tile = blockIdx.y, d = blockIdx.z;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int bt0 = tile * NB;
@@ -567,16 +630,38 @@ gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, co
     cluster_wait();
 
     const int DH = D * H;
+    // the step's operands from global memory: G (r, z, n, W_hn h + b_hn), h_{t-1} (Y, or h0 at the first step) and dY.
+    // Step s + 1's are loaded during step s, so their latency hides behind the rest of the step and the dgh tile waits only
+    // for the incoming dh.  Where they are issued was measured per precision at configs[1] (per-phase clock64 stamps on an
+    // H100): at bf16x3 after the multiply, when the step's dgi / dgh / plane stores have drained (about 600 cycles per step
+    // less than right after the gate math); at bf16 right after the gate math (about 500 cycles less than after the
+    // multiply, where the loads delay the partial-sum exchange).
+    float gr[PAIRS], gz[PAIRS], gn[PAIRS], ghn[PAIRS], hprev[PAIRS], dyv[PAIRS];
+    auto load_step = [&](int s) {
+        const int t = d == 0 ? T - 1 - s : s;
+        const bool first = d == 0 ? t == 0 : t == T - 1;
+#pragma unroll
+        for (int i = 0; i < PAIRS; ++i) {
+            const int p = tid + i * SCAN_THREADS, u = p % U, b = bt0 + p / U, j = c * U + u;
+            const int64_t row = (int64_t)b * T + t;
+            const float* gs = G + ((int64_t)d * B * T + row) * 4 * H + j;
+            gr[i] = gs[0]; gz[i] = gs[H]; gn[i] = gs[2 * H]; ghn[i] = gs[3 * H];
+            if (first) hprev[i] = h0 ? h0[((int64_t)d * B + b) * H + j] : 0.f;
+            else hprev[i] = Y[((int64_t)b * T + (d == 0 ? t - 1 : t + 1)) * DH + d * H + j];
+            dyv[i] = dY[row * DH + d * H + j];
+        }
+    };
+    load_step(0);
     for (int s = 0; s < T; ++s) {
         const int t = d == 0 ? T - 1 - s : s;
         const bool first = d == 0 ? t == 0 : t == T - 1;
         if (s > 0) {
 #pragma unroll
             for (int i = 0; i < PAIRS; ++i) {
-                const int p = tid + i * SCAN_THREADS;
+                const int p = tid + i * SCAN_THREADS, x = xslot(p % U, p / U);
                 float v = dhz[i];
 #pragma unroll
-                for (int src = 0; src < CS; ++src) v += slot(src)[p];
+                for (int src = 0; src < CS; ++src) v += slot(src)[x];
                 dhr[i] = v;
             }
         }
@@ -586,12 +671,8 @@ gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, co
         for (int i = 0; i < PAIRS; ++i) {
             const int p = tid + i * SCAN_THREADS, u = p % U, bl = p / U, b = bt0 + bl, j = c * U + u;
             const int64_t row = (int64_t)b * T + t;
-            const float* gs = G + ((int64_t)d * B * T + row) * 4 * H + j;
-            const float r = gs[0], z = gs[H], n = gs[2 * H], hnv = gs[3 * H];
-            float hpv;
-            if (first) hpv = h0 ? h0[((int64_t)d * B + b) * H + j] : 0.f;
-            else hpv = Y[((int64_t)b * T + (d == 0 ? t - 1 : t + 1)) * DH + d * H + j];
-            const float dh = dhr[i] + dY[row * DH + d * H + j];
+            const float r = gr[i], z = gz[i], n = gn[i], hnv = ghn[i], hpv = hprev[i];
+            const float dh = dhr[i] + dyv[i];
             float dan = dh * (1.f - z) * (1.f - n * n);
             float dar = dan * hnv * r * (1.f - r);
             float daz = dh * (hpv - n) * z * (1.f - z);
@@ -618,6 +699,7 @@ gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, co
             gih[po] = hi;
             if (NH == 2) gil[po] = lo;
         }
+        if (NS == 1 && s + 1 < T) load_step(s + 1);
         __syncthreads();
         // planes of this step's rows from the dgh tile, 16-byte stores: dgh (zeros at a sequence's first step) and dgi's r, z
         for (int i = tid; i < NH * NB * (Q / 8); i += SCAN_THREADS) {
@@ -659,23 +741,26 @@ gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, co
                 }
             }
         }
+        if (NS != 1 && s + 1 < T) load_step(s + 1);
         __syncthreads();                                     // dgh tile consumed: its space takes the own partial
         cluster_wait();                                      // phase (2) complete: peers' receive slots are free
+        // accumulators e = 0, 1 (and 2, 3) are adjacent batch columns of one unit: one 8-byte store each
 #pragma unroll
         for (int m = 0; m < MT; ++m)
 #pragma unroll
             for (int n = 0; n < 2; ++n)
 #pragma unroll
-                for (int e = 0; e < 4; ++e) {
+                for (int e = 0; e < 4; e += 2) {
                     const int k = (warp + 8 * m) * 16 + (lane >> 2) + (e >= 2 ? 8 : 0);
-                    const int bl = n * 8 + 2 * (lane & 3) + (e & 1);
-                    const int dst = k / U, kl = k % U;
+                    const int bl = n * 8 + 2 * (lane & 3);
+                    const int dst = k / U, x = xslot(k % U, bl);
+                    const float2 v = make_float2(acc[m][n][e], acc[m][n][e + 1]);
                     if (dst == c) {
-                        own[bl * U + kl] = acc[m][n][e];
+                        *reinterpret_cast<float2*>(own + x) = v;
                     } else {
                         // at CTA dst, the slot of source c is (c < dst ? c : c - 1)
-                        const float* rs = recv + (c < dst ? c : c - 1) * NB * U + bl * U + kl;
-                        st_cluster_f32(mapa(smem_u32(rs), dst), acc[m][n][e]);
+                        const float* rs = recv + (c < dst ? c : c - 1) * NB * U + x;
+                        st_cluster_v2_f32(mapa(smem_u32(rs), dst), v);
                     }
                 }
         cluster_arrive();                                    // phase (1): this step's partial sums are delivered
@@ -683,10 +768,10 @@ gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, co
     }
 #pragma unroll
     for (int i = 0; i < PAIRS; ++i) {
-        const int p = tid + i * SCAN_THREADS, u = p % U, b = p / U;
+        const int p = tid + i * SCAN_THREADS, u = p % U, b = p / U, x = xslot(u, b);
         float v = dhz[i];
 #pragma unroll
-        for (int src = 0; src < CS; ++src) v += slot(src)[p];
+        for (int src = 0; src < CS; ++src) v += slot(src)[x];
         dhc[((int64_t)d * B + bt0 + b) * H + c * U + u] = v;
     }
 }
