@@ -17,7 +17,7 @@ void bigru_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* bigru_last_error(void) { return g_err; }
-extern "C" int bigru_version(void) { return 207; }
+extern "C" int bigru_version(void) { return 208; }
 
 extern "C" int bigru_device_check(int dev) {
     int n = 0;
@@ -251,6 +251,16 @@ extern "C" int bigru_stash_argmax_offset(const bigru_plan* p, size_t* byte_offse
 extern "C" int bigru_stash_output_offset(const bigru_plan* p, int layer, size_t* byte_offset) {
     if (!p || !byte_offset || layer < 0 || layer >= p->L) { bigru_set_error("stash_output_offset: bad argument"); return BIGRU_ERR_ARG; }
     *byte_offset = (size_t)stash_layout(*p).Y[layer] * sizeof(float);
+    return BIGRU_OK;
+}
+
+extern "C" int bigru_scan_geometry(const bigru_plan* p, int scan, int* R, int* n_split) {
+    if (!p || !R || !n_split || (scan != 0 && scan != 1)) { bigru_set_error("scan_geometry: bad argument"); return BIGRU_ERR_ARG; }
+    if (p->prec == BIGRU_PREC_FP32) { bigru_set_error("scan_geometry: BIGRU_PREC_FP32 runs no cluster scans"); return BIGRU_ERR_UNSUPPORTED; }
+    int geom[2] = {0, 0};
+    if (scan == 0) TRY(tc_scan_fwd(*p, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, geom));
+    else TRY(tc_scan_bwd(*p, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, geom));
+    *R = geom[0]; *n_split = geom[1];
     return BIGRU_OK;
 }
 

@@ -5,24 +5,29 @@
 //   * wg_gemm             - a persistent TMA + mbarrier pipelined wgmma GEMM (wg_gemm_kernel) over bf16 operand planes that
 //                           the scans and to_planes_kernel write next to the fp32 activations; deterministic split-K.
 //                           tc_gemm_launch keeps the GemmArgs contract for the small head / h0 GEMMs (operands packed).
-//   * gru_scan_fwd_kernel - one layer's whole forward recurrence in one launch: a thread-block cluster per (direction,
-//                           16-row batch tile); CTA c of the cluster owns hidden units [64c, 64c+64) and keeps their W_hh
-//                           rows (3 gates x 64 units x H) resident in shared memory for all T steps.  Each step it multiplies
-//                           them with h_{t-1} of the tile, runs the gate math in registers and bulk-copies its slice of h_t
-//                           into the shared memory of every CTA of the cluster (distributed shared memory), where an
-//                           mbarrier counts the bytes in.
+//   * gru_scan_fwd_kernel - one layer's whole forward recurrence in one launch: a thread-block cluster per direction and
+//                           one or, at bf16x3, two 16-row batch tiles (how many take two follows from how many clusters
+//                           the device holds at once: scan_geometry); CTA c of the cluster owns hidden units [64c, 64c+64) and keeps
+//                           their W_hh rows (3 gates x 64 units x H) resident in shared memory for all T steps.  Each step it
+//                           multiplies them with h_{t-1} of the tile, runs the gate math in registers and bulk-copies its
+//                           slice of h_t into the shared memory of every CTA of the cluster (distributed shared memory),
+//                           where an mbarrier counts the bytes in.
 //   * gru_scan_bwd_kernel - the backward recurrence, reduction-partitioned: CTA c keeps W_hh^T restricted to its own units'
 //                           gate rows (H x 192), multiplies it with its local dgh tile and sends each peer the fp32 partial
-//                           sums of dh_{t-1} for the peer's units; the owner adds them up.
+//                           sums of dh_{t-1} for the peer's units; the owner adds them up.  One 16-row tile per cluster, or 8
+//                           rows in a short last round (scan_bwd_geometry).
 // Precision: NS = 1 (bf16) uses single bf16 operands; NS = 3 (bf16x3) splits every operand x = hi + lo (both bf16, |lo| <=
 // 2^-9 |x|) and adds hi*hi + hi*lo + lo*hi (the dropped lo*lo term is below 2^-16 relative), all with fp32 accumulation:
 // fp32-class results on the tensor cores.  State, gate math, stash and gradients are fp32 in both.
 // H100 budget that shapes the scans: 227 KB of shared memory per block holds a 64-unit slice of W_hh at H = 256 as hi/lo
-// pairs (192 KB) or at H = 512 in bf16 (192 KB); clusters of H/64 <= 8 CTAs stay within the portable cluster size.
+// pairs (192 KB) or at H = 512 in bf16 (192 KB), next to the forward's h tile (one 32-row buffer at bf16x3); clusters of
+// H/64 <= 8 CTAs stay within the portable cluster size.
 #pragma once
 #include "common.cuh"
 #include "kernels_f32.cuh"
 #include <algorithm>
+#include <map>
+#include <mutex>
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -353,12 +358,17 @@ __global__ void splitk_reduce_kernel(const float* __restrict__ part, int splits,
 //   gi [D][B*T][3H] (x W_ih^T + b_ih), Y [B][T][D*H], G [D][B*T][4H] = (r, z, n, W_hn h + b_hn), hn [D][B][H].
 // Y also goes out as bf16 planes (yh, and yl at bf16x3) in Y's layout: the next layer's projection and the weight gradients
 // read them.
-// Grid (CS, B/16, D), cluster (CS, 1, 1), 256 threads.  Warp w owns units 16*(w/2) .. +16 of the CTA's slice and batch
-// columns 8*(w%2) .. +8: its r, z and n accumulators hold the same (unit, column) pairs, so the gate math needs no exchange.
-// The h tile is double-buffered and laid out [buf][NH][CS][16 rows][64 units]: CTA c's part of a plane is one 2 KB block at
-// the same offset in every CTA.  Each step a CTA writes its h_t into its own block of the next buffer, and one thread sends
-// that block to every peer with a bulk copy, which completes on the peer's per-buffer "full" mbarrier.  Before its next
-// multiply a CTA waits on that barrier for the (CS - 1) blocks of its peers; there is no cluster barrier per step.
+// Grid (CS, clusters, 1), cluster (CS, 1, 1), 256 threads.  A cluster takes one or two (bf16x3 only) 16-row batch tiles of
+// one direction (scan_tile): nb = 16 or 32 rows.  Warp w owns units 16*(w/2) .. +16 of the CTA's slice and nb/2 batch columns from
+// (w%2)*nb/2, one or two n8 blocks: each W fragment it loads feeds every block, so a 32-row tile reads W from shared memory
+// as often as a 16-row one.  Its r, z and n accumulators hold the same (unit, column) pairs, so the gate math needs no
+// exchange.  Every output element comes from the same MMA sequence over k whatever the tile size: a row's bits do not
+// depend on its cluster's tile.
+// The h tile is laid out [NBUF][NH][CS][nb rows][64 units] in one region that holds two 16-row buffers or one 32-row
+// buffer (NBUF = 2 or 1): CTA c's part of a plane is one block at the same offset in every CTA.  Each step a CTA writes its h_t into its own block, and one thread sends that block to every peer with a bulk
+// copy, which completes on the peer's "full" mbarrier of that buffer.  Before its next multiply a CTA waits on that barrier
+// for the (CS - 1) blocks of its peers.  With one buffer (bf16x3, 32 rows) a CTA also arrives on every peer's "empty"
+// mbarrier after its multiply: its reads of the tile are done.  There is no cluster barrier per step.
 // OUT selects at compile time which of Y, G and the Y planes are written (hn_out is written whenever it is non-null): the
 // training forward keeps all three for the backward; inference writes the planes of a lower layer (the next projection reads
 // them) and the fp32 Y of the top layer (the pooling head reads it).  The h arithmetic is the same in every instantiation.
@@ -373,34 +383,62 @@ constexpr int SCAN_TRAIN = SCAN_Y | SCAN_G | SCAN_PLANES, SCAN_INFER_LOWER = SCA
 template <int H, int NS>
 struct FwdSmem {
     static constexpr int NH = NS == 1 ? 1 : 2;
+    // rows of the largest tile a cluster takes: 32 at bf16x3, where a CTA has its SM to itself; 16 at bf16, where a 32-row
+    // body's registers would keep a second CTA off the SM (H <= 256) or its tile would not fit (H = 512)
+    static constexpr int NBMAX = NS == 1 ? SCAN_NB : 2 * SCAN_NB;
+    // buffers of the largest tile: a double-buffered 32-row tile does not fit.  The same bytes hold two 16-row buffers, so
+    // 16-row tiles are double-buffered at every precision
+    static constexpr int NBUF = NBMAX == SCAN_NB ? 2 : 1;
     static constexpr int WP = H * 2;                        // W row pitch (bytes): K = H
     static constexpr int WBYTES = 3 * SCAN_U * WP;          // one of hi / lo
-    static constexpr int HBYTES = SCAN_NB * H * 2;          // h tile, one of hi / lo
-    static constexpr int SLICE = SCAN_NB * SCAN_U * 2;      // one CTA's units of one h plane: 16 rows x 128 B
-    static constexpr int TOTAL = NH * WBYTES + 2 * NH * HBYTES + 2 * 8;   // + the two buffers' full barriers
+    static constexpr int HBYTES = NBMAX * H * 2;            // h tile, one of hi / lo
+    static constexpr int SLICE = NBMAX * SCAN_U * 2;        // one CTA's block of one h plane: NBMAX rows x 128 B
+    static constexpr int TOTAL = NH * WBYTES + NBUF * NH * HBYTES + 2 * 8;   // + two full barriers, or full and empty
 };
 
-// byte offset of h element (row b, unit k) in one buffer plane of the forward h tile: 128-byte rows within the 2 KB block
-// of the units' CTA, chunks XOR-swizzled as in swz
-__device__ __forceinline__ uint32_t hsw(int b, int k) {
-    return (uint32_t)((k / SCAN_U) * (SCAN_NB * SCAN_U * 2)) + swz<SCAN_U * 2>(b, k % SCAN_U);
+// the batch tile of cluster q (blockIdx.y): the first D * m2 clusters take 32 rows, m2 per direction; the others 16.  ntd:
+// 16-row tiles per direction (B / 16)
+__device__ __forceinline__ void scan_tile(int q, int m2, int ntd, int D, int& d, int& bt0, int& nb) {
+    if (q < D * m2) {
+        d = q / m2; bt0 = (q % m2) * 2 * SCAN_NB; nb = 2 * SCAN_NB;
+    } else {
+        const int r = q - D * m2, o = ntd - 2 * m2;
+        d = r / o; bt0 = (2 * m2 + r % o) * SCAN_NB; nb = SCAN_NB;
+    }
 }
 
-template <int H, int NS, int OUT, bool LEN>
-__global__ void __launch_bounds__(SCAN_THREADS, 1)
-gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh, const float* __restrict__ bhh, int64_t zW,
-                    const float* __restrict__ h0, float* __restrict__ Y, float* __restrict__ G, float* __restrict__ hn_out,
-                    bf16_t* __restrict__ yh, bf16_t* __restrict__ yl, int B, int T, int D, const int* __restrict__ lens) {
+// byte offset of h element (row b, unit k) in one plane of the forward h tile: 128-byte rows within the block of the units'
+// CTA, chunks XOR-swizzled as in swz
+template <int NBMAX>
+__device__ __forceinline__ uint32_t hsw(int b, int k) {
+    return (uint32_t)((k / SCAN_U) * (NBMAX * SCAN_U * 2)) + swz<SCAN_U * 2>(b, k % SCAN_U);
+}
+
+__device__ __forceinline__ void mbar_arrive_peer(uint64_t* bar, uint32_t cta) {
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(mapa(smem_u32(bar), cta)) : "memory");
+}
+
+// the scan of one cluster whose tile has JN * 16 rows from bt0, direction d
+template <int H, int NS, int OUT, bool LEN, int JN>
+__device__ __forceinline__ void gru_scan_fwd_tile(const float* __restrict__ gi, const float* __restrict__ Whh,
+                                                  const float* __restrict__ bhh, int64_t zW, const float* __restrict__ h0,
+                                                  float* __restrict__ Y, float* __restrict__ G, float* __restrict__ hn_out,
+                                                  bf16_t* __restrict__ yh, bf16_t* __restrict__ yl, int B, int T, int D,
+                                                  const int* __restrict__ lens, int d, int bt0) {
     using S = FwdSmem<H, NS>;
-    constexpr int U = SCAN_U, CS = H / U, NH = S::NH;
-    static_assert(SCAN_THREADS % (SCAN_NB * (U / 8)) == 0, "a thread copies the same Y plane row in every pass");
+    constexpr int U = SCAN_U, CS = H / U, NH = S::NH, JMAX = JN, jn = JN, nb = JN * SCAN_NB;   // jn n8 blocks per warp
+    // the h region holds two 16-row buffers or one 32-row buffer: a 16-row tile is double-buffered, a 32-row tile is not
+    constexpr int NBMAX = nb, NBUF = S::NBUF * S::NBMAX / nb;
+    constexpr int HBYTES = nb * H * 2, SLICE = nb * U * 2;  // one buffer of one h plane; one CTA's block of it
+    static_assert(NBUF * HBYTES == S::NBUF * S::HBYTES, "both tile sizes fill the h region");
+    static_assert(SCAN_THREADS % (nb * (U / 8)) == 0, "a thread copies the same Y plane row in every pass");
     extern __shared__ __align__(128) uint8_t smem[];
     uint8_t* Wsm = smem;                                     // [NH][3U rows][H]
-    uint8_t* Hsm = smem + NH * S::WBYTES;                    // [2 buffers][NH][CS][NB rows][U]
-    uint64_t* full = reinterpret_cast<uint64_t*>(Hsm + 2 * NH * S::HBYTES);   // [2 buffers]
-    const int c = (int)cluster_rank(), tile = blockIdx.y, d = blockIdx.z;
+    uint8_t* Hsm = smem + NH * S::WBYTES;                    // [NBUF][NH][CS][NBMAX rows][U]
+    uint64_t* full = reinterpret_cast<uint64_t*>(Hsm + NBUF * NH * HBYTES);   // [2]: two buffers' full, or full and empty
+    uint64_t* empty = full + 1;                              // NBUF == 1
+    const int c = (int)cluster_rank();
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int bt0 = tile * SCAN_NB;
     const float* W = Whh + d * zW;
 
     for (int i = tid; i < 3 * U * H; i += SCAN_THREADS) {
@@ -411,147 +449,198 @@ gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh,
         *reinterpret_cast<bf16_t*>(Wsm + swz<S::WP>(q, k)) = hi;
         if (NH == 2) *reinterpret_cast<bf16_t*>(Wsm + S::WBYTES + swz<S::WP>(q, k)) = lo;
     }
-    for (int i = tid; i < SCAN_NB * H; i += SCAN_THREADS) {
+    for (int i = tid; i < nb * H; i += SCAN_THREADS) {
         const int b = i / H, k = i % H;
         const float v = h0 ? h0[((int64_t)d * B + bt0 + b) * H + k] : 0.f;
         bf16_t hi, lo;
         split_bf16(v, hi, lo);
-        *reinterpret_cast<bf16_t*>(Hsm + hsw(b, k)) = hi;
-        if (NH == 2) *reinterpret_cast<bf16_t*>(Hsm + S::HBYTES + hsw(b, k)) = lo;
+        *reinterpret_cast<bf16_t*>(Hsm + hsw<NBMAX>(b, k)) = hi;
+        if (NH == 2) *reinterpret_cast<bf16_t*>(Hsm + HBYTES + hsw<NBMAX>(b, k)) = lo;
     }
     if (tid == 0) {
         mbar_init(full, 1);
-        mbar_init(full + 1, 1);
+        mbar_init(full + 1, NBUF == 2 ? 1 : CS - 1);     // the second buffer's full, or empty
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
 
     const int ug = warp >> 1, nt = warp & 1;
-    int unit[2], bcol[2];
+    int unit[2], bcol[JMAX][2];
     unit[0] = ug * 16 + (lane >> 2); unit[1] = unit[0] + 8;
-    bcol[0] = nt * 8 + 2 * (lane & 3); bcol[1] = bcol[0] + 1;
-    float bias[3][2], hp[4];
+#pragma unroll
+    for (int j = 0; j < JMAX; ++j) {
+        bcol[j][0] = (nt * jn + j) * 8 + 2 * (lane & 3); bcol[j][1] = bcol[j][0] + 1;
+    }
+    float bias[3][2], hp[JMAX][4];
 #pragma unroll
     for (int gte = 0; gte < 3; ++gte)
 #pragma unroll
-        for (int j = 0; j < 2; ++j) bias[gte][j] = bhh[d * zW + gte * H + c * U + unit[j]];
+        for (int i = 0; i < 2; ++i) bias[gte][i] = bhh[d * zW + gte * H + c * U + unit[i]];
+    // lengths of this thread's batch columns, and of the row it copies to the Y planes (the same row in every pass of the
+    // copy loop: SCAN_THREADS is a multiple of nb * U / 8)
+    int len[JMAX][2], rlen = T;
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-        const int b = bt0 + bcol[e & 1], j = c * U + unit[e >> 1];
-        hp[e] = h0 ? h0[((int64_t)d * B + b) * H + j] : 0.f;
+    for (int j = 0; j < JMAX; ++j) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const int b = bt0 + bcol[j][e & 1], k = c * U + unit[e >> 1];
+            hp[j][e] = h0 ? h0[((int64_t)d * B + b) * H + k] : 0.f;
+        }
+        len[j][0] = len[j][1] = T;
+        if (LEN) { len[j][0] = lens[bt0 + bcol[j][0]]; len[j][1] = lens[bt0 + bcol[j][1]]; }
     }
-    // lengths of this thread's two batch columns, and of the row it copies to the Y planes (the same row in every pass of
-    // the copy loop: SCAN_THREADS is a multiple of SCAN_NB * U / 8)
-    int len[2] = {T, T}, rlen = T;
-    if (LEN) {
-        len[0] = lens[bt0 + bcol[0]]; len[1] = lens[bt0 + bcol[1]];
-        rlen = lens[bt0 + (tid / (U / 8)) % SCAN_NB];
-    }
-    // every CTA of the cluster has started, staged its tiles and initialised its barriers before any bulk copy
+    if (LEN) rlen = lens[bt0 + (tid / (U / 8)) % nb];
+    // every CTA of the cluster has started, staged its tiles and initialised its barriers before any bulk copy or arrive
     cluster_arrive();
     cluster_wait();
 
-    // Step s multiplies with buffer buf = s & 1 (h_{s-1}; h0 at s = 0) and produces h_s in buffer nbuf = buf ^ 1.  Each
-    // buffer's full barrier completes every other step, so the wait at step s >= 1 is for phase (s - 1) / 2 of full[buf].
-    // The last step sends nothing: only its own block is read (Y planes).
-    // Write after read on the double buffer: a peer sends its h_{s+1} into this CTA's buffer buf (the one step s reads)
-    // only after its own full barrier for h_s has completed, which needs this CTA's h_s, which this CTA sends only after the
-    // __syncthreads that follows its step-s multiply.  So every read of buffer buf is ordered before the copy that
-    // overwrites it (the copy's complete_tx releases at cluster scope, the peer's wait acquires at cluster scope).
-    // Likewise the own block of a buffer is rewritten at step s + 2 only after this CTA's full barrier for h_{s+1}
-    // completed, which needs every peer's h_{s+1}, which each peer computed after receiving all of this CTA's step-s copy:
-    // the bulk copies that read it are done.
+    // Step s multiplies with buffer buf (h_{s-1}; h0 at s = 0) and produces h_s in buffer nbuf: with two buffers buf = s & 1
+    // and nbuf = buf ^ 1, and each buffer's full barrier completes every other step (phase (s - 1) / 2 is awaited at step
+    // s); with one buffer both are 0, and full and empty complete once per step (phase s).  The last step sends nothing:
+    // only its own block is read (Y planes).
+    // Two buffers, write after read: a peer sends its h_{s+1} into this CTA's buffer buf (the one step s reads) only after
+    // its own full barrier for h_s has completed, which needs this CTA's h_s, which this CTA sends only after the
+    // __syncthreads that follows its step-s multiply.  The own block of a buffer is rewritten at step s + 2 only after this
+    // CTA's full barrier for h_{s+1} completed, which needs every peer's h_{s+1}, which each peer computed after receiving
+    // all of this CTA's step-s copy: the bulk copies that read it are done.
+    // One buffer, write after read on a peer's block: a peer sends h_s into this CTA's tile only after its empty barrier of
+    // step s has completed, which needs this CTA's arrive, which follows the __syncthreads that ends this CTA's step-s
+    // multiply.  On the own block: this CTA rewrites it with h_s only after its own empty barrier of step s has completed.
+    // Each peer arrived there after its step-s multiply, which followed its full barrier of step s - 1, which completed when
+    // this CTA's copy of h_{s-1} out of the own block had landed.
+    // The Y planes read the own block before the __syncthreads that ends the next multiply.  Arrives release and waits
+    // acquire at cluster scope; the copies' complete_tx does the same.
     const int DH = D * H;
     for (int s = 0; s < T; ++s) {
         const int t = d == 0 ? s : T - 1 - s;
-        const int buf = s & 1;
+        const int buf = NBUF == 2 ? s & 1 : 0, nbuf = NBUF == 2 ? buf ^ 1 : 0;
         // the peers' blocks of h_{s-1} have landed; and the barrier of the buffer this step fills expects theirs of h_s
-        if (s > 0) mbar_wait<true>(full + buf, ((s - 1) >> 1) & 1);
-        if (tid == 0 && s + 1 < T) mbar_arrive_expect_tx(full + (buf ^ 1), (CS - 1) * NH * S::SLICE);
-        float giv[3][4];
+        if (s > 0) mbar_wait<true>(full + buf, (NBUF == 2 ? (s - 1) >> 1 : s - 1) & 1);
+        if (tid == 0 && s + 1 < T) mbar_arrive_expect_tx(full + nbuf, (CS - 1) * NH * nb * U * 2);
+        float giv[3][JMAX][4];
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const int64_t row = (int64_t)(bt0 + bcol[e & 1]) * T + t;
-            const float* gr = gi + ((int64_t)d * B * T + row) * 3 * H + c * U + unit[e >> 1];
+        for (int j = 0; j < JMAX; ++j)
 #pragma unroll
-            for (int gte = 0; gte < 3; ++gte) giv[gte][e] = gr[gte * H];
-        }
-        float acc[3][4];
+            for (int e = 0; e < 4; ++e) {
+                const int64_t row = (int64_t)(bt0 + bcol[j][e & 1]) * T + t;
+                const float* gr = gi + ((int64_t)d * B * T + row) * 3 * H + c * U + unit[e >> 1];
+#pragma unroll
+                for (int gte = 0; gte < 3; ++gte) giv[gte][j][e] = gr[gte * H];
+            }
+        float acc[3][JMAX][4];
 #pragma unroll
         for (int gte = 0; gte < 3; ++gte)
 #pragma unroll
-            for (int e = 0; e < 4; ++e) acc[gte][e] = 0.f;
-        const uint32_t hbase = smem_u32(Hsm + buf * NH * S::HBYTES);
+            for (int j = 0; j < JMAX; ++j)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) acc[gte][j][e] = 0.f;
+        const uint32_t hbase = smem_u32(Hsm + buf * NH * HBYTES);
         const uint32_t wbase = smem_u32(Wsm);
 #pragma unroll 4
         for (int ks = 0; ks < H / 16; ++ks) {
-            uint32_t bh[NH][2];
-            const int brow = nt * 8 + (lane & 7), bk = ks * 16 + ((lane >> 3) & 1) * 8;
+            uint32_t bh[JMAX][NH][2];
+            const int bk = ks * 16 + ((lane >> 3) & 1) * 8;
 #pragma unroll
-            for (int h = 0; h < NH; ++h) ldsm_x2(hbase + h * S::HBYTES + hsw(brow, bk), bh[h]);
+            for (int j = 0; j < JMAX; ++j)
+#pragma unroll
+                for (int h = 0; h < NH; ++h)
+                    ldsm_x2(hbase + h * HBYTES + hsw<NBMAX>((nt * jn + j) * 8 + (lane & 7), bk), bh[j][h]);
 #pragma unroll
             for (int gte = 0; gte < 3; ++gte) {
                 const int arow = gte * U + ug * 16 + (lane & 15), ak = ks * 16 + (lane >> 4) * 8;
                 uint32_t a[NH][4];
 #pragma unroll
                 for (int h = 0; h < NH; ++h) ldsm_x4(wbase + h * S::WBYTES + swz<S::WP>(arow, ak), a[h]);
-                if (NS != 1) {
-                    mma_bf16(acc[gte], a[0], bh[NH - 1][0], bh[NH - 1][1]);
-                    mma_bf16(acc[gte], a[NH - 1], bh[0][0], bh[0][1]);
-                }
-                mma_bf16(acc[gte], a[0], bh[0][0], bh[0][1]);
-            }
-        }
-        const int nbuf = buf ^ 1;
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-            const int b = bt0 + bcol[e & 1], ul = unit[e >> 1], j = c * U + ul;
-            const float r = sigmoid_f(giv[0][e] + acc[0][e] + bias[0][e >> 1]);
-            const float z = sigmoid_f(giv[1][e] + acc[1][e] + bias[1][e >> 1]);
-            const float hnv = acc[2][e] + bias[2][e >> 1];
-            const float n = tanhf(giv[2][e] + r * hnv);
-            const bool pad = LEN && t >= len[e & 1];
-            const float h = pad ? hp[e] : (1.f - z) * n + z * hp[e];
-            hp[e] = h;
-            const int64_t row = (int64_t)b * T + t;
-            if (OUT & SCAN_Y) Y[row * DH + d * H + j] = pad ? 0.f : h;
-            if ((OUT & SCAN_G) && !pad) {
-                float* gs = G + ((int64_t)d * B * T + row) * 4 * H + j;
-                gs[0] = r; gs[H] = z; gs[2 * H] = n; gs[3 * H] = hnv;
+                for (int j = 0; j < JMAX; ++j) {
+                    if (NS != 1) {
+                        mma_bf16(acc[gte][j], a[0], bh[j][NH - 1][0], bh[j][NH - 1][1]);
+                        mma_bf16(acc[gte][j], a[NH - 1], bh[j][0][0], bh[j][0][1]);
+                    }
+                    mma_bf16(acc[gte][j], a[0], bh[j][0][0], bh[j][0][1]);
+                }
             }
-            if (hn_out && s == T - 1) hn_out[((int64_t)d * B + b) * H + j] = h;
-            bf16_t hi, lo;
-            split_bf16(h, hi, lo);
-            uint8_t* la = Hsm + nbuf * NH * S::HBYTES + hsw(bcol[e & 1], j);
-            *reinterpret_cast<bf16_t*>(la) = hi;
-            if (NH == 2) *reinterpret_cast<bf16_t*>(la + S::HBYTES) = lo;
         }
+        if (NBUF == 1) {
+            // this CTA's reads of the tile are done: tell every peer (threads 0 .. CS - 2, one peer each)
+            __syncthreads();
+            if (tid < CS - 1) mbar_arrive_peer(empty, (c + 1 + tid) % CS);
+        }
+        float hv[JMAX][4];
+#pragma unroll
+        for (int j = 0; j < JMAX; ++j)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const int b = bt0 + bcol[j][e & 1], ul = unit[e >> 1], k = c * U + ul;
+                const float r = sigmoid_f(giv[0][j][e] + acc[0][j][e] + bias[0][e >> 1]);
+                const float z = sigmoid_f(giv[1][j][e] + acc[1][j][e] + bias[1][e >> 1]);
+                const float hnv = acc[2][j][e] + bias[2][e >> 1];
+                const float n = tanhf(giv[2][j][e] + r * hnv);
+                const bool pad = LEN && t >= len[j][e & 1];
+                const float h = pad ? hp[j][e] : (1.f - z) * n + z * hp[j][e];
+                hp[j][e] = h;
+                hv[j][e] = h;
+                const int64_t row = (int64_t)b * T + t;
+                if (OUT & SCAN_Y) Y[row * DH + d * H + k] = pad ? 0.f : h;
+                if ((OUT & SCAN_G) && !pad) {
+                    float* gs = G + ((int64_t)d * B * T + row) * 4 * H + k;
+                    gs[0] = r; gs[H] = z; gs[2 * H] = n; gs[3 * H] = hnv;
+                }
+                if (hn_out && s == T - 1) hn_out[((int64_t)d * B + b) * H + k] = h;
+            }
+        // every peer has multiplied with h_{s-1}, so this CTA's copies of it out of the own block are done
+        if (NBUF == 1) mbar_wait<true>(empty, s & 1);
+#pragma unroll
+        for (int j = 0; j < JMAX; ++j)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                bf16_t hi, lo;
+                split_bf16(hv[j][e], hi, lo);
+                uint8_t* la = Hsm + nbuf * NH * HBYTES + hsw<NBMAX>(bcol[j][e & 1], c * U + unit[e >> 1]);
+                *reinterpret_cast<bf16_t*>(la) = hi;
+                if (NH == 2) *reinterpret_cast<bf16_t*>(la + HBYTES) = lo;
+            }
         // the own block of h_s is complete; make it visible to the bulk copies (async proxy), then send it to every peer
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
         __syncthreads();
-        const uint32_t own = smem_u32(Hsm + nbuf * NH * S::HBYTES + c * S::SLICE);
+        const uint32_t own = smem_u32(Hsm + nbuf * NH * HBYTES + c * SLICE);
         if (tid == 0 && s + 1 < T) {
 #pragma unroll
             for (int p = 1; p < CS; ++p) {
                 const uint32_t dst = (c + p) % CS;
 #pragma unroll
-                for (int h = 0; h < NH; ++h) bulk_copy_to_peer(own + h * S::HBYTES, S::SLICE, full + nbuf, dst);
+                for (int h = 0; h < NH; ++h) bulk_copy_to_peer(own + h * HBYTES, nb * U * 2, full + nbuf, dst);
             }
         }
-        // the Y planes of this CTA's units from its own block, 16-byte stores, while the copies are in flight.  The block
-        // is rewritten two steps later (see above).  A padded row's tile holds the carried state: its plane rows are zeros.
+        // the Y planes of this CTA's units from its own block, 16-byte stores, while the copies are in flight.  A padded
+        // row's tile holds the carried state: its plane rows are zeros.
         if (OUT & SCAN_PLANES) {
-            for (int i = tid; i < NH * SCAN_NB * (U / 8); i += SCAN_THREADS) {
-                const int h = i / (SCAN_NB * U / 8), r = (i / (U / 8)) % SCAN_NB, kl = (i % (U / 8)) * 8;
-                uint4 v = *reinterpret_cast<const uint4*>(Hsm + nbuf * NH * S::HBYTES + h * S::HBYTES + c * S::SLICE +
-                                                          swz<U * 2>(r, kl));
+            for (int i = tid; i < NH * nb * (U / 8); i += SCAN_THREADS) {
+                const int h = i / (nb * U / 8), r = (i / (U / 8)) % nb, kl = (i % (U / 8)) * 8;
+                uint4 v = *reinterpret_cast<const uint4*>(Hsm + (nbuf * NH + h) * HBYTES + c * SLICE + swz<U * 2>(r, kl));
                 if (LEN && t >= rlen) v = make_uint4(0u, 0u, 0u, 0u);
                 *reinterpret_cast<uint4*>((h ? yl : yh) + ((int64_t)(bt0 + r) * T + t) * DH + d * H + c * U + kl) = v;
             }
         }
     }
-    // no CTA leaves while a bulk copy into or out of its shared memory may be in flight
+    // no CTA leaves while a bulk copy or an arrive into or out of its shared memory may be in flight
     cluster_arrive();
     cluster_wait();
+}
+
+template <int H, int NS, int OUT, bool LEN>
+__global__ void __launch_bounds__(SCAN_THREADS, 1)
+gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh, const float* __restrict__ bhh, int64_t zW,
+                    const float* __restrict__ h0, float* __restrict__ Y, float* __restrict__ G, float* __restrict__ hn_out,
+                    bf16_t* __restrict__ yh, bf16_t* __restrict__ yl, int B, int T, int D, int m2, const int* __restrict__ lens) {
+    int d, bt0, nb;
+    scan_tile(blockIdx.y, m2, B / SCAN_NB, D, d, bt0, nb);
+    if constexpr (FwdSmem<H, NS>::NBMAX == 2 * SCAN_NB) {
+        if (nb == 2 * SCAN_NB) {
+            gru_scan_fwd_tile<H, NS, OUT, LEN, 2>(gi, Whh, bhh, zW, h0, Y, G, hn_out, yh, yl, B, T, D, lens, d, bt0);
+            return;
+        }
+    }
+    gru_scan_fwd_tile<H, NS, OUT, LEN, 1>(gi, Whh, bhh, zW, h0, Y, G, hn_out, yh, yl, B, T, D, lens, d, bt0);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -588,23 +677,25 @@ __device__ __forceinline__ int xslot(int kl, int b) {
     return kl * SCAN_NB + (((b >> 1) ^ g) << 1) + (b & 1);
 }
 
-template <int H, int NS, bool LEN>
-__global__ void __launch_bounds__(SCAN_THREADS, 1)
-gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, const float* __restrict__ h0,
-                    const float* __restrict__ dY, float* __restrict__ dhc, float* __restrict__ dgi, float* __restrict__ dgh,
-                    const float* __restrict__ Whh, int64_t zW, bf16_t* __restrict__ gih, bf16_t* __restrict__ gil,
-                    bf16_t* __restrict__ ghh, bf16_t* __restrict__ ghl, int B, int T, int D, const int* __restrict__ lens) {
+// the scan of one cluster whose tile has NR (16 or 8) rows from bt0, direction d; the shared-memory layout is that of 16
+template <int H, int NS, bool LEN, int NR>
+__device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, const float* __restrict__ Y,
+                                                  const float* __restrict__ h0, const float* __restrict__ dY,
+                                                  float* __restrict__ dhc, float* __restrict__ dgi, float* __restrict__ dgh,
+                                                  const float* __restrict__ Whh, int64_t zW, bf16_t* __restrict__ gih,
+                                                  bf16_t* __restrict__ gil, bf16_t* __restrict__ ghh, bf16_t* __restrict__ ghl,
+                                                  int B, int T, int D, const int* __restrict__ lens, int d, int bt0) {
     using S = BwdSmem<H, NS>;
     constexpr int U = SCAN_U, CS = H / U, NH = S::NH, Q = S::Q, NB = SCAN_NB;
     constexpr int MT = H / 16 / 8;                           // m-tiles (16 rows of W^T) per warp
-    constexpr int PAIRS = NB * U / SCAN_THREADS;             // (unit, column) pairs per thread in the gate math
+    constexpr int PAIRS = NR * U / SCAN_THREADS;             // (unit, column) pairs per thread in the gate math
+    constexpr int NBLK = NR / 8;                             // n8 blocks of the tile
     extern __shared__ __align__(128) uint8_t smem[];
     uint8_t* Wsm = smem;                                     // [NH][H rows][Q]
     uint8_t* Dsm = smem + NH * S::WBYTES;                    // [NH][NB rows][Q]; also this CTA's own partial [U][NB] fp32
     float* recv = reinterpret_cast<float*>(Dsm + NH * S::DBYTES);   // [CS-1][U][NB] (xslot)
-    const int c = (int)cluster_rank(), tile = blockIdx.y, d = blockIdx.z;
+    const int c = (int)cluster_rank();
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int bt0 = tile * NB;
     const float* W = Whh + d * zW;
     float* own = reinterpret_cast<float*>(Dsm);
     auto slot = [&](int src) -> float* { return src == c ? own : recv + (src < c ? src : src - 1) * NB * U; };
@@ -702,8 +793,8 @@ gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, co
         if (NS == 1 && s + 1 < T) load_step(s + 1);
         __syncthreads();
         // planes of this step's rows from the dgh tile, 16-byte stores: dgh (zeros at a sequence's first step) and dgi's r, z
-        for (int i = tid; i < NH * NB * (Q / 8); i += SCAN_THREADS) {
-            const int h = i / (NB * Q / 8), r = (i / (Q / 8)) % NB, q = (i % (Q / 8)) * 8, gte = q / U;
+        for (int i = tid; i < NH * NR * (Q / 8); i += SCAN_THREADS) {
+            const int h = i / (NR * Q / 8), r = (i / (Q / 8)) % NR, q = (i % (Q / 8)) * 8, gte = q / U;
             uint4 v = *reinterpret_cast<const uint4*>(Dsm + h * S::DBYTES + swz<S::WP>(r, q));
             const int64_t o = ((int64_t)d * B * T + (int64_t)(bt0 + r) * T + t) * 3 * H + gte * H + c * U + q % U;
             if (gte < 2) *reinterpret_cast<uint4*>((h ? gil : gih) + o) = v;
@@ -715,7 +806,7 @@ gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, co
 #pragma unroll
         for (int m = 0; m < MT; ++m)
 #pragma unroll
-            for (int n = 0; n < 2; ++n)
+            for (int n = 0; n < NBLK; ++n)
 #pragma unroll
                 for (int e = 0; e < 4; ++e) acc[m][n][e] = 0.f;
         const uint32_t wbase = smem_u32(Wsm), dbase = smem_u32(Dsm);
@@ -732,7 +823,7 @@ gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, co
 #pragma unroll
                 for (int h = 0; h < NH; ++h) ldsm_x4(wbase + h * S::WBYTES + swz<S::WP>(arow, ak), a[h]);
 #pragma unroll
-                for (int n = 0; n < 2; ++n) {
+                for (int n = 0; n < NBLK; ++n) {
                     if (NS != 1) {
                         mma_bf16(acc[m][n], a[0], bv[NH - 1][2 * n], bv[NH - 1][2 * n + 1]);
                         mma_bf16(acc[m][n], a[NH - 1], bv[0][2 * n], bv[0][2 * n + 1]);
@@ -748,7 +839,7 @@ gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, co
 #pragma unroll
         for (int m = 0; m < MT; ++m)
 #pragma unroll
-            for (int n = 0; n < 2; ++n)
+            for (int n = 0; n < NBLK; ++n)
 #pragma unroll
                 for (int e = 0; e < 4; e += 2) {
                     const int k = (warp + 8 * m) * 16 + (lane >> 2) + (e >= 2 ? 8 : 0);
@@ -773,6 +864,27 @@ gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, co
 #pragma unroll
         for (int src = 0; src < CS; ++src) v += slot(src)[x];
         dhc[((int64_t)d * B + bt0 + b) * H + c * U + u] = v;
+    }
+}
+
+// Grid (CS, clusters, 1), cluster (CS, 1, 1).  The first D * B / 16 - L8 clusters take one 16-row tile each, in (direction,
+// tile) order; the last L8 tiles are split into two 8-row clusters each (scan_bwd_geometry), so a short last round of
+// clusters takes less time.  An 8-row cluster multiplies one n8 block with the same MMA sequence per element: a row's bits
+// do not depend on its tile.
+template <int H, int NS, bool LEN>
+__global__ void __launch_bounds__(SCAN_THREADS, 1)
+gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, const float* __restrict__ h0,
+                    const float* __restrict__ dY, float* __restrict__ dhc, float* __restrict__ dgi, float* __restrict__ dgh,
+                    const float* __restrict__ Whh, int64_t zW, bf16_t* __restrict__ gih, bf16_t* __restrict__ gil,
+                    bf16_t* __restrict__ ghh, bf16_t* __restrict__ ghl, int B, int T, int D, int L8, const int* __restrict__ lens) {
+    const int ntd = B / SCAN_NB, n16 = D * ntd - L8, q = blockIdx.y;
+    if (q < n16) {
+        gru_scan_bwd_tile<H, NS, LEN, SCAN_NB>(G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, lens, q / ntd,
+                                                (q % ntd) * SCAN_NB);
+    } else {
+        const int f = n16 + (q - n16) / 2;
+        gru_scan_bwd_tile<H, NS, LEN, SCAN_NB / 2>(G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, lens,
+                                                    f / ntd, (f % ntd) * SCAN_NB + ((q - n16) & 1) * (SCAN_NB / 2));
     }
 }
 
@@ -917,49 +1029,107 @@ static int tc_gemm_launch(const GemmArgs& g, int prec, int cls, htc::bf16_t* ws,
     return wg_gemm(j, A, false, B, false, prec, st);
 }
 
-template <typename... KArgs, typename... Args>
-static int launch_cluster(void (*kernel)(KArgs...), int cs, int ntiles, int D, int smem, cudaStream_t st, Args... args) {
-    CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+template <typename K>
+static cudaLaunchConfig_t cluster_config(K kernel, int cs, int ny, int nz, int smem, cudaStream_t st, cudaLaunchAttribute* attr) {
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(cs, ntiles, D);
+    cfg.gridDim = dim3(cs, ny, nz);
     cfg.blockDim = dim3(htc::SCAN_THREADS);
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
-    cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
+    return cfg;
+}
+
+template <typename... KArgs, typename... Args>
+static int launch_cluster(void (*kernel)(KArgs...), int cs, int ny, int nz, int smem, cudaStream_t st, Args... args) {
+    CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    cudaLaunchAttribute attr[1];
+    const cudaLaunchConfig_t cfg = cluster_config(kernel, cs, ny, nz, smem, st, attr);
     CUDA_TRY(cudaLaunchKernelEx(&cfg, kernel, args...));
     return BIGRU_OK;
 }
 
-template <int HH, int NS, bool LEN>
-static int scan_fwd_launch(int out, int cs, int nt, int D, cudaStream_t st, const float* gi, const float* Whh, const float* bhh,
-                           int64_t zW, const float* h0, float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, int B, int T,
-                           const int* len) {
-    constexpr int smem = htc::FwdSmem<HH, NS>::TOTAL;
-    switch (out) {
-        case htc::SCAN_TRAIN:
-            return launch_cluster(htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_TRAIN, LEN>, cs, nt, D, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D, len);
-        case htc::SCAN_INFER_LOWER:
-            return launch_cluster(htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_INFER_LOWER, LEN>, cs, nt, D, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D, len);
-        case htc::SCAN_INFER_TOP:
-            return launch_cluster(htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_INFER_TOP, LEN>, cs, nt, D, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D, len);
+// R: clusters of `kernel` (cs CTAs, smem bytes each) that the current device holds at once, queried once per kernel and device
+template <typename... KArgs>
+static int cluster_residency(void (*kernel)(KArgs...), int cs, int smem, int* R) {
+    static std::mutex mu;
+    static std::map<std::pair<const void*, int>, int> cache;
+    int dev = 0;
+    CUDA_TRY(cudaGetDevice(&dev));
+    const std::pair<const void*, int> key((const void*)kernel, dev);
+    {
+        std::lock_guard<std::mutex> g(mu);
+        const auto it = cache.find(key);
+        if (it != cache.end()) { *R = it->second; return BIGRU_OK; }
     }
-    bigru_set_error("tc_scan_fwd: no kernel writes this set of outputs (Y %d, G %d, planes %d)", Y != nullptr, G != nullptr, yh != nullptr);
-    return BIGRU_ERR_ARG;
+    CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    cudaLaunchAttribute attr[1];
+    const cudaLaunchConfig_t cfg = cluster_config(kernel, cs, 1, 1, smem, 0, attr);
+    int n = 0;
+    CUDA_TRY(cudaOccupancyMaxActiveClusters(&n, (void*)kernel, &cfg));
+    if (n <= 0) { bigru_set_error("scan: no %d-CTA cluster with %d bytes of shared memory fits on this device", cs, smem); return BIGRU_ERR_DEVICE; }
+    {
+        std::lock_guard<std::mutex> g(mu);
+        cache[key] = n;
+    }
+    *R = n;
+    return BIGRU_OK;
+}
+
+// Forward scan geometry.  n = D * B / 16 tiles; R clusters fit at once.  rounds = ceil(n / 2R) rounds of clusters; the
+// n2 = n - rounds * R clusters beyond rounds * R one-tile clusters take two tiles (rounded up to a multiple of D: a
+// cluster's tiles share a direction), so at most rounds * R clusters run.  R >= n / 2 gives one round of two-tile
+// clusters; R >= n gives n one-tile clusters, and so does a kernel without 32-row tiles (two = false).  Results do not
+// depend on the geometry.  Returns m2 = n2 / D, the two-tile clusters per direction, and the cluster count.
+static void scan_geometry(int R, bool two, int B, int D, int* m2, int* clusters) {
+    const int ntd = B / htc::SCAN_NB, n = D * ntd;
+    int n2 = 0;
+    if (two) {
+        const int rounds = (n + 2 * R - 1) / (2 * R);
+        n2 = std::max(0, n - rounds * R);
+        n2 = std::min((n2 + D - 1) / D * D, D * (ntd / 2));
+    }
+    *m2 = n2 / D;
+    *clusters = n - n2;
+}
+
+template <int HH, int NS, bool LEN>
+static int scan_fwd_launch(int out, int cs, int B, int D, cudaStream_t st, const float* gi, const float* Whh, const float* bhh,
+                           int64_t zW, const float* h0, float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, int T,
+                           const int* len, int* geom) {
+    constexpr int smem = htc::FwdSmem<HH, NS>::TOTAL;
+    void (*k)(const float*, const float*, const float*, int64_t, const float*, float*, float*, float*, htc::bf16_t*, htc::bf16_t*,
+              int, int, int, int, const int*) = nullptr;
+    switch (out) {
+        case htc::SCAN_TRAIN: k = htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_TRAIN, LEN>; break;
+        case htc::SCAN_INFER_LOWER: k = htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_INFER_LOWER, LEN>; break;
+        case htc::SCAN_INFER_TOP: k = htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_INFER_TOP, LEN>; break;
+        default:
+            bigru_set_error("tc_scan_fwd: no kernel writes this set of outputs (Y %d, G %d, planes %d)", Y != nullptr, G != nullptr, yh != nullptr);
+            return BIGRU_ERR_ARG;
+    }
+    int R = 0, m2 = 0, clusters = 0;
+    TRY(cluster_residency(k, cs, smem, &R));
+    scan_geometry(R, htc::FwdSmem<HH, NS>::NBMAX == 2 * htc::SCAN_NB, B, D, &m2, &clusters);
+    if (geom) { geom[0] = R; geom[1] = D * m2; return BIGRU_OK; }
+    ProfScope ps(KC_TC_SCAN_FWD, 2.0 * D * B * (double)T * 3 * HH * HH, 0.0, st);
+    return launch_cluster(k, cs, clusters, 1, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D, m2, len);
 }
 
 // one layer's forward recurrence; shapes were validated by the plan (H in {128, 256, 512}, B % 16 == 0).  A null Y, G or yh:
-// that output is not written (the instantiations: all three, planes only, Y only).  len: per-row lengths [B] or null
+// that output is not written (the instantiations: all three, planes only, Y only).  len: per-row lengths [B] or null.
+// geom non-null: launch nothing and return the training instantiation's residency R and two-tile cluster count n2 in
+// geom[0], geom[1] (test support)
 static int tc_scan_fwd(const bigru_plan& p, int l, const float* gi, const float* Whh, const float* bhh, const float* h0,
-                       float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, const int* len, cudaStream_t st) {
-    const int H = p.H, D = p.D, B = p.B, T = p.T, cs = H / htc::SCAN_U, nt = B / htc::SCAN_NB;
+                       float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, const int* len, cudaStream_t st,
+                       int* geom = nullptr) {
+    const int H = p.H, D = p.D, B = p.B, T = p.T, cs = H / htc::SCAN_U;
     const int64_t zW = p.ld_block(l);
-    const int out = (Y ? htc::SCAN_Y : 0) | (G ? htc::SCAN_G : 0) | (yh ? htc::SCAN_PLANES : 0);
-    ProfScope ps(KC_TC_SCAN_FWD, 2.0 * D * B * (double)T * 3 * H * H, 0.0, st);
-#define FWD(HH, NS) return len ? scan_fwd_launch<HH, NS, true>(out, cs, nt, D, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, len) \
-                               : scan_fwd_launch<HH, NS, false>(out, cs, nt, D, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, len)
+    const int out = geom ? htc::SCAN_TRAIN : (Y ? htc::SCAN_Y : 0) | (G ? htc::SCAN_G : 0) | (yh ? htc::SCAN_PLANES : 0);
+#define FWD(HH, NS) return len ? scan_fwd_launch<HH, NS, true>(out, cs, B, D, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, T, len, geom) \
+                               : scan_fwd_launch<HH, NS, false>(out, cs, B, D, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, T, len, geom)
     if (p.prec == BIGRU_PREC_BF16X3) {
         if (H == 128) FWD(128, 3);
         if (H == 256) FWD(256, 3);
@@ -973,14 +1143,37 @@ static int tc_scan_fwd(const bigru_plan& p, int l, const float* gi, const float*
     return BIGRU_ERR_UNSUPPORTED;
 }
 
+// Backward scan geometry.  n = D * B / 16 tiles; R clusters fit at once.  With rounds = ceil(n / R) > 1, the last round
+// holds L = n - (rounds - 1) * R tiles; when 2L <= R they run as 2L clusters of 8 rows, which take less time than L of 16.
+// Results do not depend on the geometry.  Returns L8 = the split tiles and the cluster count.
+static void scan_bwd_geometry(int R, int B, int D, int* L8, int* clusters) {
+    const int n = D * (B / htc::SCAN_NB), rounds = (n + R - 1) / R, L = n - (rounds - 1) * R;
+    *L8 = rounds > 1 && 2 * L <= R ? L : 0;
+    *clusters = n + *L8;
+}
+
+template <int HH, int NS, bool LEN>
+static int scan_bwd_launch(int cs, int B, int D, cudaStream_t st, const float* G, const float* Y, const float* h0, const float* dY,
+                           float* dhc, float* dgi, float* dgh, const float* Whh, int64_t zW, htc::bf16_t* gih, htc::bf16_t* gil,
+                           htc::bf16_t* ghh, htc::bf16_t* ghl, int T, const int* len, int* geom) {
+    constexpr int smem = htc::BwdSmem<HH, NS>::TOTAL;
+    auto k = htc::gru_scan_bwd_kernel<HH, NS, LEN>;
+    int R = 0, L8 = 0, clusters = 0;
+    TRY(cluster_residency(k, cs, smem, &R));
+    scan_bwd_geometry(R, B, D, &L8, &clusters);
+    if (geom) { geom[0] = R; geom[1] = L8; return BIGRU_OK; }
+    ProfScope ps(KC_TC_SCAN_BWD, 2.0 * D * B * (double)T * 3 * HH * HH, 0.0, st);
+    return launch_cluster(k, cs, clusters, 1, smem, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, L8, len);
+}
+
+// one layer's backward recurrence; geom as in tc_scan_fwd (geom[1]: the tiles split into two 8-row clusters)
 static int tc_scan_bwd(const bigru_plan& p, int l, const float* G, const float* Y, const float* h0, const float* dY, float* dhc,
                        float* dgi, float* dgh, const float* Whh, htc::bf16_t* gih, htc::bf16_t* gil, htc::bf16_t* ghh,
-                       htc::bf16_t* ghl, const int* len, cudaStream_t st) {
-    const int H = p.H, D = p.D, B = p.B, T = p.T, cs = H / htc::SCAN_U, nt = B / htc::SCAN_NB;
+                       htc::bf16_t* ghl, const int* len, cudaStream_t st, int* geom = nullptr) {
+    const int H = p.H, D = p.D, B = p.B, T = p.T, cs = H / htc::SCAN_U;
     const int64_t zW = p.ld_block(l);
-    ProfScope ps(KC_TC_SCAN_BWD, 2.0 * D * B * (double)T * 3 * H * H, 0.0, st);
-#define BWD(HH, NS) return len ? launch_cluster(htc::gru_scan_bwd_kernel<HH, NS, true>, cs, nt, D, htc::BwdSmem<HH, NS>::TOTAL, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, len) \
-                           : launch_cluster(htc::gru_scan_bwd_kernel<HH, NS, false>, cs, nt, D, htc::BwdSmem<HH, NS>::TOTAL, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, len)
+#define BWD(HH, NS) return len ? scan_bwd_launch<HH, NS, true>(cs, B, D, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, T, len, geom) \
+                           : scan_bwd_launch<HH, NS, false>(cs, B, D, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, T, len, geom)
     if (p.prec == BIGRU_PREC_BF16X3) {
         if (H == 128) BWD(128, 3);
         if (H == 256) BWD(256, 3);

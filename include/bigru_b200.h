@@ -113,6 +113,13 @@ int  bigru_stash_output_offset(const bigru_plan* plan, int layer, size_t* byte_o
 int  bigru_workspace_region(const bigru_plan* plan, int which, int layer, int* in_scratch, size_t* byte_offset,
                             size_t* lo_byte_offset, int64_t* pitch);
 
+/* --- Recurrence scan geometry of a tensor-core plan on the current device (test support).  *R: clusters of the scan the
+ *  device holds at once.  scan 0, the forward (training instantiation): *n_split = clusters that take two 16-row batch
+ *  tiles (the lowest cluster ids; always 0 at BIGRU_PREC_BF16).  scan 1, the backward: *n_split = batch tiles of the last
+ *  round split into two 8-row clusters each (the highest cluster ids).  No result depends on them.
+ *  BIGRU_PREC_FP32: BIGRU_ERR_UNSUPPORTED; another scan: BIGRU_ERR_ARG. */
+int  bigru_scan_geometry(const bigru_plan* plan, int scan, int* R, int* n_split);
+
 /* --- BiGRU.forward (biGRU_model.py:63-138): dropout :87-94, nn.GRU :102, head :111-137.
  *  d_x[B,T,F]; d_h0 nullable [L*D,B,H] (the `hidden` argument); d_logits[B,C];
  *  d_hn nullable [L*D,B,H]; training!=0 applies dropout p (spatial!=0: per (b,f) channel over T,
