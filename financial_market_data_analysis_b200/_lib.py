@@ -40,6 +40,10 @@ SIGNATURES = {
     "bigru_forward_lengths": (_i, [_vp, _vp, _vp, _vp, _f, _i, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_backward_lengths": (_i, [_vp, _vp, _vp, _vp, _f, _i, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_infer_lengths": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "bigru_gru_plan_create": (_i, [_i, _i, _i, _i, _i, _i, _i, C.POINTER(_vp)]),
+    "bigru_gru_forward": (_i, [_vp, _vp, _vp, _vp, _f, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "bigru_gru_infer": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "bigru_gru_backward": (_i, [_vp, _vp, _vp, _vp, _f, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_loss": (_i, [_i, _vp, _vp, _vp, _vp, _i, _i, _d, _vp, _vp, _vp]),
     "bigru_sqnorm": (_i, [_vp, _i64, _vp, _vp, _vp]),
     "bigru_adam_tick": (_i, [_vp, _vp, _vp]),

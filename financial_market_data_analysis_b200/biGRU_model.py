@@ -12,7 +12,6 @@ process group.  There is no CPU path: parameters must live on a CUDA device.
 """
 from __future__ import annotations
 
-import math
 import os
 from typing import Optional
 
@@ -22,6 +21,8 @@ import torch.nn as nn
 
 if __package__:
     from . import _lib
+    from ._modelbase import _PRECISIONS, _FlatModel, _stream_ptr
+    from .gru import GRU
     from .parallel import allreduce_flat_
 else:
     # drop-in route of the reference's callers (`predict.py:16`, the notebook): this directory itself is on sys.path and
@@ -32,115 +33,10 @@ else:
     if os.path.dirname(_here) not in _sys.path:
         _sys.path.insert(0, os.path.dirname(_here))
     _lib = _importlib.import_module(os.path.basename(_here) + "._lib")
+    _base = _importlib.import_module(os.path.basename(_here) + "._modelbase")
+    _PRECISIONS, _FlatModel, _stream_ptr = _base._PRECISIONS, _base._FlatModel, _base._stream_ptr
+    GRU = _importlib.import_module(os.path.basename(_here) + ".gru").GRU
     allreduce_flat_ = _importlib.import_module(os.path.basename(_here) + ".parallel").allreduce_flat_
-
-_PRECISIONS = {"fp32": _lib.PREC_FP32, "bf16": _lib.PREC_BF16, "bf16x3": _lib.PREC_BF16X3}
-
-
-def _stream_ptr(device=None):
-    """Raw cudaStream_t of torch's current stream ON THE MODEL'S DEVICE (not the process-wide current device)."""
-    return torch.cuda.current_stream(device).cuda_stream
-
-
-class _Padding:
-    """What the C plans of one model run at, and the zero padding between the model's own shapes and the plan's.
-
-    The tensor-core kernels exist for whole batch tiles (32 rows at "bf16x3" and at "bf16" with 512 hidden units, 16 rows
-    otherwise at "bf16") and for 128 / 256 (/ 512 at "bf16") hidden units.  Other batch sizes run with zero rows appended:
-    batch rows are independent and the padded rows receive a zero upstream gradient.  Smaller hidden sizes run with zero
-    units appended (see BiGRU.plan_hidden).  Logits, loss and every gradient of the real rows and parameters are those of
-    the unpadded model (up to summation order)."""
-
-    def __init__(self, model, device):
-        H = model.hidden_size
-        prec = model.precision if model.precision != "auto" else ("bf16x3" if H <= 256 else "fp32")
-        sizes = {"bf16x3": (128, 256), "bf16": (128, 256, 512)}.get(prec, ())
-        self.precision = prec
-        self.hidden = next((hp for hp in sizes if H <= hp), H)
-        self.tile = 32 if (prec == "bf16x3" or (prec == "bf16" and self.hidden == 512)) else (16 if prec == "bf16" else 1)
-        self.padded = self.hidden != H
-        self._dims = (H, model.n_directions, model.n_layers, model.n_features, model.output_size)
-        self._device = device
-        self._index = None
-
-    def batch(self, B: int) -> int:
-        """The batch size a plan runs for B real rows."""
-        return (B + self.tile - 1) // self.tile * self.tile
-
-    def pad(self, t, Bp, dim=0, units=False):
-        """t with zero rows appended along `dim` up to Bp and, when `units`, zero hidden units up to the plan's (last dim)."""
-        if t is None:
-            return None
-        shape = list(t.shape)
-        shape[dim] = Bp
-        if units:
-            shape[-1] = self.hidden
-        if list(t.shape) == shape:
-            return t
-        out = t.new_zeros(shape)
-        out[tuple(slice(0, n) for n in t.shape)] = t
-        return out
-
-    def lengths(self, lens, Bp, T):
-        """Per-row lengths [Bp] of a plan: `lens` (None stays None) with the appended zero rows T steps long."""
-        if lens is None or lens.shape[0] == Bp:
-            return lens
-        out = lens.new_full((Bp,), T)
-        out[:lens.shape[0]] = lens
-        return out
-
-    def crop(self, t, B, dim=0, units=False):
-        """The first B rows along `dim` of a plan-sized tensor and, when `units`, its real hidden units."""
-        if t is None:
-            return None
-        if units and t.shape[-1] != self._dims[0]:
-            t = t[..., :self._dims[0]]
-        return t if t.shape[dim] == B else t.narrow(dim, 0, B)
-
-    def _map(self):
-        """(index tensor, padded parameter count): position of every real parameter inside the padded plan's flat vector."""
-        if self._index is None:
-            H, D, L, F, C = self._dims
-            Hp = self.hidden
-            idx, off_p = [], 0
-
-            def rows(n_cols_pad, col_map):
-                # a [3H][cols] block -> padded [3Hp][cols_pad]: row g*H + j -> g*Hp + j, column through col_map
-                r = (np.arange(3)[:, None] * Hp + np.arange(H)[None, :]).reshape(-1)
-                return (r[:, None] * n_cols_pad + col_map[None, :]).reshape(-1)
-
-            for l in range(L):
-                Ip = F if l == 0 else D * Hp
-                cm = np.arange(F) if l == 0 else (np.arange(D)[:, None] * Hp + np.arange(H)[None, :]).reshape(-1)
-                for d in range(D):
-                    idx.append(off_p + rows(Ip, cm)); off_p += 3 * Hp * Ip                         # W_ih
-                    idx.append(off_p + rows(Hp, np.arange(H))); off_p += 3 * Hp * Hp               # W_hh
-                    b = (np.arange(3)[:, None] * Hp + np.arange(H)[None, :]).reshape(-1)
-                    idx.append(off_p + b); off_p += 3 * Hp                                        # b_ih
-                    idx.append(off_p + b); off_p += 3 * Hp                                        # b_hh
-            cmh = (np.arange(3)[:, None] * Hp + np.arange(H)[None, :]).reshape(-1)                # head: last | max | avg, H wide each
-            idx.append(off_p + (np.arange(C)[:, None] * 3 * Hp + cmh[None, :]).reshape(-1)); off_p += C * 3 * Hp
-            idx.append(off_p + np.arange(C)); off_p += C
-            self._index = (torch.from_numpy(np.concatenate(idx).astype(np.int64)).to(self._device), off_p)
-        return self._index
-
-    def params(self, flat, out=None):
-        """The flat parameter vector as the plan sees it: `flat` itself, or its entries scattered into a zero-padded vector
-        (`out` when given; its padded entries must be zero)."""
-        if not self.padded:
-            return flat
-        index, n = self._map()
-        assert index.numel() == flat.numel()
-        if out is None:
-            out = flat.new_zeros(n)
-        return out.index_copy_(0, index, flat.detach())
-
-    def grads(self, pgrad, out=None):
-        """The real parameters' entries of a plan-sized gradient vector (into `out` when given)."""
-        if not self.padded:
-            return pgrad
-        return torch.index_select(pgrad, 0, self._map()[0], out=out) if out is not None else torch.index_select(pgrad, 0, self._map()[0])
-
 
 class _AdamState:
     """Optimiser state of the fused step.  The flat gradient and the scalar loss share one buffer (``gext`` = P gradients + 1
@@ -183,82 +79,6 @@ class _StepBuffers:
         self.logits = torch.empty(Bp, C, device=x.device, dtype=torch.float32)
         # the loss writes dlogits of the real rows only: the padded rows stay zero
         self.dlogits = (torch.zeros if Bp != tgt.shape[0] else torch.empty)(Bp, C, device=x.device, dtype=torch.float32)
-
-
-class _GRUWeights(nn.Module):
-    """Holds the recurrent parameters under torch.nn.GRU's names, shapes, registration order and
-    initialisation (U(-1/sqrt(H), 1/sqrt(H)), drawn in registration order), i.e. what
-    biGRU_model.py:54-56 constructs.  It has no forward of its own: the recurrence runs inside
-    libbigru_b200."""
-
-    def __init__(self, input_size, hidden_size, num_layers, bidirectional, dropout):
-        super().__init__()
-        self.input_size, self.hidden_size, self.num_layers = input_size, hidden_size, num_layers
-        self.bidirectional, self.dropout, self.batch_first, self.bias = bidirectional, float(dropout), True, True
-        dirs = 2 if bidirectional else 1
-        for layer in range(num_layers):
-            fan = input_size if layer == 0 else hidden_size * dirs
-            for d in range(dirs):
-                sfx = f"l{layer}" + ("_reverse" if d else "")
-                self.register_parameter(f"weight_ih_{sfx}", nn.Parameter(torch.empty(3 * hidden_size, fan)))
-                self.register_parameter(f"weight_hh_{sfx}", nn.Parameter(torch.empty(3 * hidden_size, hidden_size)))
-                self.register_parameter(f"bias_ih_{sfx}", nn.Parameter(torch.empty(3 * hidden_size)))
-                self.register_parameter(f"bias_hh_{sfx}", nn.Parameter(torch.empty(3 * hidden_size)))
-        bound = 1.0 / math.sqrt(hidden_size) if hidden_size > 0 else 0.0
-        with torch.no_grad():
-            for p in self.parameters():
-                p.uniform_(-bound, bound)
-
-    def forward(self, *args, **kwargs):
-        raise RuntimeError("BiGRU.gru only stores parameters; call BiGRU.forward (libbigru_b200 runs the recurrence)")
-
-
-class _Plan:
-    """A C plan plus its device workspaces for one (B, T) shape.  Each workspace is allocated on first use: a plan that only
-    runs ``BiGRU.infer`` holds the inference workspace alone, not the stash and scratch of the training forward."""
-
-    def __init__(self, model: "BiGRU", B: int, T: int, device):
-        lib = _lib.load()
-        _lib.check(lib.bigru_device_check(device.index if device.index is not None else torch.cuda.current_device()),
-                   "bigru_device_check")
-        h = _lib.C.c_void_p()
-        _lib.check(lib.bigru_plan_create(B, T, model.n_features, model.plan_hidden(B), model.n_layers, model.output_size,
-                                         int(model.bidirectional), _PRECISIONS[model.resolved_precision(B)], _lib.C.byref(h)),
-                   "bigru_plan_create")
-        self.handle, self.B, self.T, self.device = h, B, T, device
-        a, b, c = _lib.C.c_size_t(), _lib.C.c_size_t(), _lib.C.c_size_t()
-        _lib.check(lib.bigru_workspace_bytes(h, _lib.C.byref(a), _lib.C.byref(b)), "bigru_workspace_bytes")
-        _lib.check(lib.bigru_infer_workspace_bytes(h, _lib.C.byref(c)), "bigru_infer_workspace_bytes")
-        self.stash_bytes, self.scratch_bytes, self.infer_bytes = a.value, b.value, c.value
-        self._scratch = self._infer_ws = None
-        self._free_stash = []
-
-    @property
-    def scratch(self):
-        if self._scratch is None:
-            self._scratch = torch.empty(max(self.scratch_bytes, 16), dtype=torch.uint8, device=self.device)
-        return self._scratch
-
-    def infer_workspace(self):
-        if self._infer_ws is None:
-            self._infer_ws = torch.empty(max(self.infer_bytes, 16), dtype=torch.uint8, device=self.device)
-        return self._infer_ws
-
-    def acquire_stash(self):
-        if self._free_stash:
-            return self._free_stash.pop()
-        return torch.empty(max(self.stash_bytes, 16), dtype=torch.uint8, device=self.device)
-
-    def release_stash(self, s):
-        if len(self._free_stash) < 2:
-            self._free_stash.append(s)
-
-    def __del__(self):
-        try:
-            if self.handle:
-                _lib.load().bigru_plan_destroy(self.handle)
-        except Exception:
-            pass
 
 
 class _BiGRUFunction(torch.autograd.Function):
@@ -320,7 +140,7 @@ class _BiGRUFunction(torch.autograd.Function):
         return (None, pad.crop(dx, B), pad.crop(dh0, B, dim=1, units=True), None) + pg
 
 
-class BiGRU(nn.Module):
+class BiGRU(_FlatModel):
     """Bidirectional GRU classifier (reference: biGRU_model.py:8).
 
     Parameters (same order and defaults as the reference, :32-33): hidden_size, n_features,
@@ -356,7 +176,8 @@ class BiGRU(nn.Module):
         self.dropout = nn.Dropout(self.dropout_p)
         if self.spatial_dropout:
             self.spatial_dropout1d = nn.Dropout2d(self.dropout_p)
-        self.gru = _GRUWeights(n_features, hidden_size, n_layers, bidirectional, 0 if n_layers == 1 else dropout)
+        self.gru = GRU(n_features, hidden_size, n_layers, batch_first=True, dropout=0 if n_layers == 1 else dropout,
+                       bidirectional=bidirectional, precision=self.precision)
         self.linear = nn.Linear(hidden_size * 3, output_size)
 
         self.device = torch.device("cpu")
@@ -387,53 +208,35 @@ class BiGRU(nn.Module):
         out += [self.linear.weight, self.linear.bias]
         return out
 
+    _kind = "BiGRU"
+
+    def _dims(self):
+        return self.hidden_size, self.n_directions, self.n_layers, self.n_features, self.output_size
+
+    def _create_plan(self, lib, B, T, out):
+        _lib.check(lib.bigru_plan_create(B, T, self.n_features, self.plan_hidden(B), self.n_layers, self.output_size,
+                                         int(self.bidirectional), _PRECISIONS[self.resolved_precision(B)], _lib.C.byref(out)),
+                   "bigru_plan_create")
+
     def _flatten(self):
-        """(Re)pack every parameter into one contiguous vector and make the nn.Parameters views of it,
-        keeping the Parameter objects (optimisers hold references to them)."""
-        params = self._ordered_params()
-        dev = params[0].device
-        total = sum(p.numel() for p in params)
-        flat = torch.empty(total, dtype=torch.float32, device=dev)
-        views, off = [], 0
-        with torch.no_grad():
-            for p in params:
-                n = p.numel()
-                flat[off:off + n].copy_(p.detach().reshape(-1).to(device=dev, dtype=torch.float32))
-                p.data = flat[off:off + n].view(p.shape)
-                views.append((off, n, tuple(p.shape)))
-                off += n
+        """(Re)pack every parameter into one contiguous vector (the recurrent prefix of which is also ``self.gru``'s), keeping
+        the Parameter objects and the fused step's Adam moments."""
+        super()._flatten()
+        self.gru._adopt(self._flat[:self.gru_param_count()], self._views[:4 * self.n_layers * self.n_directions])
+        total = self._flat.numel()
         old = getattr(self, "_adam", None)
-        self._flat, self._views = flat, views
-        self._pad = _Padding(self, dev)
-        self._plans = {}
         self._graphs = {}
         self._adam = None
         if old is not None and old.m.numel() == total:          # keep the Adam moments across a re-flatten (.to() / .cuda())
             st = self._fused_state()
-            st.m.copy_(old.m.to(dev)); st.v.copy_(old.v.to(dev))
+            st.m.copy_(old.m.to(self._flat.device)); st.v.copy_(old.v.to(self._flat.device))
             st.step = old.step
             st.dstep.fill_(old.step)
             self._mirror_optimizer_state()
 
-    def _is_flat(self):
-        f = self._flat
-        if f is None:
-            return False
-        base = f.data_ptr()
-        for p, (off, n, _) in zip(self._ordered_params(), self._views):
-            if p.device != f.device or p.dtype != torch.float32 or p.data_ptr() != base + 4 * off:
-                return False
-        return True
-
-    def _apply(self, fn, *args, **kwargs):
-        out = super()._apply(fn, *args, **kwargs)       # .cuda() / .to() create fresh tensors per parameter
-        self._flatten()
-        return out
-
-    def flat_parameters(self) -> torch.Tensor:
-        if not self._is_flat():
-            self._flatten()
-        return self._flat
+    def gru_param_count(self) -> int:
+        """Entries of the flat vector that belong to ``self.gru`` (its leading part, in nn.GRU's order)."""
+        return self._flat.numel() - self.linear.weight.numel() - self.linear.bias.numel()
 
     # ------------------------------------------------------------------ plans
     def resolved_precision(self, batch: int = 0) -> str:
@@ -450,59 +253,6 @@ class BiGRU(nn.Module):
     def _padded_batch(self, batch: int) -> int:
         """The batch size a plan runs for `batch` real rows (whole batch tiles on the tensor-core paths, _Padding)."""
         return self._pad.batch(batch)
-
-    def _plan_params(self, out=None):
-        """The flat parameter vector as the C plan sees it (zero-padded hidden units scattered in when plan_hidden() > hidden_size)."""
-        return self._pad.params(self._flat, out)
-
-    def _plan_grads(self, pgrad, out=None):
-        """The real parameters' entries of a plan-sized gradient vector."""
-        return self._pad.grads(pgrad, out)
-
-    def _plan_for(self, x) -> _Plan:
-        key = (int(x.shape[0]), int(x.shape[1]), self.resolved_precision(int(x.shape[0])), x.device.index)
-        plan = self._plans.get(key)
-        if plan is None:
-            if len(self._plans) > 8:
-                self._plans.clear()
-            plan = self._plans[key] = _Plan(self, key[0], key[1], x.device)
-        return plan
-
-    def _prepare_input(self, input_seq, hidden):
-        if not self._is_flat():
-            self._flatten()
-        dev = self._flat.device
-        if dev.type != "cuda":
-            raise RuntimeError("BiGRU (H100-native) has no CPU path: move the model to a CUDA device with .cuda() first")
-        if input_seq.dim() != 3 or input_seq.shape[2] != self.n_features:
-            raise ValueError(f"input_seq must be [batch, seq_len, {self.n_features}], got {tuple(input_seq.shape)}")
-        x = input_seq.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
-        h0 = None
-        if hidden is not None:
-            want = (self.n_layers * self.n_directions, x.shape[0], self.hidden_size)
-            if tuple(hidden.shape) != want:
-                raise RuntimeError(f"Expected hidden size {want}, got {tuple(hidden.shape)}")
-            h0 = hidden.to(device=dev, dtype=torch.float32).contiguous()
-        return x, h0
-
-    @staticmethod
-    def _prepare_lengths(lengths, x, hidden):
-        """`lengths` (a list, a CPU or a CUDA tensor of integers) as an int32 tensor [B] on x's device, checked on the host:
-        shape [B], every value in [1, T], and no initial state with it.  None stays None (every row T steps long)."""
-        if lengths is None:
-            return None
-        if hidden is not None:
-            raise ValueError("lengths together with an initial hidden state (hidden) are not supported")
-        B, T = int(x.shape[0]), int(x.shape[1])
-        host = lengths.detach().cpu() if isinstance(lengths, torch.Tensor) else torch.as_tensor(lengths)
-        if host.dtype.is_floating_point or host.dtype.is_complex or host.dtype == torch.bool:
-            raise ValueError(f"lengths must hold integers, got {host.dtype}")
-        if tuple(host.shape) != (B,):
-            raise ValueError(f"lengths must have shape [{B}] (one per batch row), got {tuple(host.shape)}")
-        if B and (int(host.min()) < 1 or int(host.max()) > T):
-            raise ValueError(f"every length must lie in [1, {T}], got values from {int(host.min())} to {int(host.max())}")
-        # from pinned memory, so that the copy does not wait for the work already queued on the stream
-        return host.to(torch.int32).pin_memory().to(x.device, non_blocking=True)
 
     def pooled_argmax(self) -> torch.Tensor:
         """argmax_t of the max-pooled direction sum [batch, hidden] as taken by the last ``forward`` (the routing of the

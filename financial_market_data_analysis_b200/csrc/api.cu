@@ -17,7 +17,7 @@ void bigru_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* bigru_last_error(void) { return g_err; }
-extern "C" int bigru_version(void) { return 208; }
+extern "C" int bigru_version(void) { return 209; }
 
 extern "C" int bigru_device_check(int dev) {
     int n = 0;
@@ -40,6 +40,9 @@ extern "C" int bigru_device_check(int dev) {
 // ------------------------------------------------------------------------------------------
 // Tensor-core precisions add bf16 planes of the GEMM operands (hi, and lo at bf16x3; see tc_hopper.cuh) in their
 // producers' layouts.  Plane offsets are rounded to 64 floats: TMA needs 16-byte aligned bases.
+// A plan with C = 0 (bigru_gru_plan_create) has no pooling head: it is nn.GRU.  Its top layer's fp32 Y is the caller's d_y, so
+// its stash keeps no top-layer Y, no cat and no arg, and its scratch no dcat; every other region is that of a plan with a head.
+static inline bool has_head(const bigru_plan& p) { return p.C > 0; }
 struct StashF32 {       // kept forward -> backward
     int64_t Y[16], G[16], X[16];   // per layer: output [B*T*D*H], gates [D][B*T][4H], dropped input [B*T*I_l]
     int64_t YP[16], XP[16];        // per layer: planes of Y [B*T][D*H] and of the layer input [B*T][in_pitch(l)]
@@ -58,15 +61,15 @@ static StashF32 stash_layout(const bigru_plan& p) {
     int64_t o = 0;
     const int64_t BT = (int64_t)p.B * p.T;
     for (int l = 0; l < p.L; ++l) {
-        s.Y[l] = o; o += BT * p.D * p.H;
+        s.Y[l] = o; if (has_head(p) || l < p.L - 1) o += BT * p.D * p.H;
         s.G[l] = o; o += (int64_t)p.D * BT * 4 * p.H;
         s.X[l] = o; o += BT * p.in_size(l);
         o = rup(o, 64);
         s.YP[l] = o; o += plane_floats(p, BT * p.D * p.H);
         s.XP[l] = o; o += plane_floats(p, BT * in_pitch(p, l));
     }
-    s.cat = o; o += (int64_t)p.B * 3 * p.H;
-    s.arg = o; o += (int64_t)p.B * p.H;
+    s.cat = o; if (has_head(p)) o += (int64_t)p.B * 3 * p.H;
+    s.arg = o; if (has_head(p)) o += (int64_t)p.B * p.H;
     s.total = o;
     return s;
 }
@@ -88,7 +91,7 @@ static ScratchF32 scratch_layout(const bigru_plan& p) {
     s.dYa = o; o += BT * wide;
     s.dYb = o; o += BT * wide;
     s.dhc = o; o += (int64_t)p.D * p.B * p.H;
-    s.dcat = o; o += (int64_t)p.B * 3 * p.H;
+    s.dcat = o; if (has_head(p)) o += (int64_t)p.B * 3 * p.H;
     s.csum = o; o += (int64_t)COLSUM_MAX_CHUNKS * (3 * p.H > p.C ? 3 * p.H : p.C);   // colsum_launch partials
     o = rup(o, 64);
     s.dgiP = o; o += plane_floats(p, (int64_t)p.D * BT * 3 * p.H);                     // planes of dgi, dgh
@@ -106,7 +109,7 @@ static ScratchF32 scratch_layout(const bigru_plan& p) {
         }
         const int64_t h[4] = {tc_gemm_ws_elems(B, C, H3, 1, p.prec), tc_gemm_ws_elems(B, H3, C, 1, p.prec),
                               tc_gemm_ws_elems(C, H3, B, 1, p.prec), tc_gemm_ws_elems(H3, p.H, B, 1, p.prec)};   // head, w0
-        for (int64_t v : h) need = std::max(need, v);
+        for (int i = has_head(p) ? 0 : 3; i < 4; ++i) need = std::max(need, h[i]);
         o += plane_floats(p, need);
         s.part = o; o += part;
     }
@@ -117,7 +120,8 @@ static ScratchF32 scratch_layout(const bigru_plan& p) {
 // layer.  Tensor-core precisions: a lower layer writes only its Y planes (yp[l % 2]; none at L = 1, one buffer at L = 2,
 // ping-pong from L = 3), the top layer only its fp32 Y (y[0]), which the pooling head reads; tcw holds the packed W_ih and
 // head operands.  fp32: every layer writes fp32 Y into y[l % 2] (its per-step gh GEMM reads h_{t-1} from there) and gh is
-// the per-step gh buffer; no planes, no tcw.
+// the per-step gh buffer; no planes, no tcw.  Head-less plans (bigru_gru_infer): the top layer writes the caller's d_y, so
+// y[0] exists only at fp32 below the top (L > 1), y[1] only at fp32 from L = 3; no cat, no arg, no head operands.
 struct InferF32 {
     int64_t gi, gh, y[2], cat, arg, xp, yp[2], tcw, total;
 };
@@ -128,17 +132,18 @@ static InferF32 infer_layout(const bigru_plan& p) {
     const bool tc = p.prec != BIGRU_PREC_FP32;
     s.gi = o; o += (int64_t)p.D * BT * 3 * p.H;
     s.gh = o; if (!tc) o += (int64_t)p.D * p.B * 3 * p.H;
-    s.y[0] = o; o += BT * DH;
-    s.y[1] = o; if (!tc && p.L > 1) o += BT * DH;
-    s.cat = o; o += (int64_t)p.B * 3 * p.H;
-    s.arg = o; o += (int64_t)p.B * p.H;
+    const int in_ws = has_head(p) ? p.L : p.L - 1;            // layers whose fp32 Y lives in the workspace at fp32
+    s.y[0] = o; if (tc ? has_head(p) : in_ws >= 1) o += BT * DH;
+    s.y[1] = o; if (!tc && in_ws >= 2) o += BT * DH;
+    s.cat = o; if (has_head(p)) o += (int64_t)p.B * 3 * p.H;
+    s.arg = o; if (has_head(p)) o += (int64_t)p.B * p.H;
     o = rup(o, 64);
     s.xp = o; o += plane_floats(p, BT * in_pitch(p, 0));
     s.yp[0] = o; if (p.L > 1) o += plane_floats(p, BT * DH);
     s.yp[1] = o; if (p.L > 2) o += plane_floats(p, BT * DH);
     s.tcw = o;
     if (tc) {
-        int64_t need = tc_gemm_ws_elems(p.B, p.C, 3LL * p.H, 1, p.prec);                       // head
+        int64_t need = has_head(p) ? tc_gemm_ws_elems(p.B, p.C, 3LL * p.H, 1, p.prec) : 0;    // head
         for (int l = 0; l < p.L; ++l) need = std::max(need, tc_pack_elems(3LL * p.H, p.in_size(l), p.D, p.prec));   // W_ih
         o += plane_floats(p, need);
     }
@@ -181,13 +186,19 @@ static Planes input_planes(const bigru_plan& p, const float* planes, int l, bool
     return own ? plan_planes(p, planes, 0, p.in_size(l), BT, 1, in_pitch(p, l))
                : plan_planes(p, planes, 0, (int64_t)p.D * p.H, BT, 1, (int64_t)p.D * p.H);
 }
+// Whether layer l reads a dropped copy of its input in training with dropout: BiGRU drops every layer's input (layer 0: its
+// input dropout, above: nn.GRU's inter-layer dropout); a head-less plan is nn.GRU(dropout=p), which never drops x.  Layer l's
+// input has planes of its own (`own`) at layer 0 and wherever it is dropped; otherwise it reads the previous layer's Y planes.
+// The forward and the backward both ask here, so the backward reads the copies and planes the forward wrote.
+static inline bool input_dropped(const bigru_plan& p, bool do_drop, int l) { return do_drop && (l > 0 || has_head(p)); }
+static inline bool own_planes(const bigru_plan& p, bool do_drop, int l) { return l == 0 || input_dropped(p, do_drop, l); }
 static htc::bf16_t* mut(const Planes& q) { return const_cast<htc::bf16_t*>(q.hi); }
 static htc::bf16_t* mut_lo(const Planes& q) { return const_cast<htc::bf16_t*>(q.lo); }
 
-extern "C" int bigru_plan_create(int B, int T, int F, int H, int L, int C, int bidirectional, int precision,
-                                 bigru_plan** out) {
+// C = 0: the head-less plan of bigru_gru_plan_create
+static int plan_create(int B, int T, int F, int H, int L, int C, int bidirectional, int precision, bigru_plan** out) {
     if (!out) { bigru_set_error("plan_create: out is null"); return BIGRU_ERR_ARG; }
-    if (B <= 0 || T <= 0 || F <= 0 || H <= 0 || L <= 0 || L > 16 || C <= 0) {
+    if (B <= 0 || T <= 0 || F <= 0 || H <= 0 || L <= 0 || L > 16 || C < 0) {
         bigru_set_error("plan_create: bad shape B=%d T=%d F=%d H=%d L=%d C=%d", B, T, F, H, L, C);
         return BIGRU_ERR_ARG;
     }
@@ -209,6 +220,20 @@ extern "C" int bigru_plan_create(int B, int T, int F, int H, int L, int C, int b
     return BIGRU_OK;
 }
 
+extern "C" int bigru_plan_create(int B, int T, int F, int H, int L, int C, int bidirectional, int precision,
+                                 bigru_plan** out) {
+    if (C <= 0) {
+        bigru_set_error("plan_create: bad shape B=%d T=%d F=%d H=%d L=%d C=%d (bigru_gru_plan_create makes a plan without a head)",
+                        B, T, F, H, L, C);
+        return BIGRU_ERR_ARG;
+    }
+    return plan_create(B, T, F, H, L, C, bidirectional, precision, out);
+}
+
+extern "C" int bigru_gru_plan_create(int B, int T, int F, int H, int L, int bidirectional, int precision, bigru_plan** out) {
+    return plan_create(B, T, F, H, L, 0, bidirectional, precision, out);
+}
+
 extern "C" int bigru_plan_destroy(bigru_plan* plan) { delete plan; return BIGRU_OK; }
 extern "C" int64_t bigru_param_count(const bigru_plan* plan) { return plan ? plan->nparams : -1; }
 
@@ -219,6 +244,7 @@ extern "C" int bigru_param_offset(const bigru_plan* p, int layer, int dir, int w
         return BIGRU_ERR_ARG;
     }
     if (layer == p->L) {
+        if (!has_head(*p)) { bigru_set_error("param_offset: a plan without a head has layers 0..L-1 only"); return BIGRU_ERR_ARG; }
         if (which == 0) { *offset = p->off_linw(); *rows = p->C; *cols = 3 * p->H; }
         else if (which == 2) { *offset = p->off_linb(); *rows = p->C; *cols = 1; }
         else { bigru_set_error("param_offset: linear has which 0 (weight) or 2 (bias)"); return BIGRU_ERR_ARG; }
@@ -243,6 +269,7 @@ extern "C" int bigru_workspace_bytes(const bigru_plan* p, size_t* stash_bytes, s
 // where the head keeps argmax_t of the pooled output (int32 [B][H]) inside the stash of the last forward
 extern "C" int bigru_stash_argmax_offset(const bigru_plan* p, size_t* byte_offset) {
     if (!p || !byte_offset) { bigru_set_error("stash_argmax_offset: null argument"); return BIGRU_ERR_ARG; }
+    if (!has_head(*p)) { bigru_set_error("stash_argmax_offset: a plan without a head pools nothing"); return BIGRU_ERR_ARG; }
     *byte_offset = (size_t)stash_layout(*p).arg * sizeof(float);
     return BIGRU_OK;
 }
@@ -250,6 +277,10 @@ extern "C" int bigru_stash_argmax_offset(const bigru_plan* p, size_t* byte_offse
 // where the forward keeps layer l's output Y[B][T][D*H] (fp32) inside the stash
 extern "C" int bigru_stash_output_offset(const bigru_plan* p, int layer, size_t* byte_offset) {
     if (!p || !byte_offset || layer < 0 || layer >= p->L) { bigru_set_error("stash_output_offset: bad argument"); return BIGRU_ERR_ARG; }
+    if (!has_head(*p) && layer == p->L - 1) {
+        bigru_set_error("stash_output_offset: a plan without a head writes its top layer's output into the caller's d_y");
+        return BIGRU_ERR_ARG;
+    }
     *byte_offset = (size_t)stash_layout(*p).Y[layer] * sizeof(float);
     return BIGRU_OK;
 }
@@ -276,10 +307,11 @@ extern "C" int bigru_workspace_region(const bigru_plan* p, int which, int layer,
                         which == BIGRU_WS_DGH_PLANES;
     const bool stashed = which == BIGRU_WS_GATES || which == BIGRU_WS_Y_PLANES || which == BIGRU_WS_IN_PLANES;
     // stash regions exist for every layer; the scratch keeps layer 0's recurrence gradients, the upstream gradients of layers
-    // 0 and 1 and the head's dcat (layer L, as in bigru_param_offset)
+    // 0 and 1 and the head's dcat (layer L, as in bigru_param_offset).  A head-less plan has no dcat, and its top layer's
+    // upstream gradient is the caller's d_dy
     const bool layer_ok = stashed ? layer >= 0 && layer < p->L
-                        : which == BIGRU_WS_DY ? layer >= 0 && layer < p->L && layer < 2
-                        : which == BIGRU_WS_DCAT ? layer == p->L : layer == 0;
+                        : which == BIGRU_WS_DY ? layer >= 0 && layer < p->L && layer < 2 && (has_head(*p) || layer < p->L - 1)
+                        : which == BIGRU_WS_DCAT ? layer == p->L && has_head(*p) : layer == 0;
     if (which < 0 || which >= BIGRU_WS_COUNT || !layer_ok) {
         bigru_set_error("workspace_region: bad region %d or layer %d", which, layer);
         return BIGRU_ERR_ARG;
@@ -351,7 +383,8 @@ static FwdBufs infer_bufs(const bigru_plan& p, float* ws) {
     return b;
 }
 
-// len: per-row lengths [B] (device, 1 <= len <= T; the caller validates them) or null for T everywhere
+// len: per-row lengths [B] (device, 1 <= len <= T; the caller validates them) or null for T everywhere.  A plan without a head
+// runs the same sequence without the pooling head (logits unused); its buf.Y[L-1] is the caller's d_y.
 static int forward_plan(const bigru_plan& p, const float* params, const float* x, const float* h0, const int* len, float drop,
                         int spatial, int training, uint64_t seed, const FwdBufs& buf, float* logits, float* hn,
                         cudaStream_t st) {
@@ -369,7 +402,7 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
     const float* inp = x;
     for (int l = 0; l < p.L; ++l) {
         const int I = (int)p.in_size(l);
-        if (do_drop && (l == 0 || p.L > 1)) {
+        if (input_dropped(p, do_drop, l)) {
             // l == 0: input dropout (elementwise or per-channel); l > 0: nn.GRU inter-layer dropout
             float* xd = buf.X[l];
             KLAUNCH(KC_MISC, 0.0, 0.0, st, dropout_kernel<<<132 * 8, 256, 0, st>>>(inp, xd, BT * I, T, I, l == 0 ? spatial : 0, drop, seed, (uint32_t)l));
@@ -380,7 +413,7 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
         const float* h0l = h0 ? h0 + (int64_t)l * D * B * H : nullptr;
         float* hnl = hn ? hn + (int64_t)l * D * B * H : nullptr;
         if (p.prec != BIGRU_PREC_FP32) {
-            const bool own = l == 0 || do_drop;
+            const bool own = own_planes(p, do_drop, l);
             const Planes xp = input_planes(p, own ? buf.XP[l] : buf.YP[l - 1], l, own);
             if (own)
                 KLAUNCH(KC_PACK, 0.0, 0.0, st, htc::to_planes_kernel<<<132 * 8, 256, 0, st>>>(inp, BT, I, (int)xp.pitch, mut(xp), mut_lo(xp)));
@@ -433,6 +466,7 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
         }
         inp = Y;
     }
+    if (!has_head(p)) return BIGRU_OK;
     KLAUNCH(KC_HEAD, 0.0, 0.0, st, head_pool_kernel<<<nblk((int64_t)B * H, 128), 128, 0, st>>>(buf.Y[p.L - 1], buf.cat, (int*)buf.arg, B, T, H, D, len));
     GemmArgs lin = gemm_args(buf.cat, params + p.off_linw(), logits, B, p.C, 3 * H, 3 * H, 1, 3 * H, 1, p.C);
     lin.bias = params + p.off_linb();
@@ -442,10 +476,13 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
 
 // ------------------------------------------------------------------------------------------
 // backward: the head, then layers L-1 .. 0.  The upstream gradient of layer l lives in dYa when L-1-l is even, else in dYb.
+// A plan without a head skips the head: its top layer reads its output from y and its upstream gradient from dy, and
+// layer l's carry starts from dhn's slice l (the gradient of h_n; null: zero) instead of the head's d(last) or zero.
 // ------------------------------------------------------------------------------------------
 static int backward_plan(const bigru_plan& p, const float* params, const float* x, const float* h0, const int* len, float drop,
                          int spatial, int training, uint64_t seed, const float* stash, float* scratch,
-                         const float* dlogits, float* grads, float* dx, float* dh0, cudaStream_t st) {
+                         const float* dlogits, const float* y, const float* dy, const float* dhn, float* grads, float* dx,
+                         float* dh0, cudaStream_t st) {
     if (len && (h0 || dh0)) {
         bigru_set_error("backward: lengths together with an initial hidden state or its gradient are not supported");
         return BIGRU_ERR_UNSUPPORTED;
@@ -462,26 +499,32 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
     const bool tc = p.prec != BIGRU_PREC_FP32;
     float* dhc = scratch + W.dhc;
     htc::bf16_t* tcw = reinterpret_cast<htc::bf16_t*>(scratch + W.tcw);
+    const bool head = has_head(p);
     CUDA_TRY(cudaMemsetAsync(grads, 0, sizeof(float) * p.nparams, st));
-    // head: dcat = dlogits lin_w ; dlin_w = dlogits^T cat ; dlin_b = colsum(dlogits)
-    GemmArgs a = gemm_args(dlogits, params + p.off_linw(), scratch + W.dcat, B, 3 * H, C, C, 1, 1, 3 * H, 3 * H);
-    TRY(plan_gemm(p, a, KC_HEAD, tcw, st));
-    GemmArgs w = gemm_args(dlogits, stash + S.cat, grads + p.off_linw(), C, 3 * H, B, 1, C, 1, 3 * H, 3 * H);
-    TRY(plan_gemm(p, w, KC_HEAD, tcw, st));
-    TRY(colsum_launch(dlogits, grads + p.off_linb(), B, C, C, 1, 0, 0, scratch + W.csum, st));
-    KLAUNCH(KC_HEAD, 0.0, 0.0, st, head_bwd_dy_kernel<<<nblk(BT * H, 256), 256, 0, st>>>(scratch + W.dcat, (const int*)(stash + S.arg), scratch + W.dYa, dhc, B, T, H, D, len));
+    if (head) {
+        // head: dcat = dlogits lin_w ; dlin_w = dlogits^T cat ; dlin_b = colsum(dlogits)
+        GemmArgs a = gemm_args(dlogits, params + p.off_linw(), scratch + W.dcat, B, 3 * H, C, C, 1, 1, 3 * H, 3 * H);
+        TRY(plan_gemm(p, a, KC_HEAD, tcw, st));
+        GemmArgs w = gemm_args(dlogits, stash + S.cat, grads + p.off_linw(), C, 3 * H, B, 1, C, 1, 3 * H, 3 * H);
+        TRY(plan_gemm(p, w, KC_HEAD, tcw, st));
+        TRY(colsum_launch(dlogits, grads + p.off_linb(), B, C, C, 1, 0, 0, scratch + W.csum, st));
+        KLAUNCH(KC_HEAD, 0.0, 0.0, st, head_bwd_dy_kernel<<<nblk(BT * H, 256), 256, 0, st>>>(scratch + W.dcat, (const int*)(stash + S.arg), scratch + W.dYa, dhc, B, T, H, D, len));
+    }
     for (int l = p.L - 1; l >= 0; --l) {
         const int I = (int)p.in_size(l);
         const bool even = (p.L - 1 - l) % 2 == 0;
-        const bool drop_l = do_drop && (l == 0 || p.L > 1);
-        float* dY = scratch + (even ? W.dYa : W.dYb);
+        const bool drop_l = input_dropped(p, do_drop, l);
+        const bool caller_top = !head && l == p.L - 1;           // output and upstream gradient in the caller's y, dy
+        const float* dY = caller_top ? dy : scratch + (even ? W.dYa : W.dYb);
         float* dYnext = scratch + (even ? W.dYb : W.dYa);
-        const float* Y = stash + S.Y[l];
+        const float* Y = caller_top ? y : stash + S.Y[l];
         const float* G = stash + S.G[l];
         const float* h0l = h0 ? h0 + (int64_t)l * D * B * H : nullptr;
         float* dgi = scratch + W.dgi;
         float* dgh = scratch + W.dgh;
-        if (l != p.L - 1) CUDA_TRY(cudaMemsetAsync(dhc, 0, sizeof(float) * D * B * H, st));
+        if (!head && dhn) CUDA_TRY(cudaMemcpyAsync(dhc, dhn + (int64_t)l * D * B * H, sizeof(float) * D * B * H,
+                                                   cudaMemcpyDeviceToDevice, st));
+        else if (!head || l != p.L - 1) CUDA_TRY(cudaMemsetAsync(dhc, 0, sizeof(float) * D * B * H, st));
         const Planes gip = plan_planes(p, scratch, W.dgiP, H3, BT, D, H3);
         const Planes ghp = plan_planes(p, scratch, W.dghP, H3, BT, D, H3);
         // recurrence: dgi, dgh [D][B*T][3H] and dh0 in dhc
@@ -511,7 +554,7 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
                 htc::WgJob j = wg_job(grads + p.off_wih(l, 0), (int)H3, I, I, D, kb);
                 j.zC = p.ld_block(l); j.a.zsel = 1; j.part = part;
                 j.splits = wg_splits(cdiv64(H3, htc::WG_BM) * cdiv64(I, htc::WG_BN) * D, kb);
-                const bool own = l == 0 || do_drop;
+                const bool own = own_planes(p, do_drop, l);
                 TRY(wg_gemm(j, gip, true, input_planes(p, stash + (own ? S.XP[l] : S.YP[l - 1]), l, own), true, p.prec, st));
             }
             // the dgh planes are zero at each sequence's first step, so the ±1-row shift needs no mask.  With lengths they are
@@ -586,6 +629,14 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
 // ------------------------------------------------------------------------------------------
 // exported compute entry points
 // ------------------------------------------------------------------------------------------
+// the BiGRU entry points take plans with a head, the bigru_gru_* ones plans without
+static int head_check(const bigru_plan& p, bool head, const char* what) {
+    if (has_head(p) == head) return BIGRU_OK;
+    bigru_set_error(head ? "%s: the plan has no pooling head (bigru_gru_plan_create); use the bigru_gru_* entry points"
+                         : "%s: the plan has a pooling head (bigru_plan_create); use bigru_plan_create's entry points", what);
+    return BIGRU_ERR_ARG;
+}
+
 extern "C" int bigru_forward(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
                              float dropout_p, int spatial, int training, uint64_t seed, void* d_stash,
                              void* d_scratch, float* d_logits, float* d_hn, void* stream) {
@@ -600,6 +651,7 @@ extern "C" int bigru_forward_lengths(const bigru_plan* plan, const float* d_para
         bigru_set_error("forward: null argument");
         return BIGRU_ERR_ARG;
     }
+    TRY(head_check(*plan, true, "forward"));
     if (dropout_p < 0.f || dropout_p >= 1.f) { bigru_set_error("forward: dropout_p must be in [0,1)"); return BIGRU_ERR_ARG; }
     return forward_plan(*plan, d_params, d_x, d_h0, d_lengths, dropout_p, spatial, training, seed,
                         train_bufs(*plan, (float*)d_stash, (float*)d_scratch), d_logits, d_hn, (cudaStream_t)stream);
@@ -623,6 +675,7 @@ extern "C" int bigru_infer_lengths(const bigru_plan* plan, const float* d_params
         bigru_set_error("infer: null argument");
         return BIGRU_ERR_ARG;
     }
+    TRY(head_check(*plan, true, "infer"));
     return forward_plan(*plan, d_params, d_x, d_h0, d_lengths, 0.f, 0, 0, 0, infer_bufs(*plan, (float*)d_workspace), d_logits,
                         nullptr, (cudaStream_t)stream);
 }
@@ -643,8 +696,52 @@ extern "C" int bigru_backward_lengths(const bigru_plan* plan, const float* d_par
         bigru_set_error("backward: null argument");
         return BIGRU_ERR_ARG;
     }
+    TRY(head_check(*plan, true, "backward"));
     return backward_plan(*plan, d_params, d_x, d_h0, d_lengths, dropout_p, spatial, training, seed, (const float*)d_stash,
-                         (float*)d_scratch, d_dlogits, d_grads, d_dx, d_dh0, (cudaStream_t)stream);
+                         (float*)d_scratch, d_dlogits, nullptr, nullptr, nullptr, d_grads, d_dx, d_dh0, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------------------------------
+// nn.GRU: the head-less plan through the same launch sequences (DESIGN.md §4.6)
+// ------------------------------------------------------------------------------------------
+extern "C" int bigru_gru_forward(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
+                                 float dropout_p, int training, uint64_t seed, void* d_stash, void* d_scratch, float* d_y,
+                                 float* d_hn, const int32_t* d_lengths, void* stream) {
+    if (!plan || !d_params || !d_x || !d_stash || !d_scratch || !d_y) {
+        bigru_set_error("gru_forward: null argument");
+        return BIGRU_ERR_ARG;
+    }
+    TRY(head_check(*plan, false, "gru_forward"));
+    if (dropout_p < 0.f || dropout_p >= 1.f) { bigru_set_error("gru_forward: dropout_p must be in [0,1)"); return BIGRU_ERR_ARG; }
+    FwdBufs b = train_bufs(*plan, (float*)d_stash, (float*)d_scratch);
+    b.Y[plan->L - 1] = d_y;
+    return forward_plan(*plan, d_params, d_x, d_h0, d_lengths, dropout_p, 0, training, seed, b, nullptr, d_hn,
+                        (cudaStream_t)stream);
+}
+
+extern "C" int bigru_gru_infer(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
+                               void* d_workspace, float* d_y, float* d_hn, const int32_t* d_lengths, void* stream) {
+    if (!plan || !d_params || !d_x || !d_workspace || !d_y) {
+        bigru_set_error("gru_infer: null argument");
+        return BIGRU_ERR_ARG;
+    }
+    TRY(head_check(*plan, false, "gru_infer"));
+    FwdBufs b = infer_bufs(*plan, (float*)d_workspace);
+    b.Y[plan->L - 1] = d_y;
+    return forward_plan(*plan, d_params, d_x, d_h0, d_lengths, 0.f, 0, 0, 0, b, nullptr, d_hn, (cudaStream_t)stream);
+}
+
+extern "C" int bigru_gru_backward(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
+                                  float dropout_p, int training, uint64_t seed, const void* d_stash, void* d_scratch,
+                                  const float* d_y, const float* d_dy, const float* d_dhn, float* d_grads, float* d_dx,
+                                  float* d_dh0, const int32_t* d_lengths, void* stream) {
+    if (!plan || !d_params || !d_x || !d_stash || !d_scratch || !d_y || !d_dy || !d_grads) {
+        bigru_set_error("gru_backward: null argument");
+        return BIGRU_ERR_ARG;
+    }
+    TRY(head_check(*plan, false, "gru_backward"));
+    return backward_plan(*plan, d_params, d_x, d_h0, d_lengths, dropout_p, 0, training, seed, (const float*)d_stash,
+                         (float*)d_scratch, nullptr, d_y, d_dy, d_dhn, d_grads, d_dx, d_dh0, (cudaStream_t)stream);
 }
 
 extern "C" int bigru_chunk_minmax(const float* d_table, int64_t N, int F, int64_t row_lo, int64_t row_hi, float* d_min,

@@ -69,7 +69,7 @@ int  bigru_plan_create(int B, int T, int F, int H, int L, int C, int bidirection
                        bigru_plan** out);
 int  bigru_plan_destroy(bigru_plan* plan);
 int64_t bigru_param_count(const bigru_plan* plan);
-/* which: 0 w_ih, 1 w_hh, 2 b_ih, 3 b_hh for layer<L; layer==L: 0 lin_w, 2 lin_b */
+/* which: 0 w_ih, 1 w_hh, 2 b_ih, 3 b_hh for layer<L; layer==L: 0 lin_w, 2 lin_b (BIGRU_ERR_ARG on a plan without a head) */
 int  bigru_param_offset(const bigru_plan* plan, int layer, int dir, int which,
                         int64_t* offset, int64_t* rows, int64_t* cols);
 /* stash: activations kept from forward for backward; scratch: reusable temporary space */
@@ -165,6 +165,36 @@ int  bigru_backward(const bigru_plan* plan, const float* d_params, const float* 
                     float dropout_p, int spatial, int training, uint64_t seed,
                     const void* d_stash, void* d_scratch, const float* d_dlogits,
                     float* d_grads, float* d_dx, float* d_dh0, void* stream);
+
+/* --- torch.nn.GRU on the same kernels: a plan without the pooling head (C = 0), for any head or model built on a GRU
+ *  encoder (biGRU_model.py:102 `self.gru(input_seq, hidden)`).  Shapes and precisions follow bigru_plan_create.  Its
+ *  parameter vector is the recurrent prefix of the flat order above (nn.GRU's own parameters, order and count; no lin_w,
+ *  lin_b); bigru_param_offset(layer == L): BIGRU_ERR_ARG.  Workspace sizes come from bigru_workspace_bytes and
+ *  bigru_infer_workspace_bytes of this plan.  The BiGRU entry points (bigru_forward*, bigru_infer*, bigru_backward*,
+ *  bigru_stash_argmax_offset, BIGRU_WS_DCAT) refuse such a plan with BIGRU_ERR_ARG, and the bigru_gru_* entry points refuse a
+ *  plan with a head the same way.  The top layer's output lives in the caller's d_y, not in the stash:
+ *  bigru_stash_output_offset(L-1) and BIGRU_WS_DY of layer L-1 are BIGRU_ERR_ARG.  d_lengths, d_h0 / d_dh0 rules and
+ *  BIGRU_ERR_UNSUPPORTED cases are those of the *_lengths entry points above. */
+int  bigru_gru_plan_create(int B, int T, int F, int H, int L, int bidirectional, int precision, bigru_plan** out);
+/*  Training forward: d_y[B][T][D*H] (required) gets the top layer's output (direction d in columns [d*H, d*H+H), 0 at padded
+ *  steps), d_hn [L*D][B][H] (nullable) the final state of every layer and direction.  training != 0 with dropout_p > 0 drops
+ *  each layer's output except the last's, elementwise, as nn.GRU(dropout=p) does; x is never dropped.  The masks come from
+ *  the generator keyed by (seed, layer) that bigru_forward uses, so for layers above 0 they are BiGRU's inter-layer masks. */
+int  bigru_gru_forward(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
+                       float dropout_p, int training, uint64_t seed, void* d_stash, void* d_scratch, float* d_y,
+                       float* d_hn, const int32_t* d_lengths, void* stream);
+/*  Eval forward on bigru_infer_workspace_bytes(plan) bytes of d_workspace; d_y and d_hn bit-identical to bigru_gru_forward
+ *  with training = 0 (the same launch sequence and kernels, as for bigru_infer). */
+int  bigru_gru_infer(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
+                     void* d_workspace, float* d_y, float* d_hn, const int32_t* d_lengths, void* stream);
+/*  Backward of the last bigru_gru_forward on this plan and stash, with the same arguments and lengths.  d_y: that forward's
+ *  output (read where the top layer's h_{t-1} is needed).  d_dy [B][T][D*H] (required): the gradient of d_y, ignored at
+ *  padded steps.  d_dhn [L*D][B][H] (nullable: zero): the gradient of h_n; layer l's slice seeds that layer's dh carry.
+ *  Outputs: d_grads (the plan's parameter vector, overwritten), d_dx [B][T][F] and d_dh0 [L*D][B][H] (both nullable). */
+int  bigru_gru_backward(const bigru_plan* plan, const float* d_params, const float* d_x, const float* d_h0,
+                        float dropout_p, int training, uint64_t seed, const void* d_stash, void* d_scratch,
+                        const float* d_y, const float* d_dy, const float* d_dhn, float* d_grads, float* d_dx,
+                        float* d_dh0, const int32_t* d_lengths, void* stream);
 
 /* --- losses (biGRU_model.py:202 `self.loss_fn(pred, target)`), fused value + d(loss)/d(logits).
  *  kind CE: d_target int64[B]; BCE/MLSM: d_target float[B,C]; d_weight/d_pos_weight nullable [C]
