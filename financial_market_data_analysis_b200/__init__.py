@@ -9,7 +9,8 @@ sys.path makes ``from biGRU_model import BiGRU`` / ``from sql_pytorch_dataloader
 from . import _lib
 from .biGRU_model import BiGRU
 from .gru import GRU
+from .gru_cell import GRUCell
 from .sql_pytorch_dataloader import (MySQLBatchLoader, MySQLChunkLoader, TrainValTestSplit,
                                      window_indices)
 
-__all__ = ["BiGRU", "GRU", "MySQLBatchLoader", "MySQLChunkLoader", "TrainValTestSplit", "window_indices", "_lib"]
+__all__ = ["BiGRU", "GRU", "GRUCell", "MySQLBatchLoader", "MySQLChunkLoader", "TrainValTestSplit", "window_indices", "_lib"]

@@ -44,6 +44,9 @@ SIGNATURES = {
     "bigru_gru_forward": (_i, [_vp, _vp, _vp, _vp, _f, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_gru_infer": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_gru_backward": (_i, [_vp, _vp, _vp, _vp, _f, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "bigru_cell_workspace_bytes": (_i, [_i, _i, _i, _i, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
+    "bigru_cell_forward": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "bigru_cell_backward": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_loss": (_i, [_i, _vp, _vp, _vp, _vp, _i, _i, _d, _vp, _vp, _vp]),
     "bigru_sqnorm": (_i, [_vp, _i64, _vp, _vp, _vp]),
     "bigru_adam_tick": (_i, [_vp, _vp, _vp]),

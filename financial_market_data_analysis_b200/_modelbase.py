@@ -11,6 +11,11 @@ from . import _lib
 _PRECISIONS = {"fp32": _lib.PREC_FP32, "bf16": _lib.PREC_BF16, "bf16x3": _lib.PREC_BF16X3}
 
 
+def _resolve_precision(precision: str, hidden: int) -> str:
+    """The precision a model of `hidden` units runs at: "auto" is "bf16x3" up to 256 hidden units, "fp32" beyond."""
+    return precision if precision != "auto" else ("bf16x3" if hidden <= 256 else "fp32")
+
+
 def _stream_ptr(device=None):
     """Raw cudaStream_t of torch's current stream ON THE MODEL'S DEVICE (not the process-wide current device)."""
     return torch.cuda.current_stream(device).cuda_stream
@@ -28,7 +33,7 @@ class _Padding:
 
     def __init__(self, dims, precision, device):
         H = dims[0]
-        prec = precision if precision != "auto" else ("bf16x3" if H <= 256 else "fp32")
+        prec = _resolve_precision(precision, H)
         sizes = {"bf16x3": (128, 256), "bf16": (128, 256, 512)}.get(prec, ())
         self.precision = prec
         self.hidden = next((hp for hp in sizes if H <= hp), H)

@@ -4,7 +4,9 @@
 #include "tc_hopper.cuh"
 #include "features.cuh"
 #include "infer_small.cuh"
+#include "cell.cuh"
 
+#include <atomic>
 #include <cstring>
 #include <new>
 
@@ -17,7 +19,7 @@ void bigru_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* bigru_last_error(void) { return g_err; }
-extern "C" int bigru_version(void) { return 209; }
+extern "C" int bigru_version(void) { return 210; }
 
 extern "C" int bigru_device_check(int dev) {
     int n = 0;
@@ -742,6 +744,65 @@ extern "C" int bigru_gru_backward(const bigru_plan* plan, const float* d_params,
     TRY(head_check(*plan, false, "gru_backward"));
     return backward_plan(*plan, d_params, d_x, d_h0, d_lengths, dropout_p, 0, training, seed, (const float*)d_stash,
                          (float*)d_scratch, nullptr, d_y, d_dy, d_dhn, d_grads, d_dx, d_dh0, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------------------------------
+// nn.GRUCell (cell.cuh, DESIGN.md §4.7): no plan; shapes are checked on every call, before the device
+// ------------------------------------------------------------------------------------------
+static int cell_check(int B, int I, int H, int precision, const char* what) {
+    if (B < 1 || I < 1 || H < 1) { bigru_set_error("%s: bad shape B=%d I=%d H=%d", what, B, I, H); return BIGRU_ERR_ARG; }
+    if (precision != BIGRU_PREC_FP32 && precision != BIGRU_PREC_BF16 && precision != BIGRU_PREC_BF16X3) {
+        bigru_set_error("%s: unknown precision %d", what, precision);
+        return BIGRU_ERR_ARG;
+    }
+    if (B > CELL_MAX_B || I > CELL_MAX_DIM || H > CELL_MAX_DIM) {
+        bigru_set_error("%s: B=%d I=%d H=%d beyond the cell's limits (B <= %d, I and H <= %d)", what, B, I, H, CELL_MAX_B, CELL_MAX_DIM);
+        return BIGRU_ERR_UNSUPPORTED;
+    }
+    return BIGRU_OK;
+}
+// the current device is an sm_90 device (asked once per device)
+static int cell_device_check() {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess) {
+        cudaGetLastError();
+        bigru_set_error("no CUDA device (libbigru_b200 has no CPU fallback)");
+        return BIGRU_ERR_DEVICE;
+    }
+    static std::atomic<int> ok[64];
+    if (dev < 64 && ok[dev].load(std::memory_order_relaxed)) return BIGRU_OK;
+    TRY(bigru_device_check(dev));
+    if (dev < 64) ok[dev].store(1, std::memory_order_relaxed);
+    return BIGRU_OK;
+}
+
+extern "C" int bigru_cell_workspace_bytes(int B, int I, int H, int precision, size_t* stash_bytes, size_t* scratch_bytes) {
+    if (!stash_bytes || !scratch_bytes) { bigru_set_error("cell_workspace_bytes: null argument"); return BIGRU_ERR_ARG; }
+    TRY(cell_check(B, I, H, precision, "cell_workspace_bytes"));
+    *stash_bytes = sizeof(float) * (size_t)B * 4 * H;
+    *scratch_bytes = sizeof(float) * (size_t)2 * B * 3 * H;
+    return BIGRU_OK;
+}
+
+extern "C" int bigru_cell_forward(int B, int I, int H, int precision, const float* d_params, const float* d_x, const float* d_h,
+                                  float* d_hout, void* d_stash, void* stream) {
+    if (!d_params || !d_x || !d_hout) { bigru_set_error("cell_forward: null argument"); return BIGRU_ERR_ARG; }
+    TRY(cell_check(B, I, H, precision, "cell_forward"));
+    TRY(cell_device_check());
+    return cell_fwd_launch(B, I, H, precision, d_params, d_x, d_h, d_hout, (float*)d_stash, (cudaStream_t)stream);
+}
+
+extern "C" int bigru_cell_backward(int B, int I, int H, int precision, const float* d_params, const float* d_x, const float* d_h,
+                                   const void* d_stash, const float* d_dhout, float* d_grads, float* d_dx, float* d_dh,
+                                   void* d_scratch, void* stream) {
+    if (!d_params || !d_x || !d_stash || !d_dhout || !d_grads || !d_scratch) {
+        bigru_set_error("cell_backward: null argument");
+        return BIGRU_ERR_ARG;
+    }
+    TRY(cell_check(B, I, H, precision, "cell_backward"));
+    TRY(cell_device_check());
+    return cell_bwd_launch(B, I, H, precision, d_params, d_x, d_h, (const float*)d_stash, d_dhout, d_grads, d_dx, d_dh,
+                           (float*)d_scratch, (cudaStream_t)stream);
 }
 
 extern "C" int bigru_chunk_minmax(const float* d_table, int64_t N, int F, int64_t row_lo, int64_t row_hi, float* d_min,

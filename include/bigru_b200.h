@@ -196,6 +196,25 @@ int  bigru_gru_backward(const bigru_plan* plan, const float* d_params, const flo
                         const float* d_y, const float* d_dy, const float* d_dhn, float* d_grads, float* d_dx,
                         float* d_dh0, const int32_t* d_lengths, void* stream);
 
+/* --- torch.nn.GRUCell: one step h' = GRUCell(x, h), for loops that advance a step at a time (a decoder over a GRU encoder,
+ *  one step per new bar in a live path).  No plan: a cell keeps no per-shape state.  d_params is nn.GRUCell's vector
+ *  w_ih[3H,I] w_hh[3H,H] b_ih[3H] b_hh[3H], the layer-0, direction-0 block of the flat order above (a GRU(I, H, 1)'s vector);
+ *  d_x [B][I], d_h and d_hout [B][H] (d_hout must not overlap an input).  Every precision takes every shape 1 <= B <= 32768,
+ *  1 <= I, H <= 65536 (beyond: BIGRU_ERR_UNSUPPORTED), d_h included at BIGRU_PREC_BF16; ragged edges are handled inside the
+ *  kernels, nothing is padded.  Operands are split into bf16 (hi, and lo at BIGRU_PREC_BF16X3) where the kernels load them; state,
+ *  gate math and outputs are fp32.  A row's bits depend neither on B, nor on the row's position, nor on d_stash.
+ *  Workspaces (bytes, every precision): stash B*4H*4 (G [B][4H] = r, z, n, W_hn h + b_hn), scratch 2*B*3H*4 (dgi, dgh). */
+int  bigru_cell_workspace_bytes(int B, int I, int H, int precision, size_t* stash_bytes, size_t* scratch_bytes);
+/*  One launch.  d_h nullable: the zero state.  d_stash nullable: inference (nothing kept for a backward). */
+int  bigru_cell_forward(int B, int I, int H, int precision, const float* d_params, const float* d_x, const float* d_h,
+                        float* d_hout, void* d_stash, void* stream);
+/*  Backward of a bigru_cell_forward with the same shapes, precision, d_params, d_x and d_h whose stash was kept.  d_dhout [B][H]:
+ *  the gradient of d_hout.  d_grads (parameter vector) is overwritten, each element written once, in a fixed order (bitwise
+ *  reproducible); d_dx [B][I] and d_dh [B][H] nullable.  Three launches, two when both are null. */
+int  bigru_cell_backward(int B, int I, int H, int precision, const float* d_params, const float* d_x, const float* d_h,
+                         const void* d_stash, const float* d_dhout, float* d_grads, float* d_dx, float* d_dh, void* d_scratch,
+                         void* stream);
+
 /* --- losses (biGRU_model.py:202 `self.loss_fn(pred, target)`), fused value + d(loss)/d(logits).
  *  kind CE: d_target int64[B]; BCE/MLSM: d_target float[B,C]; d_weight/d_pos_weight nullable [C]
  *  (BCE only).  Mean reduction over `denom` elements (B for CE, B*C otherwise; pass the GLOBAL
