@@ -1,6 +1,10 @@
-"""What ``BiGRU`` and ``GRU`` share: the zero padding between a model's shapes and its C plans' (``_Padding``), the plans and
-their workspaces (``_Plan``), and the single flat fp32 parameter vector the C ABI reads (``_FlatModel``)."""
+"""What ``BiGRU``, ``GRU`` and ``GRUCell`` share: the zero padding between a model's shapes and its C plans' (``_Padding``),
+the plans and their workspaces (``_Plan``), one C call's padded inputs, plan and dropout seed (``_PaddedCall``), and the
+single flat fp32 parameter vector the C ABI reads (``_FlatModel``)."""
 from __future__ import annotations
+
+import os
+from typing import Optional
 
 import numpy as np
 import torch
@@ -48,7 +52,8 @@ class _Padding:
         return (B + self.tile - 1) // self.tile * self.tile
 
     def pad(self, t, Bp, dim=0, units=False):
-        """t with zero rows appended along `dim` up to Bp and, when `units`, zero hidden units up to the plan's (last dim)."""
+        """t with zero rows appended along `dim` up to Bp and, when `units`, zero hidden units up to the plan's (last dim),
+        contiguous as the C ABI reads it."""
         if t is None:
             return None
         shape = list(t.shape)
@@ -56,7 +61,7 @@ class _Padding:
         if units:
             shape[-1] = self.hidden
         if list(t.shape) == shape:
-            return t
+            return t.contiguous()
         out = t.new_zeros(shape)
         out[tuple(slice(0, n) for n in t.shape)] = t
         return out
@@ -90,7 +95,7 @@ class _Padding:
         H, D = self._dims[0], self._dims[1]
         B, T = dy.shape[0], dy.shape[1]
         if not self.padded:
-            return self.pad(dy, Bp).contiguous()
+            return self.pad(dy, Bp)
         out = dy.new_zeros(Bp, T, D, self.hidden)
         out[:B, :, :, :H] = dy.reshape(B, T, D, H)
         return out.view(Bp, T, D * self.hidden)
@@ -187,12 +192,42 @@ class _Plan:
             pass
 
 
+class _PaddedCall:
+    """What one C call of a plan-running model gets from the real x [B][T][F], h0 [L*D][B][H] and lengths [B] (None: no
+    initial state, every row T steps): the real batch ``B``, the plan's batch ``Bp`` (the model's _Padding rule unless
+    given), ``x``, ``h0`` and ``lengths`` zero-padded to it, and the ``plan`` of Bp rows.
+
+    A training forward passes ``training``, the dropout flag of its C call: it gets the dropout ``seed``, drawn from torch's
+    host generator when the flag is set and 0 otherwise, and recorded as ``model._last_seed``.  Without ``training``
+    (inference) no seed is drawn and ``_last_seed`` is left as it is."""
+
+    def __init__(self, model, x, h0, lengths, training=None, Bp=None):
+        pad = model._pad
+        self.B = x.shape[0]
+        self.Bp = Bp = pad.batch(self.B) if Bp is None else Bp
+        self.x, self.h0 = pad.pad(x, Bp), pad.pad(h0, Bp, dim=1, units=True)
+        self.lengths = pad.lengths(lengths, Bp, x.shape[1])
+        self.plan = model._plan_for(self.x)
+        self.training, self.seed = bool(training), 0
+        if training is not None:
+            if training:                                  # the dropout masks are a pure function of (seed, layer, element)
+                self.seed = int(torch.randint(0, 2 ** 62, (1,)).item())
+            model._last_seed = self.seed
+
+
 class _FlatModel(nn.Module):
     """A module whose parameters are views of one contiguous fp32 vector in the C ABI's order (``_ordered_params``), with
-    the plans that run it.  Subclasses give ``_dims()`` (hidden, directions, layers, features, head outputs), ``precision``,
-    ``_create_plan`` and ``_ordered_params``."""
+    the plans that run it.  Subclasses give ``_dims()`` (hidden, directions, layers, features, head outputs),
+    ``_create_plan`` and ``_ordered_params``, and pass ``precision`` to the constructor."""
 
     _kind = "model"
+
+    def __init__(self, precision: Optional[str]):
+        """``precision``: "fp32", "bf16x3", "bf16" or "auto"; None reads $BIGRU_B200_PRECISION (default "auto")."""
+        super().__init__()
+        self.precision = precision or os.environ.get("BIGRU_B200_PRECISION", "auto")
+        if self.precision != "auto" and self.precision not in _PRECISIONS:
+            raise ValueError(f"precision must be one of {sorted(_PRECISIONS) + ['auto']}")
 
     def _flatten(self):
         """(Re)pack every parameter into one contiguous vector and make the nn.Parameters views of it,
@@ -244,6 +279,16 @@ class _FlatModel(nn.Module):
         """The real parameters' entries of a plan-sized gradient vector."""
         return self._pad.grads(pgrad, out)
 
+    def _grad_views(self, grads):
+        """Each parameter's gradient as a view of a gradient vector in the flat vector's order."""
+        return tuple(grads[o:o + n].view(shape) for (o, n, shape) in self._views)
+
+    def _backward_result(self, pgrad, dx, dh0, B):
+        """What the autograd backward of (model, x, h0, lengths, *params) returns from the plan-sized gradient vector and
+        dx / dh0 of the padded batch: dx and dh0 cropped to the B real rows and units, and views of the real entries."""
+        pad = self._pad
+        return (None, pad.crop(dx, B), pad.crop(dh0, B, dim=1, units=True), None) + self._grad_views(self._plan_grads(pgrad))
+
     def _plan_for(self, x) -> _Plan:
         key = (int(x.shape[0]), int(x.shape[1]), self._pad.precision, x.device.index)
         plan = self._plans.get(key)
@@ -253,13 +298,16 @@ class _FlatModel(nn.Module):
             plan = self._plans[key] = _Plan(self, key[0], key[1], x.device)
         return plan
 
-    def _prepare_input(self, input_seq, hidden):
-        """input_seq [B, T, F] and hidden [L*D, B, H] (or None) as contiguous fp32 tensors on the model's device."""
-        if not self._is_flat():
-            self._flatten()
-        dev = self._flat.device
+    def _cuda_device(self):
+        """The device of the flat parameter vector (re-packed first if needed), which must be a CUDA device."""
+        dev = self.flat_parameters().device
         if dev.type != "cuda":
             raise RuntimeError(f"{self._kind} (H100-native) has no CPU path: move the model to a CUDA device with .cuda() first")
+        return dev
+
+    def _prepare_input(self, input_seq, hidden):
+        """input_seq [B, T, F] and hidden [L*D, B, H] (or None) as contiguous fp32 tensors on the model's device."""
+        dev = self._cuda_device()
         H, D, L, F, _ = self._dims()
         if input_seq.dim() != 3 or input_seq.shape[2] != F:
             raise ValueError(f"input_seq must be [batch, seq_len, {F}], got {tuple(input_seq.shape)}")

@@ -21,7 +21,7 @@ import torch.nn as nn
 
 if __package__:
     from . import _lib
-    from ._modelbase import _PRECISIONS, _FlatModel, _stream_ptr
+    from ._modelbase import _PRECISIONS, _FlatModel, _PaddedCall, _stream_ptr
     from .gru import GRU
     from .parallel import allreduce_flat_
 else:
@@ -34,7 +34,7 @@ else:
         _sys.path.insert(0, os.path.dirname(_here))
     _lib = _importlib.import_module(os.path.basename(_here) + "._lib")
     _base = _importlib.import_module(os.path.basename(_here) + "._modelbase")
-    _PRECISIONS, _FlatModel, _stream_ptr = _base._PRECISIONS, _base._FlatModel, _base._stream_ptr
+    _PRECISIONS, _FlatModel, _PaddedCall, _stream_ptr = _base._PRECISIONS, _base._FlatModel, _base._PaddedCall, _base._stream_ptr
     GRU = _importlib.import_module(os.path.basename(_here) + ".gru").GRU
     allreduce_flat_ = _importlib.import_module(os.path.basename(_here) + ".parallel").allreduce_flat_
 
@@ -68,17 +68,14 @@ class _AdamState:
 
 
 class _StepBuffers:
-    """What one fused train step reads and writes: the plan and a stash of its pool, the padded inputs and per-row lengths
-    (None: every row T steps), the targets of the real rows, the loss arguments, logits / dlogits of the padded batch and the
-    dropout arguments of the C calls."""
+    """What one fused train step reads and writes: its padded call `c` (plan, padded inputs and lengths, dropout seed) and a
+    stash of the plan's pool, the targets of the real rows, the loss arguments and logits / dlogits of the padded batch."""
 
-    def __init__(self, plan, x, h0, tgt, loss, C, drop, lengths=None):
-        Bp = x.shape[0]
-        self.plan, self.stash, self.x, self.h0, self.tgt, self.loss, self.drop = plan, plan.acquire_stash(), x, h0, tgt, loss, drop
-        self.lengths = lengths
-        self.logits = torch.empty(Bp, C, device=x.device, dtype=torch.float32)
+    def __init__(self, c, tgt, loss, C):
+        self.c, self.stash, self.tgt, self.loss = c, c.plan.acquire_stash(), tgt, loss
+        self.logits = torch.empty(c.Bp, C, device=c.x.device, dtype=torch.float32)
         # the loss writes dlogits of the real rows only: the padded rows stay zero
-        self.dlogits = (torch.zeros if Bp != tgt.shape[0] else torch.empty)(Bp, C, device=x.device, dtype=torch.float32)
+        self.dlogits = (torch.zeros if c.Bp != tgt.shape[0] else torch.empty)(c.Bp, C, device=c.x.device, dtype=torch.float32)
 
 
 class _BiGRUFunction(torch.autograd.Function):
@@ -86,58 +83,39 @@ class _BiGRUFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, model, x, h0, lengths, *params):
-        lib = _lib.load()
         pad = model._pad
-        B = x.shape[0]
-        Bp = model._padded_batch(B)
-        x, h0 = pad.pad(x, Bp), pad.pad(h0, Bp, dim=1, units=True)
-        lengths = pad.lengths(lengths, Bp, x.shape[1])
-        plan = model._plan_for(x)
+        c = _PaddedCall(model, x, h0, lengths, training=model.training and model.dropout_p > 0)
         with torch.cuda.device(x.device):                 # the C ABI launches on the CURRENT device: make it the model's
             pflat = model._plan_params()
-            logits = torch.empty(Bp, model.output_size, device=x.device, dtype=torch.float32)
-            hn = torch.empty(model.n_layers * model.n_directions, Bp, pad.hidden, device=x.device, dtype=torch.float32)
-            need_grad = any(ctx.needs_input_grad)        # grad mode is off inside Function.forward; ask the ctx
-            stash = plan.acquire_stash()
-            training = bool(model.training and model.dropout_p > 0)
-            seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if training else 0
-            model._last_seed = seed                       # the dropout masks are a pure function of (seed, element index)
-            _lib.check(lib.bigru_forward_lengths(plan.handle, _lib.ptr(pflat), _lib.ptr(x), _lib.ptr(h0),
-                                                 float(model.dropout_p), int(bool(model.spatial_dropout)), int(training), seed,
-                                                 _lib.ptr(stash), _lib.ptr(plan.scratch), _lib.ptr(logits), _lib.ptr(hn),
-                                                 _lib.ptr(lengths), _stream_ptr(x.device)), "bigru_forward_lengths")
-            model._last_hidden = pad.crop(hn, B, dim=1, units=True)
-            model._last_forward = (plan, stash, B)
-            if need_grad:
-                ctx.model, ctx.pad, ctx.plan, ctx.stash, ctx.seed, ctx.training = model, pad, plan, stash, seed, training
-                ctx.pflat, ctx.real_batch, ctx.has_h0, ctx.lengths = pflat, B, h0 is not None, lengths
-                ctx.save_for_backward(x, h0 if h0 is not None else torch.empty(0, device=x.device))
+            logits = torch.empty(c.Bp, model.output_size, device=x.device, dtype=torch.float32)
+            hn = torch.empty(model.n_layers * model.n_directions, c.Bp, pad.hidden, device=x.device, dtype=torch.float32)
+            stash = c.plan.acquire_stash()
+            model._forward_c(c.plan, pflat, c.x, c.h0, c.lengths, c.training, c.seed, stash, logits, hn, _stream_ptr(x.device))
+            model._last_hidden = pad.crop(hn, c.B, dim=1, units=True)
+            model._last_forward = (c.plan, stash, c.B)
+            if any(ctx.needs_input_grad):                 # grad mode is off inside Function.forward; ask the ctx
+                ctx.model, ctx.plan, ctx.stash, ctx.seed, ctx.training = model, c.plan, stash, c.seed, c.training
+                ctx.pflat, ctx.real_batch, ctx.has_h0, ctx.lengths = pflat, c.B, c.h0 is not None, c.lengths
+                ctx.save_for_backward(c.x, c.h0 if c.h0 is not None else torch.empty(0, device=x.device))
             else:
-                plan.release_stash(stash)
-            return pad.crop(logits, B)
+                c.plan.release_stash(stash)
+            return pad.crop(logits, c.B)
 
     @staticmethod
     def backward(ctx, dlogits):
-        lib = _lib.load()
-        model, pad, plan = ctx.model, ctx.pad, ctx.plan
+        model, plan = ctx.model, ctx.plan
         x, h0 = ctx.saved_tensors
         h0 = h0 if ctx.has_h0 else None
-        B = ctx.real_batch
-        dlogits = pad.pad(dlogits.contiguous().float(), x.shape[0])       # padded rows: zero upstream gradient
+        dlogits = model._pad.pad(dlogits.float(), x.shape[0])             # padded rows: zero upstream gradient
         grads = torch.empty_like(ctx.pflat)
         dx = torch.empty_like(x) if ctx.needs_input_grad[1] else None
         dh0 = torch.empty_like(h0) if (h0 is not None and ctx.needs_input_grad[2]) else None
         with torch.cuda.device(x.device):
-            _lib.check(lib.bigru_backward_lengths(plan.handle, _lib.ptr(ctx.pflat), _lib.ptr(x), _lib.ptr(h0),
-                                                  float(model.dropout_p), int(bool(model.spatial_dropout)), int(ctx.training),
-                                                  ctx.seed, _lib.ptr(ctx.stash), _lib.ptr(plan.scratch), _lib.ptr(dlogits),
-                                                  _lib.ptr(grads), _lib.ptr(dx), _lib.ptr(dh0), _lib.ptr(ctx.lengths),
-                                                  _stream_ptr(x.device)), "bigru_backward_lengths")
+            model._backward_c(plan, ctx.pflat, x, h0, ctx.lengths, ctx.training, ctx.seed, ctx.stash, dlogits, grads, dx, dh0,
+                              _stream_ptr(x.device))
         plan.release_stash(ctx.stash)
         ctx.stash = ctx.pflat = ctx.lengths = None
-        grads = model._plan_grads(grads)                  # drop the padded hidden units' entries
-        pg = tuple(grads[o:o + n].view(shape) for (o, n, shape) in model._views)
-        return (None, pad.crop(dx, B), pad.crop(dh0, B, dim=1, units=True), None) + pg
+        return model._backward_result(grads, dx, dh0, ctx.real_batch)
 
 
 class BiGRU(_FlatModel):
@@ -157,7 +135,7 @@ class BiGRU(_FlatModel):
 
     def __init__(self, hidden_size, n_features, output_size, n_layers=1, clip=50, dropout=0.2,
                  spatial_dropout=True, bidirectional=True, precision: Optional[str] = None):
-        super().__init__()
+        super().__init__(precision)
         self.hidden_size = hidden_size
         self.n_features = n_features
         self.output_size = output_size
@@ -167,9 +145,6 @@ class BiGRU(_FlatModel):
         self.spatial_dropout = spatial_dropout
         self.bidirectional = bidirectional
         self.n_directions = 2 if bidirectional else 1
-        self.precision = precision or os.environ.get("BIGRU_B200_PRECISION", "auto")
-        if self.precision != "auto" and self.precision not in _PRECISIONS:
-            raise ValueError(f"precision must be one of {sorted(_PRECISIONS) + ['auto']}")
 
         # same submodule names and construction order as the reference (:50-60) so that a given
         # torch.manual_seed produces the same initial weights and state_dict keys
@@ -306,18 +281,13 @@ class BiGRU(_FlatModel):
 
     def _infer_slice(self, pflat, x, h0, Bp, lengths=None):
         """Logits of the rows of x (at most Bp) through bigru_infer on the plan of Bp rows; pflat: _plan_params()."""
-        pad, B = self._pad, x.shape[0]
-        x = pad.pad(x, Bp)
-        lengths = pad.lengths(lengths, Bp, x.shape[1])
-        h0 = pad.pad(h0, Bp, dim=1, units=True)
-        h0 = None if h0 is None else h0.contiguous()
-        plan = self._plan_for(x)
+        c = _PaddedCall(self, x, h0, lengths, Bp=Bp)
         with torch.no_grad(), torch.cuda.device(x.device):    # the C ABI launches on the CURRENT device: make it the model's
             logits = torch.empty(Bp, self.output_size, device=x.device, dtype=torch.float32)
-            _lib.check(_lib.load().bigru_infer_lengths(plan.handle, _lib.ptr(pflat), _lib.ptr(x), _lib.ptr(h0),
-                                                       _lib.ptr(plan.infer_workspace()), _lib.ptr(logits), _lib.ptr(lengths),
-                                                       _stream_ptr(x.device)), "bigru_infer_lengths")
-        return pad.crop(logits, B)
+            _lib.check(_lib.load().bigru_infer_lengths(c.plan.handle, _lib.ptr(pflat), _lib.ptr(c.x), _lib.ptr(c.h0),
+                                                       _lib.ptr(c.plan.infer_workspace()), _lib.ptr(logits),
+                                                       _lib.ptr(c.lengths), _stream_ptr(x.device)), "bigru_infer_lengths")
+        return self._pad.crop(logits, c.B)
 
     def add_loss_fn(self, loss_fn):
         self.loss_fn = loss_fn
@@ -437,19 +407,30 @@ class BiGRU(_FlatModel):
         """Forward, loss and backward of one step on stream `s`: the loss into st.loss and the gradient of the real parameters
         into st.grad."""
         lib = _lib.load()
-        plan, kind, wv, pwv, denom = buf.plan, *buf.loss
+        c, (kind, wv, pwv, denom) = buf.c, buf.loss
         pflat = self._plan_params(st.pflat)
         # the loss sees the real batch rows (tgt's); logits / dlogits may carry zero-padded rows behind them
         B, C = buf.tgt.shape[0], buf.logits.shape[1]
-        _lib.check(lib.bigru_forward_lengths(plan.handle, _lib.ptr(pflat), _lib.ptr(buf.x), _lib.ptr(buf.h0), *buf.drop,
-                                             _lib.ptr(buf.stash), _lib.ptr(plan.scratch), _lib.ptr(buf.logits), None,
-                                             _lib.ptr(buf.lengths), s), "bigru_forward_lengths")
+        self._forward_c(c.plan, pflat, c.x, c.h0, c.lengths, c.training, c.seed, buf.stash, buf.logits, None, s)
         _lib.check(lib.bigru_loss(kind, _lib.ptr(buf.logits), _lib.ptr(buf.tgt), _lib.ptr(wv), _lib.ptr(pwv), B, C, denom,
                                   _lib.ptr(st.loss), _lib.ptr(buf.dlogits), s), "bigru_loss")
-        _lib.check(lib.bigru_backward_lengths(plan.handle, _lib.ptr(pflat), _lib.ptr(buf.x), _lib.ptr(buf.h0), *buf.drop,
-                                              _lib.ptr(buf.stash), _lib.ptr(plan.scratch), _lib.ptr(buf.dlogits),
-                                              _lib.ptr(st.pgrad), None, None, _lib.ptr(buf.lengths), s), "bigru_backward_lengths")
+        self._backward_c(c.plan, pflat, c.x, c.h0, c.lengths, c.training, c.seed, buf.stash, buf.dlogits, st.pgrad, None, None, s)
         self._plan_grads(st.pgrad, st.grad)
+
+    def _forward_c(self, plan, pflat, x, h0, lengths, training, seed, stash, logits, hn, s):
+        """bigru_forward_lengths of a padded batch on `plan` and stream `s`, with this model's dropout."""
+        _lib.check(_lib.load().bigru_forward_lengths(plan.handle, _lib.ptr(pflat), _lib.ptr(x), _lib.ptr(h0),
+                                                     float(self.dropout_p), int(bool(self.spatial_dropout)), int(training),
+                                                     seed, _lib.ptr(stash), _lib.ptr(plan.scratch), _lib.ptr(logits),
+                                                     _lib.ptr(hn), _lib.ptr(lengths), s), "bigru_forward_lengths")
+
+    def _backward_c(self, plan, pflat, x, h0, lengths, training, seed, stash, dlogits, grads, dx, dh0, s):
+        """bigru_backward_lengths of the forward `_forward_c` ran with the same arguments."""
+        _lib.check(_lib.load().bigru_backward_lengths(plan.handle, _lib.ptr(pflat), _lib.ptr(x), _lib.ptr(h0),
+                                                      float(self.dropout_p), int(bool(self.spatial_dropout)), int(training),
+                                                      seed, _lib.ptr(stash), _lib.ptr(plan.scratch), _lib.ptr(dlogits),
+                                                      _lib.ptr(grads), _lib.ptr(dx), _lib.ptr(dh0), _lib.ptr(lengths), s),
+                   "bigru_backward_lengths")
 
     def _launch_update(self, g, st, s):
         """clip_grad_norm_(clip) + Adam on the flat buffers on stream `s`; Adam's step counter is incremented on the device."""
@@ -467,7 +448,7 @@ class BiGRU(_FlatModel):
         """CUDA graph(s) of the step on the static buffers `buf` (SURVEY.md 8(f) N5): one graph at world size 1; with data
         parallelism two (compute | update), replayed with the gradient all-reduce between them."""
         lib = _lib.load()
-        dev = buf.x.device
+        dev = buf.c.x.device
         torch.cuda.current_stream(dev).synchronize()
         n0 = lib.bigru_launch_count()
         # an explicit capture stream ON THE MODEL'S DEVICE: torch's default capture stream is created once per process, on whichever
@@ -491,7 +472,7 @@ class BiGRU(_FlatModel):
         launches = int(lib.bigru_launch_count() - n0)
         lib.bigru_launch_count_add(-launches)             # captured, not executed
         if ga is None:
-            buf.plan.release_stash(buf.stash)
+            buf.c.plan.release_stash(buf.stash)
             return
         if len(self._graphs) > 4:
             self._graphs.clear()
@@ -537,23 +518,18 @@ class BiGRU(_FlatModel):
                 ent = self._graphs.get(key)
             if ent is not None:
                 buf, ga, gb, launches = ent
-                buf.x[:B].copy_(x, non_blocking=True)      # rows >= B of the static buffer stay zero
+                buf.c.x[:B].copy_(x, non_blocking=True)    # rows >= B of the static buffer stay zero
                 buf.tgt.copy_(tgt, non_blocking=True)
                 if lens is not None:
-                    buf.lengths[:B].copy_(lens, non_blocking=True)   # rows >= B stay T steps long
+                    buf.c.lengths[:B].copy_(lens, non_blocking=True)   # rows >= B stay T steps long
                 compute, update = ga.replay, (gb.replay if gb is not None else lambda: None)
                 lib.bigru_launch_count_add(launches)
             else:
-                seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if training else 0
-                self._last_seed = seed
-                Bp = self._padded_batch(B)
-                x, h0 = self._pad.pad(x, Bp), self._pad.pad(h0, Bp, dim=1, units=True)
-                lens = self._pad.lengths(lens, Bp, int(x.shape[1]))
+                c = _PaddedCall(self, x, h0, lens, training=training)
                 if graphed:                               # a new graph key: this step runs on the graph's static buffers
-                    x, tgt = x.clone(), tgt.clone()
-                    lens = None if lens is None else lens.clone()
-                buf = _StepBuffers(self._plan_for(x), x, h0, tgt, (kind, wv, pwv, denom), C,
-                                   (float(self.dropout_p), int(bool(self.spatial_dropout)), int(training), seed), lens)
+                    c.x, tgt = c.x.clone(), tgt.clone()
+                    c.lengths = None if c.lengths is None else c.lengths.clone()
+                buf = _StepBuffers(c, tgt, (kind, wv, pwv, denom), C)
                 compute, update = (lambda: self._launch_compute(buf, st, s)), (lambda: self._launch_update(g, st, s))
             compute()
             if self._dp_world > 1:
@@ -561,7 +537,7 @@ class BiGRU(_FlatModel):
             update()
             st.advance()
             if not graphed:
-                buf.plan.release_stash(buf.stash)
+                buf.c.plan.release_stash(buf.stash)
             elif ent is None:
                 self._capture(key, buf, st, g)
             logits = self._pad.crop(buf.logits, B)

@@ -4,7 +4,6 @@ a GRU encoder."""
 from __future__ import annotations
 
 import math
-import os
 from typing import Optional
 
 import torch
@@ -12,7 +11,7 @@ import torch.nn as nn
 from torch.nn.utils.rnn import PackedSequence, pack_padded_sequence, pad_packed_sequence
 
 from . import _lib
-from ._modelbase import _PRECISIONS, _FlatModel, _stream_ptr
+from ._modelbase import _PRECISIONS, _FlatModel, _PaddedCall, _stream_ptr
 
 
 class _TrainForward:
@@ -21,30 +20,23 @@ class _TrainForward:
 
     def __init__(self, mod, x, h0, lengths):
         lib = _lib.load()
+        # the C call gets the module's own p (at one layer it drops nothing), except p = 1 at one layer, which the C ABI
+        # refuses and nn.GRU ignores there; forward refuses p = 1 wherever it would drop
+        self.drop = drop = float(mod.dropout) if mod.dropout < 1 else 0.0
         self.pad = pad = mod._pad
-        self.B = B = x.shape[0]
-        Bp = pad.batch(B)
-        self.x, self.h0 = x, h0 = pad.pad(x, Bp), pad.pad(h0, Bp, dim=1, units=True)
-        self.lengths = lengths = pad.lengths(lengths, Bp, x.shape[1])
-        self.plan = plan = mod._plan_for(x)
-        L, D, Hp = mod.num_layers, mod._dims()[1], pad.hidden
+        self.c = c = _PaddedCall(mod, x, h0, lengths, training=mod.training and drop > 0)
+        plan, D, Hp = c.plan, mod._dims()[1], pad.hidden
         with torch.cuda.device(x.device):                 # the C ABI launches on the CURRENT device: make it the model's
             self.pflat = pflat = mod._plan_params()
-            self.y = y = torch.empty(Bp, x.shape[1], D * Hp, device=x.device, dtype=torch.float32)
-            self.hn = hn = torch.empty(L * D, Bp, Hp, device=x.device, dtype=torch.float32)
+            self.y = y = torch.empty(c.Bp, x.shape[1], D * Hp, device=x.device, dtype=torch.float32)
+            self.hn = hn = torch.empty(mod.num_layers * D, c.Bp, Hp, device=x.device, dtype=torch.float32)
             self.stash = stash = plan.acquire_stash()
-            # the C call gets the module's own p (at one layer it drops nothing), except p = 1 at one layer, which the C ABI
-            # refuses and nn.GRU ignores there; forward refuses p = 1 wherever it would drop
-            self.drop = drop = float(mod.dropout) if mod.dropout < 1 else 0.0
-            self.training = training = bool(mod.training and drop > 0)
-            self.seed = seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if training else 0
-            mod._last_seed = seed                         # the dropout masks are a pure function of (seed, layer, element)
-            _lib.check(lib.bigru_gru_forward(plan.handle, _lib.ptr(pflat), _lib.ptr(x), _lib.ptr(h0), drop,
-                                             int(training), seed, _lib.ptr(stash), _lib.ptr(plan.scratch), _lib.ptr(y),
-                                             _lib.ptr(hn), _lib.ptr(lengths), _stream_ptr(x.device)), "bigru_gru_forward")
+            _lib.check(lib.bigru_gru_forward(plan.handle, _lib.ptr(pflat), _lib.ptr(c.x), _lib.ptr(c.h0), drop,
+                                             int(c.training), c.seed, _lib.ptr(stash), _lib.ptr(plan.scratch), _lib.ptr(y),
+                                             _lib.ptr(hn), _lib.ptr(c.lengths), _stream_ptr(x.device)), "bigru_gru_forward")
 
     def outputs(self):
-        return self.pad.crop_outputs(self.y, self.B), self.pad.crop(self.hn, self.B, dim=1, units=True)
+        return self.pad.crop_outputs(self.y, self.c.B), self.pad.crop(self.hn, self.c.B, dim=1, units=True)
 
 
 class _GRUFunction(torch.autograd.Function):
@@ -53,23 +45,24 @@ class _GRUFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, mod, x, h0, lengths, *params):
         f = _TrainForward(mod, x, h0, lengths)
-        ctx.mod, ctx.pad, ctx.plan, ctx.stash, ctx.seed, ctx.training, ctx.drop = mod, f.pad, f.plan, f.stash, f.seed, f.training, f.drop
-        ctx.pflat, ctx.real_batch, ctx.has_h0, ctx.lengths = f.pflat, f.B, f.h0 is not None, f.lengths
+        c = f.c
+        ctx.mod, ctx.plan, ctx.stash, ctx.seed, ctx.training, ctx.drop = mod, c.plan, f.stash, c.seed, c.training, f.drop
+        ctx.pflat, ctx.real_batch, ctx.has_h0, ctx.lengths = f.pflat, c.B, c.h0 is not None, c.lengths
         # y through save_for_backward, not a ctx attribute: when nothing is padded the output IS y, and an attribute would
         # make output -> grad_fn -> ctx -> output a cycle that keeps the stash alive until the garbage collector runs when no
         # backward follows.  Saving it also checks that nobody modified it in place before the backward reads it.
-        ctx.save_for_backward(f.x, f.h0 if f.h0 is not None else torch.empty(0, device=f.x.device), f.y)
+        ctx.save_for_backward(c.x, c.h0 if c.h0 is not None else torch.empty(0, device=c.x.device), f.y)
         return f.outputs()
 
     @staticmethod
     def backward(ctx, dy, dhn):
         lib = _lib.load()
-        mod, pad, plan = ctx.mod, ctx.pad, ctx.plan
+        mod, plan, pad = ctx.mod, ctx.plan, ctx.mod._pad
         x, h0, y = ctx.saved_tensors
         h0 = h0 if ctx.has_h0 else None
-        B, Bp = ctx.real_batch, x.shape[0]
+        Bp = x.shape[0]
         dy = pad.pad_outputs(dy.float(), Bp) if dy is not None else torch.zeros_like(y)
-        dhn = None if dhn is None else pad.pad(dhn.float(), Bp, dim=1, units=True).contiguous()
+        dhn = None if dhn is None else pad.pad(dhn.float(), Bp, dim=1, units=True)
         grads = torch.empty_like(ctx.pflat)
         dx = torch.empty_like(x) if ctx.needs_input_grad[1] else None
         dh0 = torch.empty_like(h0) if (h0 is not None and ctx.needs_input_grad[2]) else None
@@ -80,9 +73,7 @@ class _GRUFunction(torch.autograd.Function):
                                               _lib.ptr(dh0), _lib.ptr(ctx.lengths), _stream_ptr(x.device)), "bigru_gru_backward")
         plan.release_stash(ctx.stash)
         ctx.stash = ctx.pflat = ctx.lengths = None
-        grads = mod._plan_grads(grads)                    # drop the padded hidden units' entries
-        pg = tuple(grads[o:o + n].view(shape) for (o, n, shape) in mod._views)
-        return (None, pad.crop(dx, B), pad.crop(dh0, B, dim=1, units=True), None) + pg
+        return mod._backward_result(grads, dx, dh0, ctx.real_batch)
 
 
 class GRU(_FlatModel):
@@ -103,7 +94,6 @@ class GRU(_FlatModel):
 
     def __init__(self, input_size, hidden_size, num_layers=1, bias=True, batch_first=False, dropout=0.0,
                  bidirectional=False, device=None, dtype=None, precision: Optional[str] = None, proj_size=0):
-        super().__init__()
         if not bias:
             raise ValueError("GRU: bias=False is not supported (the kernels always add b_ih and b_hh)")
         if proj_size != 0:
@@ -112,12 +102,10 @@ class GRU(_FlatModel):
             raise ValueError(f"GRU: parameters are float32, got dtype={dtype}")
         if not 0 <= float(dropout) <= 1:
             raise ValueError("dropout should be a number in range [0, 1]")
+        super().__init__(precision)
         self.mode, self.input_size, self.hidden_size, self.num_layers = "GRU", input_size, hidden_size, num_layers
         self.bias, self.batch_first, self.dropout, self.bidirectional = True, batch_first, float(dropout), bidirectional
         self.proj_size = 0
-        self.precision = precision or os.environ.get("BIGRU_B200_PRECISION", "auto")
-        if self.precision != "auto" and self.precision not in _PRECISIONS:
-            raise ValueError(f"precision must be one of {sorted(_PRECISIONS) + ['auto']}")
         dirs = 2 if bidirectional else 1
         kw = {"device": device, "dtype": torch.float32}
         for layer in range(num_layers):
@@ -133,7 +121,7 @@ class GRU(_FlatModel):
         self._flatten()
 
     def reset_parameters(self):
-        """nn.GRU's initialisation: U(-1/sqrt(H), 1/sqrt(H)), drawn in registration order."""
+        """nn.GRU's and nn.GRUCell's initialisation: U(-1/sqrt(H), 1/sqrt(H)), drawn in registration order."""
         bound = 1.0 / math.sqrt(self.hidden_size) if self.hidden_size > 0 else 0.0
         with torch.no_grad():
             for p in self.parameters():
@@ -224,7 +212,7 @@ class GRU(_FlatModel):
         elif self._drops():                               # nn.GRU drops in training mode without grad mode too
             with torch.no_grad():
                 f = _TrainForward(self, xs, h0, lens)
-                f.plan.release_stash(f.stash)
+                f.c.plan.release_stash(f.stash)
                 y, hn = f.outputs()
         else:
             y, hn = self._infer(xs, h0, lens)
@@ -240,20 +228,16 @@ class GRU(_FlatModel):
 
     def _infer(self, x, h0, lengths):
         """(y, h_n) of the real rows through bigru_gru_infer, without an autograd record."""
-        pad, B = self._pad, x.shape[0]
-        Bp = pad.batch(B)
-        x, h0 = pad.pad(x, Bp), pad.pad(h0, Bp, dim=1, units=True)
-        lengths = pad.lengths(lengths, Bp, x.shape[1])
-        plan = self._plan_for(x)
+        pad, c = self._pad, _PaddedCall(self, x, h0, lengths)
         D, Hp = self._dims()[1], pad.hidden
         with torch.no_grad(), torch.cuda.device(x.device):
             pflat = self._plan_params()               # held until the call has been queued: padded plans get a fresh vector
-            y = torch.empty(Bp, x.shape[1], D * Hp, device=x.device, dtype=torch.float32)
-            hn = torch.empty(self.num_layers * D, Bp, Hp, device=x.device, dtype=torch.float32)
-            _lib.check(_lib.load().bigru_gru_infer(plan.handle, _lib.ptr(pflat), _lib.ptr(x), _lib.ptr(h0),
-                                                   _lib.ptr(plan.infer_workspace()), _lib.ptr(y), _lib.ptr(hn),
-                                                   _lib.ptr(lengths), _stream_ptr(x.device)), "bigru_gru_infer")
-        return pad.crop_outputs(y, B), pad.crop(hn, B, dim=1, units=True)
+            y = torch.empty(c.Bp, x.shape[1], D * Hp, device=x.device, dtype=torch.float32)
+            hn = torch.empty(self.num_layers * D, c.Bp, Hp, device=x.device, dtype=torch.float32)
+            _lib.check(_lib.load().bigru_gru_infer(c.plan.handle, _lib.ptr(pflat), _lib.ptr(c.x), _lib.ptr(c.h0),
+                                                   _lib.ptr(c.plan.infer_workspace()), _lib.ptr(y), _lib.ptr(hn),
+                                                   _lib.ptr(c.lengths), _stream_ptr(x.device)), "bigru_gru_infer")
+        return pad.crop_outputs(y, c.B), pad.crop(hn, c.B, dim=1, units=True)
 
     @staticmethod
     def _repack(y, lens, like):

@@ -3,8 +3,6 @@ one step at a time, for loops that choose their next input themselves (a decoder
 an attention step, one step per new bar in a live path)."""
 from __future__ import annotations
 
-import math
-import os
 from typing import Optional
 
 import torch
@@ -12,6 +10,7 @@ import torch.nn as nn
 
 from . import _lib
 from ._modelbase import _PRECISIONS, _FlatModel, _resolve_precision, _stream_ptr
+from .gru import GRU
 
 
 class _CellFunction(torch.autograd.Function):
@@ -28,7 +27,7 @@ class _CellFunction(torch.autograd.Function):
             stash = torch.empty(stash_bytes, dtype=torch.uint8, device=x.device)
             _lib.check(lib.bigru_cell_forward(B, I, H, prec, _lib.ptr(flat), _lib.ptr(x), _lib.ptr(h), _lib.ptr(hout),
                                               _lib.ptr(stash), _stream_ptr(x.device)), "bigru_cell_forward")
-        ctx.mod, ctx.prec, ctx.flat, ctx.views, ctx.has_h, ctx.scratch_bytes = mod, prec, flat, mod._views, h is not None, scratch_bytes
+        ctx.mod, ctx.prec, ctx.flat, ctx.has_h, ctx.scratch_bytes = mod, prec, flat, h is not None, scratch_bytes
         # the stash through save_for_backward, not a ctx attribute, as GRU keeps its y: a forward that no backward follows
         # frees it on refcount
         ctx.save_for_backward(x, h if h is not None else torch.empty(0, device=x.device), stash)
@@ -50,8 +49,7 @@ class _CellFunction(torch.autograd.Function):
                                                _lib.ptr(dhout), _lib.ptr(grads), _lib.ptr(dx), _lib.ptr(dh), _lib.ptr(scratch),
                                                _stream_ptr(x.device)), "bigru_cell_backward")
         ctx.flat = None
-        pg = tuple(grads[o:o + n].view(shape) for (o, n, shape) in ctx.views)
-        return (None, dx, dh) + pg
+        return (None, dx, dh) + ctx.mod._grad_views(grads)
 
 
 class GRUCell(_FlatModel):
@@ -69,15 +67,12 @@ class GRUCell(_FlatModel):
     _kind = "GRUCell"
 
     def __init__(self, input_size, hidden_size, bias=True, device=None, dtype=None, precision: Optional[str] = None):
-        super().__init__()
         if not bias:
             raise ValueError("GRUCell: bias=False is not supported (the kernels always add b_ih and b_hh)")
         if dtype is not None and dtype != torch.float32:
             raise ValueError(f"GRUCell: parameters are float32, got dtype={dtype}")
+        super().__init__(precision)
         self.input_size, self.hidden_size, self.bias = input_size, hidden_size, True
-        self.precision = precision or os.environ.get("BIGRU_B200_PRECISION", "auto")
-        if self.precision != "auto" and self.precision not in _PRECISIONS:
-            raise ValueError(f"precision must be one of {sorted(_PRECISIONS) + ['auto']}")
         kw = {"device": device, "dtype": torch.float32}
         self.weight_ih = nn.Parameter(torch.empty(3 * hidden_size, input_size, **kw))
         self.weight_hh = nn.Parameter(torch.empty(3 * hidden_size, hidden_size, **kw))
@@ -86,12 +81,7 @@ class GRUCell(_FlatModel):
         self.reset_parameters()
         self._flatten()
 
-    def reset_parameters(self):
-        """nn.GRUCell's initialisation: U(-1/sqrt(H), 1/sqrt(H)), drawn in registration order."""
-        bound = 1.0 / math.sqrt(self.hidden_size) if self.hidden_size > 0 else 0.0
-        with torch.no_grad():
-            for p in self.parameters():
-                p.uniform_(-bound, bound)
+    reset_parameters = GRU.reset_parameters
 
     def _ordered_params(self):
         return [self.weight_ih, self.weight_hh, self.bias_ih, self.bias_hh]
@@ -129,11 +119,7 @@ class GRUCell(_FlatModel):
         if hx is not None and hx.dim() not in (1, 2):
             raise ValueError(f"GRUCell: Expected hidden to be 1D or 2D, got {hx.dim()}D instead")
         unbatched = input.dim() == 1
-        if not self._is_flat():
-            self._flatten()
-        dev = self._flat.device
-        if dev.type != "cuda":
-            raise RuntimeError("GRUCell (H100-native) has no CPU path: move the model to a CUDA device with .cuda() first")
+        dev = self._cuda_device()
         x = input.unsqueeze(0) if unbatched else input
         if x.shape[1] != self.input_size:
             raise RuntimeError(f"input has inconsistent input_size: got {x.shape[1]} expected {self.input_size}")
