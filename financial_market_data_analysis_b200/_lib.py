@@ -41,6 +41,8 @@ SIGNATURES = {
     "bigru_backward_lengths": (_i, [_vp, _vp, _vp, _vp, _f, _i, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_infer_lengths": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_gru_plan_create": (_i, [_i, _i, _i, _i, _i, _i, _i, C.POINTER(_vp)]),
+    "bigru_plan_create_rd": (_i, [_i, _i, _i, _i, _i, _i, _i, _i, _f, C.POINTER(_vp)]),
+    "bigru_gru_plan_create_rd": (_i, [_i, _i, _i, _i, _i, _i, _i, _f, C.POINTER(_vp)]),
     "bigru_gru_forward": (_i, [_vp, _vp, _vp, _vp, _f, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_gru_infer": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_gru_backward": (_i, [_vp, _vp, _vp, _vp, _f, _i, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -290,13 +290,30 @@ class _FlatModel(nn.Module):
         return (None, pad.crop(dx, B), pad.crop(dh0, B, dim=1, units=True), None) + self._grad_views(self._plan_grads(pgrad))
 
     def _plan_for(self, x) -> _Plan:
-        key = (int(x.shape[0]), int(x.shape[1]), self._pad.precision, x.device.index)
+        # plans are keyed by the recurrent dropout p too: assigning model.recurrent_dropout takes effect at the next call
+        key = (int(x.shape[0]), int(x.shape[1]), self._pad.precision, x.device.index, float(getattr(self, "recurrent_dropout", 0.0)))
         plan = self._plans.get(key)
         if plan is None:
             if len(self._plans) > 8:
                 self._plans.clear()
             plan = self._plans[key] = _Plan(self, key[0], key[1], x.device)
         return plan
+
+    @staticmethod
+    def _check_recurrent_dropout(p) -> float:
+        """The recurrent dropout p as a float in [0, 1) (ValueError otherwise)."""
+        p = float(p)
+        if not 0.0 <= p < 1.0:
+            raise ValueError(f"recurrent_dropout must be in [0, 1), got {p}")
+        return p
+
+    def _create_plan_c(self, lib, creator, args, out):
+        """`creator`(*args, out), or its *_rd twin when the model has recurrent dropout (DESIGN.md §4.8)."""
+        rd = self._check_recurrent_dropout(getattr(self, "recurrent_dropout", 0.0))
+        if rd > 0:
+            _lib.check(getattr(lib, creator + "_rd")(*args, rd, _lib.C.byref(out)), creator + "_rd")
+        else:
+            _lib.check(getattr(lib, creator)(*args, _lib.C.byref(out)), creator)
 
     def _cuda_device(self):
         """The device of the flat parameter vector (re-packed first if needed), which must be a CUDA device."""

@@ -84,7 +84,7 @@ class _BiGRUFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, model, x, h0, lengths, *params):
         pad = model._pad
-        c = _PaddedCall(model, x, h0, lengths, training=model.training and model.dropout_p > 0)
+        c = _PaddedCall(model, x, h0, lengths, training=model._draws_masks())
         with torch.cuda.device(x.device):                 # the C ABI launches on the CURRENT device: make it the model's
             pflat = model._plan_params()
             logits = torch.empty(c.Bp, model.output_size, device=x.device, dtype=torch.float32)
@@ -131,11 +131,19 @@ class BiGRU(_FlatModel):
       "bf16"    single bf16 operands on tensor cores, fp32 accumulation and state (fastest, ~3e-3 on logits); H in {128, 256, 512},
       "auto"    "bf16x3" for hidden sizes up to 256 (smaller models run zero-padded to 128 / 256 hidden units), "fp32" beyond.
     Default: $BIGRU_B200_PRECISION or "auto" (the reference tolerance at tensor-core speed wherever the kernels apply).
+    Extra keyword ``recurrent_dropout`` (p in [0, 1), default 0): variational dropout of the recurrent state (Gal &
+    Ghahramani, 2016; Keras' ``recurrent_dropout``).  In a training-mode forward every layer and direction draws one mask
+    m[b, j] in {0, 1/(1-p)} per batch row and hidden unit, the same at every step, and each valid step runs
+    ``h_t = GRUCell(x_t, m * h_{t-1})``; layer outputs and the final state are unmasked, padded steps are not masked, and
+    eval mode and ``infer`` never mask.  It is not a parameter (state_dict is unchanged); assigning the attribute takes
+    effect at the next call.
     """
 
     def __init__(self, hidden_size, n_features, output_size, n_layers=1, clip=50, dropout=0.2,
-                 spatial_dropout=True, bidirectional=True, precision: Optional[str] = None):
+                 spatial_dropout=True, bidirectional=True, precision: Optional[str] = None, recurrent_dropout: float = 0.0):
+        rd = self._check_recurrent_dropout(recurrent_dropout)
         super().__init__(precision)
+        self.recurrent_dropout = rd
         self.hidden_size = hidden_size
         self.n_features = n_features
         self.output_size = output_size
@@ -189,9 +197,16 @@ class BiGRU(_FlatModel):
         return self.hidden_size, self.n_directions, self.n_layers, self.n_features, self.output_size
 
     def _create_plan(self, lib, B, T, out):
-        _lib.check(lib.bigru_plan_create(B, T, self.n_features, self.plan_hidden(B), self.n_layers, self.output_size,
-                                         int(self.bidirectional), _PRECISIONS[self.resolved_precision(B)], _lib.C.byref(out)),
-                   "bigru_plan_create")
+        self._create_plan_c(lib, "bigru_plan_create", (B, T, self.n_features, self.plan_hidden(B), self.n_layers, self.output_size,
+                                                       int(self.bidirectional), _PRECISIONS[self.resolved_precision(B)]), out)
+
+    def _draws_masks(self) -> bool:
+        """Whether a forward draws dropout noise (and a seed): training mode with input, spatial, inter-layer or recurrent
+        dropout."""
+        return bool(self.training and (self.dropout_p > 0 or self.recurrent_dropout > 0))
+
+    def extra_repr(self):
+        return f"recurrent_dropout={self.recurrent_dropout}" if self.recurrent_dropout else ""
 
     def _flatten(self):
         """(Re)pack every parameter into one contiguous vector (the recurrent prefix of which is also ``self.gru``'s), keeping
@@ -505,7 +520,7 @@ class BiGRU(_FlatModel):
             if tuple(tgt.shape) != (B, C):
                 raise ValueError(f"target must be [{B}, {C}]")
             denom = float(B * C * self._dp_world)
-        training = bool(self.training and self.dropout_p > 0)
+        training = self._draws_masks()
         with torch.cuda.device(dev):
             graphed = self.use_cuda_graph and not training and h0 is None and not torch.cuda.is_current_stream_capturing()
             wv, pwv = self._loss_vec(w, C), self._loss_vec(pw, C)

@@ -19,7 +19,7 @@ void bigru_set_error(const char* fmt, ...) {
 }
 
 extern "C" const char* bigru_last_error(void) { return g_err; }
-extern "C" int bigru_version(void) { return 210; }
+extern "C" int bigru_version(void) { return 211; }
 
 extern "C" int bigru_device_check(int dev) {
     int n = 0;
@@ -45,10 +45,13 @@ extern "C" int bigru_device_check(int dev) {
 // A plan with C = 0 (bigru_gru_plan_create) has no pooling head: it is nn.GRU.  Its top layer's fp32 Y is the caller's d_y, so
 // its stash keeps no top-layer Y, no cat and no arg, and its scratch no dcat; every other region is that of a plan with a head.
 static inline bool has_head(const bigru_plan& p) { return p.C > 0; }
+// A plan with recurrent dropout (rp > 0, DESIGN.md §4.8) adds per layer the masked state R (planes at the tensor-core
+// precisions, fp32 at fp32) after XP, and after arg the masks M [L][D][B][H] and the masked initial state H0M [L*D][B][H].
 struct StashF32 {       // kept forward -> backward
     int64_t Y[16], G[16], X[16];   // per layer: output [B*T*D*H], gates [D][B*T][4H], dropped input [B*T*I_l]
     int64_t YP[16], XP[16];        // per layer: planes of Y [B*T][D*H] and of the layer input [B*T][in_pitch(l)]
-    int64_t cat, arg, total;
+    int64_t R[16];                 // per layer: masked state m * h [B*T][D*H]
+    int64_t cat, arg, M, H0M, total;
 };
 struct ScratchF32 {
     int64_t gi, gh, dgi, dgh, dYa, dYb, dhc, dcat, csum, dgiP, dghP, tcw, part, total;
@@ -69,9 +72,12 @@ static StashF32 stash_layout(const bigru_plan& p) {
         o = rup(o, 64);
         s.YP[l] = o; o += plane_floats(p, BT * p.D * p.H);
         s.XP[l] = o; o += plane_floats(p, BT * in_pitch(p, l));
+        s.R[l] = o; if (p.rp > 0.f) o += p.prec == BIGRU_PREC_FP32 ? BT * p.D * p.H : plane_floats(p, BT * p.D * p.H);
     }
     s.cat = o; if (has_head(p)) o += (int64_t)p.B * 3 * p.H;
     s.arg = o; if (has_head(p)) o += (int64_t)p.B * p.H;
+    s.M = o; if (p.rp > 0.f) o += (int64_t)p.L * p.D * p.B * p.H;
+    s.H0M = o; if (p.rp > 0.f) o += (int64_t)p.L * p.D * p.B * p.H;
     s.total = o;
     return s;
 }
@@ -197,9 +203,10 @@ static inline bool own_planes(const bigru_plan& p, bool do_drop, int l) { return
 static htc::bf16_t* mut(const Planes& q) { return const_cast<htc::bf16_t*>(q.hi); }
 static htc::bf16_t* mut_lo(const Planes& q) { return const_cast<htc::bf16_t*>(q.lo); }
 
-// C = 0: the head-less plan of bigru_gru_plan_create
-static int plan_create(int B, int T, int F, int H, int L, int C, int bidirectional, int precision, bigru_plan** out) {
+// C = 0: the head-less plan of bigru_gru_plan_create.  rp: recurrent dropout p (the *_rd creators)
+static int plan_create(int B, int T, int F, int H, int L, int C, int bidirectional, int precision, float rp, bigru_plan** out) {
     if (!out) { bigru_set_error("plan_create: out is null"); return BIGRU_ERR_ARG; }
+    if (!(rp >= 0.f && rp < 1.f)) { bigru_set_error("plan_create: recurrent_p must be in [0,1) (got %g)", (double)rp); return BIGRU_ERR_ARG; }
     if (B <= 0 || T <= 0 || F <= 0 || H <= 0 || L <= 0 || L > 16 || C < 0) {
         bigru_set_error("plan_create: bad shape B=%d T=%d F=%d H=%d L=%d C=%d", B, T, F, H, L, C);
         return BIGRU_ERR_ARG;
@@ -210,7 +217,7 @@ static int plan_create(int B, int T, int F, int H, int L, int C, int bidirection
     }
     bigru_plan* p = new (std::nothrow) bigru_plan();
     if (!p) { bigru_set_error("plan_create: out of host memory"); return BIGRU_ERR_ARG; }
-    p->B = B; p->T = T; p->F = F; p->H = H; p->L = L; p->C = C; p->D = bidirectional ? 2 : 1; p->prec = precision;
+    p->B = B; p->T = T; p->F = F; p->H = H; p->L = L; p->C = C; p->D = bidirectional ? 2 : 1; p->prec = precision; p->rp = rp;
     p->nparams = p->off_linb() + C;
     if (precision != BIGRU_PREC_FP32) {
         int rc = tc_plan_check(*p);
@@ -224,16 +231,26 @@ static int plan_create(int B, int T, int F, int H, int L, int C, int bidirection
 
 extern "C" int bigru_plan_create(int B, int T, int F, int H, int L, int C, int bidirectional, int precision,
                                  bigru_plan** out) {
+    return bigru_plan_create_rd(B, T, F, H, L, C, bidirectional, precision, 0.f, out);
+}
+
+extern "C" int bigru_plan_create_rd(int B, int T, int F, int H, int L, int C, int bidirectional, int precision, float recurrent_p,
+                                    bigru_plan** out) {
     if (C <= 0) {
         bigru_set_error("plan_create: bad shape B=%d T=%d F=%d H=%d L=%d C=%d (bigru_gru_plan_create makes a plan without a head)",
                         B, T, F, H, L, C);
         return BIGRU_ERR_ARG;
     }
-    return plan_create(B, T, F, H, L, C, bidirectional, precision, out);
+    return plan_create(B, T, F, H, L, C, bidirectional, precision, recurrent_p, out);
 }
 
 extern "C" int bigru_gru_plan_create(int B, int T, int F, int H, int L, int bidirectional, int precision, bigru_plan** out) {
-    return plan_create(B, T, F, H, L, 0, bidirectional, precision, out);
+    return plan_create(B, T, F, H, L, 0, bidirectional, precision, 0.f, out);
+}
+
+extern "C" int bigru_gru_plan_create_rd(int B, int T, int F, int H, int L, int bidirectional, int precision, float recurrent_p,
+                                        bigru_plan** out) {
+    return plan_create(B, T, F, H, L, 0, bidirectional, precision, recurrent_p, out);
 }
 
 extern "C" int bigru_plan_destroy(bigru_plan* plan) { delete plan; return BIGRU_OK; }
@@ -291,8 +308,8 @@ extern "C" int bigru_scan_geometry(const bigru_plan* p, int scan, int* R, int* n
     if (!p || !R || !n_split || (scan != 0 && scan != 1)) { bigru_set_error("scan_geometry: bad argument"); return BIGRU_ERR_ARG; }
     if (p->prec == BIGRU_PREC_FP32) { bigru_set_error("scan_geometry: BIGRU_PREC_FP32 runs no cluster scans"); return BIGRU_ERR_UNSUPPORTED; }
     int geom[2] = {0, 0};
-    if (scan == 0) TRY(tc_scan_fwd(*p, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, geom));
-    else TRY(tc_scan_bwd(*p, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, geom));
+    if (scan == 0) TRY(tc_scan_fwd(*p, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, geom));
+    else TRY(tc_scan_bwd(*p, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, geom));
     *R = geom[0]; *n_split = geom[1];
     return BIGRU_OK;
 }
@@ -306,15 +323,16 @@ extern "C" int bigru_workspace_region(const bigru_plan* p, int which, int layer,
         return BIGRU_ERR_ARG;
     }
     const bool planes = which == BIGRU_WS_Y_PLANES || which == BIGRU_WS_IN_PLANES || which == BIGRU_WS_DGI_PLANES ||
-                        which == BIGRU_WS_DGH_PLANES;
-    const bool stashed = which == BIGRU_WS_GATES || which == BIGRU_WS_Y_PLANES || which == BIGRU_WS_IN_PLANES;
+                        which == BIGRU_WS_DGH_PLANES || (which == BIGRU_WS_RD_STATE && p->prec != BIGRU_PREC_FP32);
+    const bool rd = which == BIGRU_WS_RD_MASK || which == BIGRU_WS_RD_STATE;    // plans with recurrent dropout only
+    const bool stashed = which == BIGRU_WS_GATES || which == BIGRU_WS_Y_PLANES || which == BIGRU_WS_IN_PLANES || rd;
     // stash regions exist for every layer; the scratch keeps layer 0's recurrence gradients, the upstream gradients of layers
     // 0 and 1 and the head's dcat (layer L, as in bigru_param_offset).  A head-less plan has no dcat, and its top layer's
     // upstream gradient is the caller's d_dy
     const bool layer_ok = stashed ? layer >= 0 && layer < p->L
                         : which == BIGRU_WS_DY ? layer >= 0 && layer < p->L && layer < 2 && (has_head(*p) || layer < p->L - 1)
                         : which == BIGRU_WS_DCAT ? layer == p->L && has_head(*p) : layer == 0;
-    if (which < 0 || which >= BIGRU_WS_COUNT || !layer_ok) {
+    if (which < 0 || which >= BIGRU_WS_COUNT || !layer_ok || (rd && !(p->rp > 0.f))) {
         bigru_set_error("workspace_region: bad region %d or layer %d", which, layer);
         return BIGRU_ERR_ARG;
     }
@@ -336,6 +354,8 @@ extern "C" int bigru_workspace_region(const bigru_plan* p, int which, int layer,
         case BIGRU_WS_DGH_PLANES: off = W.dghP; pt = H3; depth_rows = p->D * BT; break;
         case BIGRU_WS_DY:         off = (p->L - 1 - layer) % 2 == 0 ? W.dYa : W.dYb; pt = DH; break;
         case BIGRU_WS_DHC:        off = W.dhc; pt = p->H; break;
+        case BIGRU_WS_RD_MASK:    off = S.M + (int64_t)layer * p->D * p->B * p->H; pt = p->H; break;
+        case BIGRU_WS_RD_STATE:   off = S.R[layer]; pt = DH; depth_rows = BT; break;
         default:                  off = W.dcat; pt = H3; break;
     }
     *in_scratch = stashed ? 0 : 1;
@@ -357,6 +377,7 @@ struct FwdBufs {
     float *gi, *gh, *cat, *arg;
     htc::bf16_t* tcw;
     float *X[16], *Y[16], *G[16], *XP[16], *YP[16];
+    float *R[16], *M, *H0M;        // recurrent dropout (training forward of a plan with rp > 0)
 };
 static FwdBufs train_bufs(const bigru_plan& p, float* stash, float* scratch) {
     const StashF32 S = stash_layout(p);
@@ -366,8 +387,9 @@ static FwdBufs train_bufs(const bigru_plan& p, float* stash, float* scratch) {
     b.tcw = reinterpret_cast<htc::bf16_t*>(scratch + W.tcw);
     for (int l = 0; l < p.L; ++l) {
         b.X[l] = stash + S.X[l]; b.Y[l] = stash + S.Y[l]; b.G[l] = stash + S.G[l];
-        b.XP[l] = stash + S.XP[l]; b.YP[l] = stash + S.YP[l];
+        b.XP[l] = stash + S.XP[l]; b.YP[l] = stash + S.YP[l]; b.R[l] = stash + S.R[l];
     }
+    b.M = stash + S.M; b.H0M = stash + S.H0M;
     return b;
 }
 static FwdBufs infer_bufs(const bigru_plan& p, float* ws) {
@@ -401,6 +423,13 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
     const int B = p.B, T = p.T, H = p.H, D = p.D;
     const int64_t BT = (int64_t)B * T;
     const bool do_drop = training && drop > 0.f;
+    // recurrent dropout (DESIGN.md §4.8): every layer's masks, and the masked initial state, before the first layer
+    const bool rd = training && p.rp > 0.f;
+    const int64_t DBH = (int64_t)D * B * H;
+    if (rd) {
+        KLAUNCH(KC_MISC, 0.0, 0.0, st, rd_mask_kernel<<<132 * 8, 256, 0, st>>>(buf.M, p.L, D, B, H, p.rp, seed));
+        if (h0) KLAUNCH(KC_MISC, 0.0, 0.0, st, mul_kernel<<<132 * 8, 256, 0, st>>>(buf.M, h0, buf.H0M, p.L * DBH));
+    }
     const float* inp = x;
     for (int l = 0; l < p.L; ++l) {
         const int I = (int)p.in_size(l);
@@ -414,6 +443,7 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
         float* G = buf.G[l];
         const float* h0l = h0 ? h0 + (int64_t)l * D * B * H : nullptr;
         float* hnl = hn ? hn + (int64_t)l * D * B * H : nullptr;
+        const float* ml = rd ? buf.M + l * DBH : nullptr;
         if (p.prec != BIGRU_PREC_FP32) {
             const bool own = own_planes(p, do_drop, l);
             const Planes xp = input_planes(p, own ? buf.XP[l] : buf.YP[l - 1], l, own);
@@ -429,12 +459,19 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
                 j.b.zsel = 1;
                 TRY(wg_gemm(j, xp, false, wp, false, p.prec, st));
             }
+            // the scan's planes: Y's, or with recurrent dropout the masked state's (dW_hh reads them)
+            float* sp = rd ? buf.R[l] : buf.YP[l];
             htc::bf16_t *yh = nullptr, *yl = nullptr;
-            if (buf.YP[l]) {
-                const Planes yp = plan_planes(p, buf.YP[l], 0, (int64_t)D * H, BT, 1, (int64_t)D * H);
+            if (sp) {
+                const Planes yp = plan_planes(p, sp, 0, (int64_t)D * H, BT, 1, (int64_t)D * H);
                 yh = mut(yp); yl = mut_lo(yp);
             }
-            TRY(tc_scan_fwd(p, l, buf.gi, params + p.off_whh(l, 0), params + p.off_bhh(l, 0), h0l, Y, G, hnl, yh, yl, len, st));
+            TRY(tc_scan_fwd(p, l, buf.gi, params + p.off_whh(l, 0), params + p.off_bhh(l, 0), h0l, Y, G, hnl, yh, yl, len, ml, st));
+            if (rd && l + 1 < p.L && !own_planes(p, do_drop, l + 1)) {
+                // the next layer's projection and dW_ih read Y's planes, split from the fp32 Y as the scan splits its tile
+                const Planes yp = plan_planes(p, buf.YP[l], 0, (int64_t)D * H, BT, 1, (int64_t)D * H);
+                KLAUNCH(KC_PACK, 0.0, 0.0, st, htc::to_planes_kernel<<<132 * 8, 256, 0, st>>>(Y, BT, D * H, D * H, mut(yp), mut_lo(yp)));
+            }
             inp = Y;
             continue;
         }
@@ -443,13 +480,16 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
         g.bias = params + p.off_bih(l, 0);
         g.batch = D; g.zA = 0; g.zB = p.ld_block(l); g.zBias = p.ld_block(l); g.zC = BT * 3 * H;
         TRY(plan_gemm(p, g, KC_TC_GEMM, buf.tcw, st));
+        // with recurrent dropout the gh GEMM reads the masked state R and the masked initial state
+        const float* Yh = rd ? buf.R[l] : Y;
+        const float* h0h = rd && h0l ? buf.H0M + l * DBH : h0l;
         for (int s = 0; s < T; ++s) {
             // gh[d] = h_prev[d] W_hh[d]^T + b_hh[d];  h_prev rows live in Y (or h0 at s == 0)
             const float* hp; int64_t sam, zA;
-            if (s == 0) { hp = h0l; sam = H; zA = (int64_t)B * H; }
+            if (s == 0) { hp = h0h; sam = H; zA = (int64_t)B * H; }
             else {
                 // direction 0 reads t = s-1, direction 1 reads t = T-s; express via base pointer + batch stride
-                hp = Y + (int64_t)(s - 1) * D * H;
+                hp = Yh + (int64_t)(s - 1) * D * H;
                 sam = (int64_t)T * D * H;
                 zA = D == 2 ? ((int64_t)(T - s) - (s - 1)) * D * H + H : 0;
             }
@@ -463,7 +503,11 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
                 r.mask_period = 1; r.mask_skip = 0;                           // every k masked -> pure bias
                 TRY(sgemm_launch(r, st));
             }
-            KLAUNCH(KC_GATES_FWD, 0.0, 0.0, st, gru_gates_fwd_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(buf.gi, buf.gh, h0l, Y, G,
+            if (rd)
+                KLAUNCH(KC_GATES_FWD, 0.0, 0.0, st, gru_gates_fwd_rd_kernel<<<nblk(DBH, 256), 256, 0, st>>>(buf.gi, buf.gh, h0l, Y, G, hnl, B, T, H,
+                                                                                               D, s, len, ml, buf.R[l]));
+            else
+                KLAUNCH(KC_GATES_FWD, 0.0, 0.0, st, gru_gates_fwd_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(buf.gi, buf.gh, h0l, Y, G,
                                                                               hnl, B, T, H, D, s, len));
         }
         inp = Y;
@@ -498,6 +542,7 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
     const int B = p.B, T = p.T, H = p.H, D = p.D, C = p.C;
     const int64_t BT = (int64_t)B * T, H3 = 3LL * H;
     const bool do_drop = training && drop > 0.f;
+    const bool rd = training && p.rp > 0.f;                  // recurrent dropout: the forward's masks are in the stash
     const bool tc = p.prec != BIGRU_PREC_FP32;
     float* dhc = scratch + W.dhc;
     htc::bf16_t* tcw = reinterpret_cast<htc::bf16_t*>(scratch + W.tcw);
@@ -522,6 +567,7 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
         const float* Y = caller_top ? y : stash + S.Y[l];
         const float* G = stash + S.G[l];
         const float* h0l = h0 ? h0 + (int64_t)l * D * B * H : nullptr;
+        const float* ml = rd ? stash + S.M + (int64_t)l * D * B * H : nullptr;
         float* dgi = scratch + W.dgi;
         float* dgh = scratch + W.dgh;
         if (!head && dhn) CUDA_TRY(cudaMemcpyAsync(dhc, dhn + (int64_t)l * D * B * H, sizeof(float) * D * B * H,
@@ -531,10 +577,13 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
         const Planes ghp = plan_planes(p, scratch, W.dghP, H3, BT, D, H3);
         // recurrence: dgi, dgh [D][B*T][3H] and dh0 in dhc
         if (tc) {
-            TRY(tc_scan_bwd(p, l, G, Y, h0l, dY, dhc, dgi, dgh, params + p.off_whh(l, 0), mut(gip), mut_lo(gip), mut(ghp), mut_lo(ghp), len, st));
+            TRY(tc_scan_bwd(p, l, G, Y, h0l, dY, dhc, dgi, dgh, params + p.off_whh(l, 0), mut(gip), mut_lo(gip), mut(ghp), mut_lo(ghp), len, ml, st));
         } else {
             for (int s = 0; s < T; ++s) {
-                KLAUNCH(KC_GATES_BWD, 0.0, 0.0, st, gru_gates_bwd_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(G, Y, h0l, dY, dhc, dgi, dgh, B, T, H, D, s, len));
+                if (rd)
+                    KLAUNCH(KC_GATES_BWD, 0.0, 0.0, st, gru_gates_bwd_rd_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(G, Y, h0l, dY, dhc, dgi, dgh, B, T, H, D, s, len, ml));
+                else
+                    KLAUNCH(KC_GATES_BWD, 0.0, 0.0, st, gru_gates_bwd_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(G, Y, h0l, dY, dhc, dgi, dgh, B, T, H, D, s, len));
                 // dhc[d] += dgh_t[d] W_hh[d]   (rows t: dir0 -> T-1-s, dir1 -> s)
                 const int t0 = T - 1 - s, t1 = s;
                 GemmArgs r = gemm_args(dgh + (int64_t)t0 * 3 * H, params + p.off_whh(l, 0), dhc, B, H, 3 * H,
@@ -544,8 +593,11 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
                 TRY(sgemm_launch(r, st));
             }
         }
-        if (dh0) CUDA_TRY(cudaMemcpyAsync(dh0 + (int64_t)l * D * B * H, dhc, sizeof(float) * D * B * H,
-                                          cudaMemcpyDeviceToDevice, st));
+        // the fp32 carry leaves the first step as the gradient of m * h0 (the scans mask it themselves)
+        if (dh0 && rd && !tc)
+            KLAUNCH(KC_MISC, 0.0, 0.0, st, mul_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(ml, dhc, dh0 + (int64_t)l * D * B * H, (int64_t)D * B * H));
+        else if (dh0) CUDA_TRY(cudaMemcpyAsync(dh0 + (int64_t)l * D * B * H, dhc, sizeof(float) * D * B * H,
+                                               cudaMemcpyDeviceToDevice, st));
         // dW_ih[d] = dgi[d]^T X and dW_hh[d] = dgh[d]^T H_prev, H_prev(b,t) = Y[b,t-1] (dir 0) / Y[b,t+1] (dir 1), the columns
         // of direction d.  The first step's h_prev is h0: its term is the w0 GEMM below.
         if (tc) {
@@ -567,7 +619,7 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
                 j.zC = p.ld_block(l); j.a.zsel = 1; j.part = part;
                 j.b.coff = H; j.b.kshift[0] = -1; j.b.kshift[1] = 1;
                 j.splits = wg_splits(cdiv64(H3, htc::WG_BM) * cdiv64(H, htc::WG_BN) * D, kb);
-                TRY(wg_gemm(j, ghp, true, plan_planes(p, stash, S.YP[l], (int64_t)D * H, BT, 1, (int64_t)D * H), true, p.prec, st));
+                TRY(wg_gemm(j, ghp, true, plan_planes(p, stash, rd ? S.R[l] : S.YP[l], (int64_t)D * H, BT, 1, (int64_t)D * H), true, p.prec, st));
             }
         } else {
             // the layer input as the projection saw it (the dropped copy when dropout was applied)
@@ -580,7 +632,7 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
                 wi.splitk = splitk;
                 TRY(sgemm_launch(wi, st));
                 if (T > 1) {
-                    const float* hp = Y + (int64_t)d * H + (d == 0 ? -(int64_t)D * H : (int64_t)D * H);
+                    const float* hp = (rd ? stash + S.R[l] : Y) + (int64_t)d * H + (d == 0 ? -(int64_t)D * H : (int64_t)D * H);
                     GemmArgs wh = gemm_args(dgh_d, hp, grads + p.off_whh(l, d), 3 * H, H, (int)BT, 1, 3 * H, 1,
                                             (int64_t)D * H, H);
                     wh.splitk = splitk; wh.mask_period = T; wh.mask_skip = d == 0 ? 0 : T - 1;
@@ -594,7 +646,8 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
             const float* dgh_d = dgh + (int64_t)d * BT * 3 * H;
             if (h0l) {
                 const int tf = d == 0 ? 0 : T - 1;
-                GemmArgs w0 = gemm_args(dgh_d + (int64_t)tf * 3 * H, h0l + (int64_t)d * B * H, grads + p.off_whh(l, d),
+                const float* h0w = rd ? stash + S.H0M + (int64_t)l * D * B * H : h0l;       // the masked h0 the first step read
+                GemmArgs w0 = gemm_args(dgh_d + (int64_t)tf * 3 * H, h0w + (int64_t)d * B * H, grads + p.off_whh(l, d),
                                         3 * H, H, B, 1, (int64_t)T * 3 * H, 1, H, H);
                 w0.beta = 1;
                 TRY(plan_gemm(p, w0, KC_TC_GEMM_DWHH, tcw, st));

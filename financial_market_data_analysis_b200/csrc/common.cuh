@@ -29,6 +29,7 @@ static inline int64_t cdiv64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 // Shapes, flat-parameter offsets and workspace carve-up.  All sizes in elements unless noted.
 struct bigru_plan {
     int B, T, F, H, L, C, D, prec;
+    float rp;                      // recurrent dropout p (bigru_plan_create_rd); 0: none
     int64_t nparams;
     int64_t layer_dir_stride[8];   // unused for L>8; offsets are computed on demand
     size_t stash_bytes, scratch_bytes;

@@ -176,10 +176,13 @@ static int colsum_launch(const float* A, float* out, int64_t rows, int cols, int
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.f / (1.f + expf(-x)); }
 
-__global__ void gru_gates_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ gh,
-                                     const float* __restrict__ h0, float* __restrict__ Y, float* __restrict__ G,
-                                     float* __restrict__ hn_out, int B, int T, int H, int D, int s,
-                                     const int* __restrict__ len) {
+// RD: recurrent dropout (DESIGN.md §4.8) with the layer's masks M [D][B][H]: the carry is z * (m * h_prev), and R
+// [B][T][D*H] gets the masked state m * h (0 at padded steps), which the next step's gh GEMM and dW_hh read instead of Y
+template <bool RD>
+__device__ __forceinline__ void gru_gates_fwd(const float* __restrict__ gi, const float* __restrict__ gh,
+                                              const float* __restrict__ h0, float* __restrict__ Y, float* __restrict__ G,
+                                              float* __restrict__ hn_out, int B, int T, int H, int D, int s,
+                                              const int* __restrict__ len, const float* __restrict__ M, float* __restrict__ R) {
     const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t total = (int64_t)D * B * H;
     if (idx >= total) return;
@@ -197,13 +200,16 @@ __global__ void gru_gates_fwd_kernel(const float* __restrict__ gi, const float* 
     const float z = sigmoid_f(gir[H + j] + ghr[H + j]);
     const float hn = ghr[2 * H + j];
     const float n = tanhf(gir[2 * H + j] + r * hn);
-    const float h = (1.f - z) * n + z * hp;
+    const float m = RD ? M[((int64_t)d * B + b) * H + j] : 1.f;
+    const float h = (1.f - z) * n + z * (RD ? m * hp : hp);
     const int n_b = len ? len[b] : T;
     if (t >= n_b) {
         Y[row * D * H + d * H + j] = 0.f;
+        if (RD) R[row * D * H + d * H + j] = 0.f;
         return;
     }
     Y[row * D * H + d * H + j] = h;
+    if (RD) R[row * D * H + d * H + j] = m * h;
     if (G) {
         float* g = G + ((int64_t)d * B * T + row) * 4 * H;
         g[j] = r; g[H + j] = z; g[2 * H + j] = n; g[3 * H + j] = hn;
@@ -211,12 +217,29 @@ __global__ void gru_gates_fwd_kernel(const float* __restrict__ gi, const float* 
     if (hn_out && (d == 0 ? t == n_b - 1 : s == T - 1)) hn_out[((int64_t)d * B + b) * H + j] = h;
 }
 
+__global__ void gru_gates_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ gh,
+                                     const float* __restrict__ h0, float* __restrict__ Y, float* __restrict__ G,
+                                     float* __restrict__ hn_out, int B, int T, int H, int D, int s,
+                                     const int* __restrict__ len) {
+    gru_gates_fwd<false>(gi, gh, h0, Y, G, hn_out, B, T, H, D, s, len, nullptr, nullptr);
+}
+__global__ void gru_gates_fwd_rd_kernel(const float* __restrict__ gi, const float* __restrict__ gh,
+                                        const float* __restrict__ h0, float* __restrict__ Y, float* __restrict__ G,
+                                        float* __restrict__ hn_out, int B, int T, int H, int D, int s,
+                                        const int* __restrict__ len, const float* __restrict__ M, float* __restrict__ R) {
+    gru_gates_fwd<true>(gi, gh, h0, Y, G, hn_out, B, T, H, D, s, len, M, R);
+}
+
 // backward gates for one step: consumes dh carry + dY_t, emits dgi/dgh rows and dh*z.  At a padded (row, t >= len[b]):
-// dgi = dgh = 0 and the carry passes through unchanged
-__global__ void gru_gates_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y,
-                                     const float* __restrict__ h0, const float* __restrict__ dY,
-                                     float* __restrict__ dhc, float* __restrict__ dgi, float* __restrict__ dgh,
-                                     int B, int T, int H, int D, int s, const int* __restrict__ len) {
+// dgi = dgh = 0 and the carry passes through unchanged.  RD: the masks M of gru_gates_fwd<true>.  The carry then arrives
+// as the gradient of the previous step's masked state, m * h (dh z + dgh W_hh), and becomes dh_{t-1} = m * carry here when
+// that step was valid; h_prev in the gate math is m * h_prev
+template <bool RD>
+__device__ __forceinline__ void gru_gates_bwd(const float* __restrict__ G, const float* __restrict__ Y,
+                                              const float* __restrict__ h0, const float* __restrict__ dY,
+                                              float* __restrict__ dhc, float* __restrict__ dgi, float* __restrict__ dgh,
+                                              int B, int T, int H, int D, int s, const int* __restrict__ len,
+                                              const float* __restrict__ M) {
     const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t total = (int64_t)D * B * H;
     if (idx >= total) return;
@@ -225,11 +248,14 @@ __global__ void gru_gates_bwd_kernel(const float* __restrict__ G, const float* _
     const int d = idx / ((int64_t)H * B);
     const int t = d == 0 ? T - 1 - s : s;
     const int64_t row = (int64_t)b * T + t;
+    // RD: whether the previous step (t + 1 forward, t - 1 reverse) applied a cell, so that the carry is masked here
+    const bool prev_cell = RD && s > 0 && !(len && (d == 0 ? t + 1 : t - 1) >= len[b]);
     if (len && t >= len[b]) {
         float* a = dgi + ((int64_t)d * B * T + row) * 3 * H;
         float* c = dgh + ((int64_t)d * B * T + row) * 3 * H;
         a[j] = a[H + j] = a[2 * H + j] = 0.f;
         c[j] = c[H + j] = c[2 * H + j] = 0.f;
+        if (prev_cell) { const int64_t ci = ((int64_t)d * B + b) * H + j; dhc[ci] *= M[ci]; }
         return;
     }
     const float* g = G + ((int64_t)d * B * T + row) * 4 * H;
@@ -239,7 +265,12 @@ __global__ void gru_gates_bwd_kernel(const float* __restrict__ G, const float* _
     if (first) hp = h0 ? h0[((int64_t)d * B + b) * H + j] : 0.f;
     else hp = Y[((int64_t)b * T + (d == 0 ? t - 1 : t + 1)) * D * H + d * H + j];
     const int64_t ci = ((int64_t)d * B + b) * H + j;
-    const float dh = dhc[ci] + dY[row * D * H + d * H + j];
+    float carry = dhc[ci];
+    if (RD) {
+        hp *= M[ci];
+        if (prev_cell) carry *= M[ci];
+    }
+    const float dh = carry + dY[row * D * H + d * H + j];
     const float dan = dh * (1.f - z) * (1.f - n * n);
     const float dar = dan * hn * r * (1.f - r);
     const float daz = dh * (hp - n) * z * (1.f - z);
@@ -248,6 +279,20 @@ __global__ void gru_gates_bwd_kernel(const float* __restrict__ G, const float* _
     a[j] = dar; a[H + j] = daz; a[2 * H + j] = dan;
     c[j] = dar; c[H + j] = daz; c[2 * H + j] = dan * r;
     dhc[ci] = dh * z;
+}
+
+__global__ void gru_gates_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y,
+                                     const float* __restrict__ h0, const float* __restrict__ dY,
+                                     float* __restrict__ dhc, float* __restrict__ dgi, float* __restrict__ dgh,
+                                     int B, int T, int H, int D, int s, const int* __restrict__ len) {
+    gru_gates_bwd<false>(G, Y, h0, dY, dhc, dgi, dgh, B, T, H, D, s, len, nullptr);
+}
+__global__ void gru_gates_bwd_rd_kernel(const float* __restrict__ G, const float* __restrict__ Y,
+                                        const float* __restrict__ h0, const float* __restrict__ dY,
+                                        float* __restrict__ dhc, float* __restrict__ dgi, float* __restrict__ dgh,
+                                        int B, int T, int H, int D, int s, const int* __restrict__ len,
+                                        const float* __restrict__ M) {
+    gru_gates_bwd<true>(G, Y, h0, dY, dhc, dgi, dgh, B, T, H, D, s, len, M);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -458,6 +503,23 @@ __global__ void dropout_kernel(const float* __restrict__ in, float* __restrict__
         const float u = bigru_uniform(seed, stream, key);
         out[i] = u < p ? 0.f : in[i] * scale;
     }
+}
+
+// Recurrent dropout masks (DESIGN.md §4.8) of every layer, M [L][D][B][H]: 0 where u < p, else 1/(1-p), with u drawn from
+// stream BIGRU_RD_STREAM + l at the batch-major key (b*D + d)*H + j, so a row's masks do not depend on the batch size
+__global__ void rd_mask_kernel(float* __restrict__ M, int L, int D, int B, int H, float p, uint64_t seed) {
+    const float scale = 1.f / (1.f - p);
+    const int64_t n = (int64_t)L * D * B * H;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int j = i % H, b = (i / H) % B, d = (i / ((int64_t)H * B)) % D, l = i / ((int64_t)H * B * D);
+        const float u = bigru_uniform(seed, BIGRU_RD_STREAM + (uint32_t)l, ((uint64_t)b * D + d) * H + j);
+        M[i] = u < p ? 0.f : scale;
+    }
+}
+
+// out = a * b elementwise (masked initial states and their gradients)
+__global__ void mul_kernel(const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ out, int64_t n) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) out[i] = a[i] * b[i];
 }
 
 // ------------------------------------------------------------------------------------------

@@ -418,13 +418,16 @@ __device__ __forceinline__ void mbar_arrive_peer(uint64_t* bar, uint32_t cta) {
     asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(mapa(smem_u32(bar), cta)) : "memory");
 }
 
-// the scan of one cluster whose tile has JN * 16 rows from bt0, direction d
-template <int H, int NS, int OUT, bool LEN, int JN>
+// the scan of one cluster whose tile has JN * 16 rows from bt0, direction d.  RD: recurrent dropout with the layer's masks
+// `mask` [D][B][H] (DESIGN.md §4.8): the h tile holds m * h (staged from m * h0), the carry is z * (m * h_{t-1}), and the own
+// block's copy (yh, yl) is the masked state; Y, hn and the carried hp stay unmasked
+template <int H, int NS, int OUT, bool LEN, int JN, bool RD = false>
 __device__ __forceinline__ void gru_scan_fwd_tile(const float* __restrict__ gi, const float* __restrict__ Whh,
                                                   const float* __restrict__ bhh, int64_t zW, const float* __restrict__ h0,
                                                   float* __restrict__ Y, float* __restrict__ G, float* __restrict__ hn_out,
                                                   bf16_t* __restrict__ yh, bf16_t* __restrict__ yl, int B, int T, int D,
-                                                  const int* __restrict__ lens, int d, int bt0) {
+                                                  const int* __restrict__ lens, int d, int bt0,
+                                                  const float* __restrict__ mask = nullptr) {
     using S = FwdSmem<H, NS>;
     constexpr int U = SCAN_U, CS = H / U, NH = S::NH, JMAX = JN, jn = JN, nb = JN * SCAN_NB;   // jn n8 blocks per warp
     // the h region holds two 16-row buffers or one 32-row buffer: a 16-row tile is double-buffered, a 32-row tile is not
@@ -451,7 +454,8 @@ __device__ __forceinline__ void gru_scan_fwd_tile(const float* __restrict__ gi, 
     }
     for (int i = tid; i < nb * H; i += SCAN_THREADS) {
         const int b = i / H, k = i % H;
-        const float v = h0 ? h0[((int64_t)d * B + bt0 + b) * H + k] : 0.f;
+        float v = h0 ? h0[((int64_t)d * B + bt0 + b) * H + k] : 0.f;
+        if constexpr (RD) v *= mask[((int64_t)d * B + bt0 + b) * H + k];
         bf16_t hi, lo;
         split_bf16(v, hi, lo);
         *reinterpret_cast<bf16_t*>(Hsm + hsw<NBMAX>(b, k)) = hi;
@@ -470,7 +474,7 @@ __device__ __forceinline__ void gru_scan_fwd_tile(const float* __restrict__ gi, 
     for (int j = 0; j < JMAX; ++j) {
         bcol[j][0] = (nt * jn + j) * 8 + 2 * (lane & 3); bcol[j][1] = bcol[j][0] + 1;
     }
-    float bias[3][2], hp[JMAX][4];
+    float bias[3][2], hp[JMAX][4], mk[RD ? JMAX : 1][4];
 #pragma unroll
     for (int gte = 0; gte < 3; ++gte)
 #pragma unroll
@@ -484,6 +488,7 @@ __device__ __forceinline__ void gru_scan_fwd_tile(const float* __restrict__ gi, 
         for (int e = 0; e < 4; ++e) {
             const int b = bt0 + bcol[j][e & 1], k = c * U + unit[e >> 1];
             hp[j][e] = h0 ? h0[((int64_t)d * B + b) * H + k] : 0.f;
+            if constexpr (RD) mk[j][e] = mask[((int64_t)d * B + b) * H + k];
         }
         len[j][0] = len[j][1] = T;
         if (LEN) { len[j][0] = lens[bt0 + bcol[j][0]]; len[j][1] = lens[bt0 + bcol[j][1]]; }
@@ -576,9 +581,12 @@ __device__ __forceinline__ void gru_scan_fwd_tile(const float* __restrict__ gi, 
                 const float hnv = acc[2][j][e] + bias[2][e >> 1];
                 const float n = tanhf(giv[2][j][e] + r * hnv);
                 const bool pad = LEN && t >= len[j][e & 1];
-                const float h = pad ? hp[j][e] : (1.f - z) * n + z * hp[j][e];
+                float h;
+                if constexpr (RD) h = pad ? hp[j][e] : (1.f - z) * n + z * (mk[j][e] * hp[j][e]);
+                else h = pad ? hp[j][e] : (1.f - z) * n + z * hp[j][e];
                 hp[j][e] = h;
-                hv[j][e] = h;
+                if constexpr (RD) hv[j][e] = mk[j][e] * h;
+                else hv[j][e] = h;
                 const int64_t row = (int64_t)b * T + t;
                 if (OUT & SCAN_Y) Y[row * DH + d * H + k] = pad ? 0.f : h;
                 if ((OUT & SCAN_G) && !pad) {
@@ -643,6 +651,24 @@ gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh,
     gru_scan_fwd_tile<H, NS, OUT, LEN, 1>(gi, Whh, bhh, zW, h0, Y, G, hn_out, yh, yl, B, T, D, lens, d, bt0);
 }
 
+// the training forward with recurrent dropout (SCAN_TRAIN outputs): yh, yl receive the masked state, not Y
+template <int H, int NS, bool LEN>
+__global__ void __launch_bounds__(SCAN_THREADS, 1)
+gru_scan_fwd_rd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh, const float* __restrict__ bhh, int64_t zW,
+                       const float* __restrict__ h0, float* __restrict__ Y, float* __restrict__ G, float* __restrict__ hn_out,
+                       bf16_t* __restrict__ yh, bf16_t* __restrict__ yl, int B, int T, int D, int m2, const int* __restrict__ lens,
+                       const float* __restrict__ mask) {
+    int d, bt0, nb;
+    scan_tile(blockIdx.y, m2, B / SCAN_NB, D, d, bt0, nb);
+    if constexpr (FwdSmem<H, NS>::NBMAX == 2 * SCAN_NB) {
+        if (nb == 2 * SCAN_NB) {
+            gru_scan_fwd_tile<H, NS, SCAN_TRAIN, LEN, 2, true>(gi, Whh, bhh, zW, h0, Y, G, hn_out, yh, yl, B, T, D, lens, d, bt0, mask);
+            return;
+        }
+    }
+    gru_scan_fwd_tile<H, NS, SCAN_TRAIN, LEN, 1, true>(gi, Whh, bhh, zW, h0, Y, G, hn_out, yh, yl, B, T, D, lens, d, bt0, mask);
+}
+
 // ------------------------------------------------------------------------------------------------------
 // Backward recurrence of one layer, both directions.  Layouts are those of gru_gates_bwd_kernel: G, Y, h0 as in the
 // forward; dY [B][T][D*H]; dhc [D][B][H] carries dh into the layer's last step (head / zero) and returns dh_{-1};
@@ -677,14 +703,17 @@ __device__ __forceinline__ int xslot(int kl, int b) {
     return kl * SCAN_NB + (((b >> 1) ^ g) << 1) + (b & 1);
 }
 
-// the scan of one cluster whose tile has NR (16 or 8) rows from bt0, direction d; the shared-memory layout is that of 16
-template <int H, int NS, bool LEN, int NR>
+// the scan of one cluster whose tile has NR (16 or 8) rows from bt0, direction d; the shared-memory layout is that of 16.
+// RD: recurrent dropout with the forward's masks `mask` [D][B][H] (DESIGN.md §4.8): the gate math reads m * h_{t-1}, and the
+// gradient leaving a valid step is dh_{t-1} = m * (dh z + sum of the partials); a padded step passes it unmasked
+template <int H, int NS, bool LEN, int NR, bool RD = false>
 __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, const float* __restrict__ Y,
                                                   const float* __restrict__ h0, const float* __restrict__ dY,
                                                   float* __restrict__ dhc, float* __restrict__ dgi, float* __restrict__ dgh,
                                                   const float* __restrict__ Whh, int64_t zW, bf16_t* __restrict__ gih,
                                                   bf16_t* __restrict__ gil, bf16_t* __restrict__ ghh, bf16_t* __restrict__ ghl,
-                                                  int B, int T, int D, const int* __restrict__ lens, int d, int bt0) {
+                                                  int B, int T, int D, const int* __restrict__ lens, int d, int bt0,
+                                                  const float* __restrict__ mask = nullptr) {
     using S = BwdSmem<H, NS>;
     constexpr int U = SCAN_U, CS = H / U, NH = S::NH, Q = S::Q, NB = SCAN_NB;
     constexpr int MT = H / 16 / 8;                           // m-tiles (16 rows of W^T) per warp
@@ -708,7 +737,7 @@ __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, c
         *reinterpret_cast<bf16_t*>(Wsm + swz<S::WP>(k, q)) = hi;
         if (NH == 2) *reinterpret_cast<bf16_t*>(Wsm + S::WBYTES + swz<S::WP>(k, q)) = lo;
     }
-    float dhr[PAIRS], dhz[PAIRS];
+    float dhr[PAIRS], dhz[PAIRS], mk[RD ? PAIRS : 1];
     int plen[PAIRS];
 #pragma unroll
     for (int i = 0; i < PAIRS; ++i) {
@@ -716,6 +745,7 @@ __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, c
         dhr[i] = dhc[((int64_t)d * B + bt0 + b) * H + c * U + u];
         dhz[i] = 0.f;
         plen[i] = LEN ? lens[bt0 + b] : T;
+        if constexpr (RD) mk[i] = mask[((int64_t)d * B + bt0 + b) * H + c * U + u];
     }
     cluster_arrive();
     cluster_wait();
@@ -740,6 +770,7 @@ __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, c
             if (first) hprev[i] = h0 ? h0[((int64_t)d * B + b) * H + j] : 0.f;
             else hprev[i] = Y[((int64_t)b * T + (d == 0 ? t - 1 : t + 1)) * DH + d * H + j];
             dyv[i] = dY[row * DH + d * H + j];
+            if constexpr (RD) hprev[i] *= mk[i];
         }
     };
     load_step(0);
@@ -753,6 +784,8 @@ __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, c
                 float v = dhz[i];
 #pragma unroll
                 for (int src = 0; src < CS; ++src) v += slot(src)[x];
+                // the previous step (t + 1 forward, t - 1 reverse) applied a cell to the masked state unless it was padded
+                if constexpr (RD) v = LEN && (d == 0 ? t + 1 : t - 1) >= plen[i] ? v : mk[i] * v;
                 dhr[i] = v;
             }
         }
@@ -863,6 +896,7 @@ __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, c
         float v = dhz[i];
 #pragma unroll
         for (int src = 0; src < CS; ++src) v += slot(src)[x];
+        if constexpr (RD) v = LEN && (d == 0 ? 0 : T - 1) >= plen[i] ? v : mk[i] * v;
         dhc[((int64_t)d * B + bt0 + b) * H + c * U + u] = v;
     }
 }
@@ -885,6 +919,25 @@ gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, co
         const int f = n16 + (q - n16) / 2;
         gru_scan_bwd_tile<H, NS, LEN, SCAN_NB / 2>(G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, lens,
                                                     f / ntd, (f % ntd) * SCAN_NB + ((q - n16) & 1) * (SCAN_NB / 2));
+    }
+}
+
+// the backward of gru_scan_fwd_rd_kernel: Y is the unmasked output; the dgh planes pair with the masked-state planes
+template <int H, int NS, bool LEN>
+__global__ void __launch_bounds__(SCAN_THREADS, 1)
+gru_scan_bwd_rd_kernel(const float* __restrict__ G, const float* __restrict__ Y, const float* __restrict__ h0,
+                       const float* __restrict__ dY, float* __restrict__ dhc, float* __restrict__ dgi, float* __restrict__ dgh,
+                       const float* __restrict__ Whh, int64_t zW, bf16_t* __restrict__ gih, bf16_t* __restrict__ gil,
+                       bf16_t* __restrict__ ghh, bf16_t* __restrict__ ghl, int B, int T, int D, int L8, const int* __restrict__ lens,
+                       const float* __restrict__ mask) {
+    const int ntd = B / SCAN_NB, n16 = D * ntd - L8, q = blockIdx.y;
+    if (q < n16) {
+        gru_scan_bwd_tile<H, NS, LEN, SCAN_NB, true>(G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, lens,
+                                                      q / ntd, (q % ntd) * SCAN_NB, mask);
+    } else {
+        const int f = n16 + (q - n16) / 2;
+        gru_scan_bwd_tile<H, NS, LEN, SCAN_NB / 2, true>(G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, lens,
+                                                          f / ntd, (f % ntd) * SCAN_NB + ((q - n16) & 1) * (SCAN_NB / 2), mask);
     }
 }
 
@@ -1098,8 +1151,17 @@ static void scan_geometry(int R, bool two, int B, int D, int* m2, int* clusters)
 template <int HH, int NS, bool LEN>
 static int scan_fwd_launch(int out, int cs, int B, int D, cudaStream_t st, const float* gi, const float* Whh, const float* bhh,
                            int64_t zW, const float* h0, float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, int T,
-                           const int* len, int* geom) {
+                           const int* len, const float* mask, int* geom) {
     constexpr int smem = htc::FwdSmem<HH, NS>::TOTAL;
+    if (mask) {
+        if (out != htc::SCAN_TRAIN) { bigru_set_error("tc_scan_fwd: recurrent dropout runs in the training forward only"); return BIGRU_ERR_ARG; }
+        auto k = htc::gru_scan_fwd_rd_kernel<HH, NS, LEN>;
+        int R = 0, m2 = 0, clusters = 0;
+        TRY(cluster_residency(k, cs, smem, &R));
+        scan_geometry(R, htc::FwdSmem<HH, NS>::NBMAX == 2 * htc::SCAN_NB, B, D, &m2, &clusters);
+        ProfScope ps(KC_TC_SCAN_FWD, 2.0 * D * B * (double)T * 3 * HH * HH, 0.0, st);
+        return launch_cluster(k, cs, clusters, 1, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D, m2, len, mask);
+    }
     void (*k)(const float*, const float*, const float*, int64_t, const float*, float*, float*, float*, htc::bf16_t*, htc::bf16_t*,
               int, int, int, int, const int*) = nullptr;
     switch (out) {
@@ -1120,16 +1182,17 @@ static int scan_fwd_launch(int out, int cs, int B, int D, cudaStream_t st, const
 
 // one layer's forward recurrence; shapes were validated by the plan (H in {128, 256, 512}, B % 16 == 0).  A null Y, G or yh:
 // that output is not written (the instantiations: all three, planes only, Y only).  len: per-row lengths [B] or null.
+// mask: the layer's recurrent-dropout masks [D][B][H] (training outputs only; yh, yl then get the masked state) or null.
 // geom non-null: launch nothing and return the training instantiation's residency R and two-tile cluster count n2 in
 // geom[0], geom[1] (test support)
 static int tc_scan_fwd(const bigru_plan& p, int l, const float* gi, const float* Whh, const float* bhh, const float* h0,
-                       float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, const int* len, cudaStream_t st,
-                       int* geom = nullptr) {
+                       float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, const int* len, const float* mask,
+                       cudaStream_t st, int* geom = nullptr) {
     const int H = p.H, D = p.D, B = p.B, T = p.T, cs = H / htc::SCAN_U;
     const int64_t zW = p.ld_block(l);
     const int out = geom ? htc::SCAN_TRAIN : (Y ? htc::SCAN_Y : 0) | (G ? htc::SCAN_G : 0) | (yh ? htc::SCAN_PLANES : 0);
-#define FWD(HH, NS) return len ? scan_fwd_launch<HH, NS, true>(out, cs, B, D, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, T, len, geom) \
-                               : scan_fwd_launch<HH, NS, false>(out, cs, B, D, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, T, len, geom)
+#define FWD(HH, NS) return len ? scan_fwd_launch<HH, NS, true>(out, cs, B, D, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, T, len, mask, geom) \
+                               : scan_fwd_launch<HH, NS, false>(out, cs, B, D, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, T, len, mask, geom)
     if (p.prec == BIGRU_PREC_BF16X3) {
         if (H == 128) FWD(128, 3);
         if (H == 256) FWD(256, 3);
@@ -1155,8 +1218,16 @@ static void scan_bwd_geometry(int R, int B, int D, int* L8, int* clusters) {
 template <int HH, int NS, bool LEN>
 static int scan_bwd_launch(int cs, int B, int D, cudaStream_t st, const float* G, const float* Y, const float* h0, const float* dY,
                            float* dhc, float* dgi, float* dgh, const float* Whh, int64_t zW, htc::bf16_t* gih, htc::bf16_t* gil,
-                           htc::bf16_t* ghh, htc::bf16_t* ghl, int T, const int* len, int* geom) {
+                           htc::bf16_t* ghh, htc::bf16_t* ghl, int T, const int* len, const float* mask, int* geom) {
     constexpr int smem = htc::BwdSmem<HH, NS>::TOTAL;
+    if (mask) {
+        auto k = htc::gru_scan_bwd_rd_kernel<HH, NS, LEN>;
+        int R = 0, L8 = 0, clusters = 0;
+        TRY(cluster_residency(k, cs, smem, &R));
+        scan_bwd_geometry(R, B, D, &L8, &clusters);
+        ProfScope ps(KC_TC_SCAN_BWD, 2.0 * D * B * (double)T * 3 * HH * HH, 0.0, st);
+        return launch_cluster(k, cs, clusters, 1, smem, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, L8, len, mask);
+    }
     auto k = htc::gru_scan_bwd_kernel<HH, NS, LEN>;
     int R = 0, L8 = 0, clusters = 0;
     TRY(cluster_residency(k, cs, smem, &R));
@@ -1166,14 +1237,15 @@ static int scan_bwd_launch(int cs, int B, int D, cudaStream_t st, const float* G
     return launch_cluster(k, cs, clusters, 1, smem, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, L8, len);
 }
 
-// one layer's backward recurrence; geom as in tc_scan_fwd (geom[1]: the tiles split into two 8-row clusters)
+// one layer's backward recurrence; mask as in tc_scan_fwd; geom as in tc_scan_fwd (geom[1]: the tiles split into two 8-row
+// clusters)
 static int tc_scan_bwd(const bigru_plan& p, int l, const float* G, const float* Y, const float* h0, const float* dY, float* dhc,
                        float* dgi, float* dgh, const float* Whh, htc::bf16_t* gih, htc::bf16_t* gil, htc::bf16_t* ghh,
-                       htc::bf16_t* ghl, const int* len, cudaStream_t st, int* geom = nullptr) {
+                       htc::bf16_t* ghl, const int* len, const float* mask, cudaStream_t st, int* geom = nullptr) {
     const int H = p.H, D = p.D, B = p.B, T = p.T, cs = H / htc::SCAN_U;
     const int64_t zW = p.ld_block(l);
-#define BWD(HH, NS) return len ? scan_bwd_launch<HH, NS, true>(cs, B, D, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, T, len, geom) \
-                           : scan_bwd_launch<HH, NS, false>(cs, B, D, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, T, len, geom)
+#define BWD(HH, NS) return len ? scan_bwd_launch<HH, NS, true>(cs, B, D, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, T, len, mask, geom) \
+                           : scan_bwd_launch<HH, NS, false>(cs, B, D, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, T, len, mask, geom)
     if (p.prec == BIGRU_PREC_BF16X3) {
         if (H == 128) BWD(128, 3);
         if (H == 256) BWD(256, 3);

@@ -24,7 +24,7 @@ class _TrainForward:
         # refuses and nn.GRU ignores there; forward refuses p = 1 wherever it would drop
         self.drop = drop = float(mod.dropout) if mod.dropout < 1 else 0.0
         self.pad = pad = mod._pad
-        self.c = c = _PaddedCall(mod, x, h0, lengths, training=mod.training and drop > 0)
+        self.c = c = _PaddedCall(mod, x, h0, lengths, training=mod.training and (drop > 0 or mod.recurrent_dropout > 0))
         plan, D, Hp = c.plan, mod._dims()[1], pad.hidden
         with torch.cuda.device(x.device):                 # the C ABI launches on the CURRENT device: make it the model's
             self.pflat = pflat = mod._plan_params()
@@ -88,12 +88,18 @@ class GRU(_FlatModel):
     The parameters are views of one flat fp32 vector (``flat_parameters()``), which ``.cuda()`` / ``.to()`` re-pack and
     ``flatten_parameters()`` re-packs on request; a call copies no parameters.  ``BiGRU.gru`` is a GRU whose vector is the
     leading part of the BiGRU's own.
+
+    ``recurrent_dropout`` (p in [0, 1), default 0): variational dropout of the recurrent state, as in ``BiGRU``: in training
+    mode one mask per layer, direction, batch row and hidden unit, the same at every step, multiplies the state entering each
+    valid step, ``h_t = GRUCell(x_t, m * h_{t-1})``; ``output`` and ``h_n`` are unmasked, and eval mode never masks.  Not a
+    parameter; assigning the attribute takes effect at the next call.
     """
 
     _kind = "GRU"
 
     def __init__(self, input_size, hidden_size, num_layers=1, bias=True, batch_first=False, dropout=0.0,
-                 bidirectional=False, device=None, dtype=None, precision: Optional[str] = None, proj_size=0):
+                 bidirectional=False, device=None, dtype=None, precision: Optional[str] = None, proj_size=0,
+                 recurrent_dropout: float = 0.0):
         if not bias:
             raise ValueError("GRU: bias=False is not supported (the kernels always add b_ih and b_hh)")
         if proj_size != 0:
@@ -102,7 +108,9 @@ class GRU(_FlatModel):
             raise ValueError(f"GRU: parameters are float32, got dtype={dtype}")
         if not 0 <= float(dropout) <= 1:
             raise ValueError("dropout should be a number in range [0, 1]")
+        rd = self._check_recurrent_dropout(recurrent_dropout)
         super().__init__(precision)
+        self.recurrent_dropout = rd
         self.mode, self.input_size, self.hidden_size, self.num_layers = "GRU", input_size, hidden_size, num_layers
         self.bias, self.batch_first, self.dropout, self.bidirectional = True, batch_first, float(dropout), bidirectional
         self.proj_size = 0
@@ -144,8 +152,8 @@ class GRU(_FlatModel):
         return self.hidden_size, 2 if self.bidirectional else 1, self.num_layers, self.input_size, 0
 
     def _create_plan(self, lib, B, T, out):
-        _lib.check(lib.bigru_gru_plan_create(B, T, self.input_size, self._pad.hidden, self.num_layers, int(self.bidirectional),
-                                             _PRECISIONS[self._pad.precision], _lib.C.byref(out)), "bigru_gru_plan_create")
+        self._create_plan_c(lib, "bigru_gru_plan_create", (B, T, self.input_size, self._pad.hidden, self.num_layers,
+                                                           int(self.bidirectional), _PRECISIONS[self._pad.precision]), out)
 
     def flatten_parameters(self):
         """Re-pack the parameters into one flat vector when they are not views of it any more (nn.GRU's name for it)."""
@@ -162,6 +170,8 @@ class GRU(_FlatModel):
             s += f", dropout={self.dropout}"
         if self.bidirectional:
             s += ", bidirectional=True"
+        if self.recurrent_dropout:
+            s += f", recurrent_dropout={self.recurrent_dropout}"
         return s + f", precision={self.precision!r}"
 
     def forward(self, input, hx=None, lengths=None):
@@ -209,7 +219,7 @@ class GRU(_FlatModel):
         if torch.is_grad_enabled() and (xs.requires_grad or (h0 is not None and h0.requires_grad)
                                         or any(p.requires_grad for p in params)):
             y, hn = _GRUFunction.apply(self, xs, h0, lens, *params)
-        elif self._drops():                               # nn.GRU drops in training mode without grad mode too
+        elif self._drops() or self._masks():              # nn.GRU drops in training mode without grad mode too
             with torch.no_grad():
                 f = _TrainForward(self, xs, h0, lens)
                 f.c.plan.release_stash(f.stash)
@@ -225,6 +235,10 @@ class GRU(_FlatModel):
     def _drops(self) -> bool:
         """Whether a call drops anything: training mode, dropout > 0 and a layer above the first."""
         return bool(self.training and self.dropout > 0 and self.num_layers > 1)
+
+    def _masks(self) -> bool:
+        """Whether a call masks the recurrent state: training mode and recurrent_dropout > 0."""
+        return bool(self.training and self.recurrent_dropout > 0)
 
     def _infer(self, x, h0, lengths):
         """(y, h_n) of the real rows through bigru_gru_infer, without an autograd record."""

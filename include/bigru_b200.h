@@ -67,6 +67,20 @@ int  bigru_device_check(int dev);
  *     (biGRU_model.py:32-60).  Immutable after creation. */
 int  bigru_plan_create(int B, int T, int F, int H, int L, int C, int bidirectional, int precision,
                        bigru_plan** out);
+/* --- recurrent (variational) dropout, Gal & Ghahramani 2016 (DESIGN.md §4.8): the same plans with recurrent_p in [0, 1)
+ *  (else BIGRU_ERR_ARG).  recurrent_p = 0 gives exactly the plan of bigru_plan_create / bigru_gru_plan_create.  On a plan with
+ *  recurrent_p > 0, a training forward (training != 0: bigru_forward*, bigru_gru_forward) draws, for every layer l and
+ *  direction d, a mask m[b][j] in {0, 1/(1-p)} per batch row and hidden unit, the same at every step, and runs each valid
+ *  step as h_t = GRUCell(x_t, m * h_{t-1}) (h_{-1} = h0, or 0).  y_t = h_t and h_n are unmasked; a padded step applies no
+ *  cell and no mask.  m[b][j] is 0 where bigru_uniform(seed, BIGRU_RD_STREAM + l, (b*D + d)*H + j) < p; input and
+ *  inter-layer dropout use the streams l < 16, which never reach BIGRU_RD_STREAM.  The backward must get the forward's seed
+ *  and training flag.  Inference (bigru_infer*, bigru_gru_infer) and training = 0 never mask.  The stash grows by the masks
+ *  and the masked states (BIGRU_WS_RD_MASK, BIGRU_WS_RD_STATE). */
+#define BIGRU_RD_STREAM 65536u
+int  bigru_plan_create_rd(int B, int T, int F, int H, int L, int C, int bidirectional, int precision, float recurrent_p,
+                          bigru_plan** out);
+int  bigru_gru_plan_create_rd(int B, int T, int F, int H, int L, int bidirectional, int precision, float recurrent_p,
+                              bigru_plan** out);
 int  bigru_plan_destroy(bigru_plan* plan);
 int64_t bigru_param_count(const bigru_plan* plan);
 /* which: 0 w_ih, 1 w_hh, 2 b_ih, 3 b_hh for layer<L; layer==L: 0 lin_w, 2 lin_b (BIGRU_ERR_ARG on a plan without a head) */
@@ -98,6 +112,10 @@ int  bigru_stash_output_offset(const bigru_plan* plan, int layer, size_t* byte_o
  *   BIGRU_WS_DY             scratch  0, 1       upstream gradient of the layer's output [B*T][D*H]; bigru_backward
  *   BIGRU_WS_DHC            scratch  0          dh_{-1} of layer 0 [D][B][H]; bigru_backward
  *   BIGRU_WS_DCAT           scratch  L (head)   d cat [B][3H] (last | max | mean); bigru_backward
+ *   BIGRU_WS_RD_MASK        stash    0..L-1     recurrent-dropout masks m [D][B][H] fp32; training bigru_forward, plans with
+ *                                               recurrent_p > 0 only
+ *   BIGRU_WS_RD_STATE       stash    0..L-1     the masked state m * h_t [B*T][D*H] (0 at padded steps): planes at the
+ *                                               tensor-core precisions, fp32 at BIGRU_PREC_FP32; as BIGRU_WS_RD_MASK
  * Planes at BIGRU_PREC_FP32: BIGRU_ERR_UNSUPPORTED.  Another layer or an unknown `which`: BIGRU_ERR_ARG. */
 #define BIGRU_WS_GATES       0
 #define BIGRU_WS_Y_PLANES    1
@@ -109,7 +127,9 @@ int  bigru_stash_output_offset(const bigru_plan* plan, int layer, size_t* byte_o
 #define BIGRU_WS_DY          7
 #define BIGRU_WS_DHC         8
 #define BIGRU_WS_DCAT        9
-#define BIGRU_WS_COUNT      10
+#define BIGRU_WS_RD_MASK    10
+#define BIGRU_WS_RD_STATE   11
+#define BIGRU_WS_COUNT      12
 int  bigru_workspace_region(const bigru_plan* plan, int which, int layer, int* in_scratch, size_t* byte_offset,
                             size_t* lo_byte_offset, int64_t* pitch);
 
