@@ -308,8 +308,11 @@ extern "C" int bigru_scan_geometry(const bigru_plan* p, int scan, int* R, int* n
     if (!p || !R || !n_split || (scan != 0 && scan != 1)) { bigru_set_error("scan_geometry: bad argument"); return BIGRU_ERR_ARG; }
     if (p->prec == BIGRU_PREC_FP32) { bigru_set_error("scan_geometry: BIGRU_PREC_FP32 runs no cluster scans"); return BIGRU_ERR_UNSUPPORTED; }
     int geom[2] = {0, 0};
-    if (scan == 0) TRY(tc_scan_fwd(*p, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, geom));
-    else TRY(tc_scan_bwd(*p, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, geom));
+    // a plan with recurrent dropout trains with the _rd scans: a non-null mask selects them (a placeholder, never read)
+    static const float placeholder = 0.f;
+    const float* mask = p->rp > 0.f ? &placeholder : nullptr;
+    if (scan == 0) TRY(tc_scan_fwd(*p, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, mask, 0, geom));
+    else TRY(tc_scan_bwd(*p, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, mask, 0, geom));
     *R = geom[0]; *n_split = geom[1];
     return BIGRU_OK;
 }

@@ -1159,6 +1159,7 @@ static int scan_fwd_launch(int out, int cs, int B, int D, cudaStream_t st, const
         int R = 0, m2 = 0, clusters = 0;
         TRY(cluster_residency(k, cs, smem, &R));
         scan_geometry(R, htc::FwdSmem<HH, NS>::NBMAX == 2 * htc::SCAN_NB, B, D, &m2, &clusters);
+        if (geom) { geom[0] = R; geom[1] = D * m2; return BIGRU_OK; }
         ProfScope ps(KC_TC_SCAN_FWD, 2.0 * D * B * (double)T * 3 * HH * HH, 0.0, st);
         return launch_cluster(k, cs, clusters, 1, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D, m2, len, mask);
     }
@@ -1184,7 +1185,7 @@ static int scan_fwd_launch(int out, int cs, int B, int D, cudaStream_t st, const
 // that output is not written (the instantiations: all three, planes only, Y only).  len: per-row lengths [B] or null.
 // mask: the layer's recurrent-dropout masks [D][B][H] (training outputs only; yh, yl then get the masked state) or null.
 // geom non-null: launch nothing and return the training instantiation's residency R and two-tile cluster count n2 in
-// geom[0], geom[1] (test support)
+// geom[0], geom[1] (test support); with a mask, those of the recurrent-dropout kernel (the mask is not read)
 static int tc_scan_fwd(const bigru_plan& p, int l, const float* gi, const float* Whh, const float* bhh, const float* h0,
                        float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, const int* len, const float* mask,
                        cudaStream_t st, int* geom = nullptr) {
@@ -1225,6 +1226,7 @@ static int scan_bwd_launch(int cs, int B, int D, cudaStream_t st, const float* G
         int R = 0, L8 = 0, clusters = 0;
         TRY(cluster_residency(k, cs, smem, &R));
         scan_bwd_geometry(R, B, D, &L8, &clusters);
+        if (geom) { geom[0] = R; geom[1] = L8; return BIGRU_OK; }
         ProfScope ps(KC_TC_SCAN_BWD, 2.0 * D * B * (double)T * 3 * HH * HH, 0.0, st);
         return launch_cluster(k, cs, clusters, 1, smem, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, L8, len, mask);
     }

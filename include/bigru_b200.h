@@ -136,7 +136,8 @@ int  bigru_workspace_region(const bigru_plan* plan, int which, int layer, int* i
 /* --- Recurrence scan geometry of a tensor-core plan on the current device (test support).  *R: clusters of the scan the
  *  device holds at once.  scan 0, the forward (training instantiation): *n_split = clusters that take two 16-row batch
  *  tiles (the lowest cluster ids; always 0 at BIGRU_PREC_BF16).  scan 1, the backward: *n_split = batch tiles of the last
- *  round split into two 8-row clusters each (the highest cluster ids).  No result depends on them.
+ *  round split into two 8-row clusters each (the highest cluster ids).  No result depends on them.  On a plan with
+ *  recurrent_p > 0 both describe the recurrent-dropout scans, which that plan's training calls launch.
  *  BIGRU_PREC_FP32: BIGRU_ERR_UNSUPPORTED; another scan: BIGRU_ERR_ARG. */
 int  bigru_scan_geometry(const bigru_plan* plan, int scan, int* R, int* n_split);
 

@@ -1,13 +1,14 @@
 """Drives the library's C ABI on one plan and takes the result apart tensor by tensor.  Test infrastructure, shared by
-test_gpu_rounding_model.py, test_gpu_fp32_path.py and test_gpu_tc_steps.py.
+test_gpu_rounding_model.py, test_gpu_fp32_path.py, test_gpu_tc_steps.py, test_gpu_scan_tiles.py and test_gpu_rd_steps.py.
 
 A shape is a dict with B, T, F, H, L, C, D (1 or 2) and h0 (bool).  `kernel` runs bigru_forward and bigru_backward at a
-precision ("fp32", "bf16" or "bf16x3"), optionally with dropout, and returns every layer's output, hn, the max-pool
-routing, the flat gradient, dx and dh0 in float64 (with regions=True also the backward's intermediates, read through
-bigru_workspace_region).  `tensors` / `kernel_steps` split such a result into the per-tensor comparisons, `stepwise`
+precision ("fp32", "bf16" or "bf16x3"), optionally with dropout, recurrent dropout and per-sequence lengths, and returns
+every layer's output, hn, the max-pool routing, the flat gradient, dx and dh0 in float64 (with regions=True also the
+backward's intermediates, read through bigru_workspace_region).  `tensors` / `kernel_steps` split such a result into the per-tensor comparisons, `stepwise`
 recomputes one forward step from the kernel's own state, `backward_steps` / `gemm_steps` each backward step of layer 0
 and each backward GEMM from the kernel's own operands, `plane_checks` the bf16 planes bit for bit, `dist` measures two
-tensors."""
+tensors.  The models take optional recurrent-dropout masks and lengths (DESIGN.md §4.8, §4.5); without them they are the
+models of the plain path, operation for operation."""
 import ctypes as C
 
 import numpy as np
@@ -73,6 +74,7 @@ def abi_names(s):
 
 # BIGRU_WS_* of include/bigru_b200.h
 WS = dict(GATES=0, Y_PLANES=1, IN_PLANES=2, DGI=3, DGH=4, DGI_PLANES=5, DGH_PLANES=6, DY=7, DHC=8, DCAT=9)
+WS_RD = dict(RD_MASK=10, RD_STATE=11)           # the regions of plans with recurrent dropout only
 PLANE_REGIONS = ("Y_PLANES", "IN_PLANES", "DGI_PLANES", "DGH_PLANES")
 
 
@@ -80,7 +82,7 @@ def region(plan, which, layer):
     """bigru_workspace_region: (rc, in_scratch, byte offset, lo byte offset, pitch)."""
     lib = _pkg()._lib.load()
     sc, off, lo, pitch = C.c_int(), C.c_size_t(), C.c_size_t(), C.c_int64()
-    rc = lib.bigru_workspace_region(plan, WS[which], layer, C.byref(sc), C.byref(off), C.byref(lo), C.byref(pitch))
+    rc = lib.bigru_workspace_region(plan, {**WS, **WS_RD}[which], layer, C.byref(sc), C.byref(off), C.byref(lo), C.byref(pitch))
     return rc, sc.value, off.value, lo.value, pitch.value
 
 
@@ -89,10 +91,11 @@ def _bits_to_f32(u16):
     return (u16.astype(np.uint32) << np.uint32(16)).view(np.float32)
 
 
-def _workspace(plan, s, prec, stash, scratch):
+def _workspace(plan, s, prec, stash, scratch, rd=False):
     """The backward's operands and intermediates (bigru_workspace_region) as host arrays: fp32 regions as float32, planes
-    as (hi, lo) pairs of bf16 bit patterns (uint16; lo None at bf16).  Rows are split into [B, T] (and a leading D where
-    there is one)."""
+    as (hi, lo) pairs of bf16 bit patterns (uint16; lo None at bf16; both None at fp32, which keeps no planes).  Rows are
+    split into [B, T] (and a leading D where there is one).  rd: also every layer's recurrent-dropout masks RDM [D, B, H]
+    and masked state RDS [B, T, D*H] (planes, or float32 at fp32)."""
     B, T, F, H, L, D = (s[k] for k in "BTFHLD")
     bufs = (stash, scratch)
 
@@ -102,6 +105,8 @@ def _workspace(plan, s, prec, stash, scratch):
         return bufs[sc][off // 4: off // 4 + n].view(*shape).cpu().numpy()
 
     def planes(which, layer, shape):
+        if prec == "fp32":
+            return None, None
         _, sc, off, lo, _ = region(plan, which, layer)
         n = int(np.prod(shape))
         v = bufs[sc].view(torch.int16)
@@ -116,17 +121,22 @@ def _workspace(plan, s, prec, stash, scratch):
               DGIP=planes("DGI_PLANES", 0, (D, B, T, 3 * H)), DGHP=planes("DGH_PLANES", 0, (D, B, T, 3 * H)),
               DY=[f32("DY", l, (B, T, D * H)) for l in range(min(L, 2))],
               DHC=f32("DHC", 0, (D, B, H)), DCAT=f32("DCAT", L, (B, 3 * H)))
+    if rd:
+        ws["RDM"] = [f32("RD_MASK", l, (D, B, H)) for l in range(L)]
+        ws["RDS"] = [(f32("RD_STATE", l, (B, T, D * H)), None) if prec == "fp32" else planes("RD_STATE", l, (B, T, D * H))
+                     for l in range(L)]
     return ws
 
 
-def kernel(s, prec, flat, x, h0, dl, p=0.0, spatial=False, seed=0, regions=False):
-    """bigru_forward + bigru_backward of shape s at precision prec; dropout p (training mode) when p > 0.  regions: the
-    result also holds "ws", the intermediates of _workspace (tensor-core precisions)."""
+def kernel(s, prec, flat, x, h0, dl, p=0.0, spatial=False, seed=0, regions=False, rd_p=0.0, lens=None):
+    """bigru_forward_lengths + bigru_backward_lengths of shape s at precision prec on a bigru_plan_create_rd plan (p = 0:
+    bigru_plan_create's plan); dropout p and recurrent dropout rd_p (training mode when either is on); lens: per-row
+    lengths [B] or None.  regions: the result also holds "ws", the intermediates of _workspace."""
     pkg = _pkg()
     lib, L_ = pkg._lib.load(), pkg._lib
     B, T, F, H, L, C_, D = (s[k] for k in "BTFHLCD")
     plan = C.c_void_p()
-    L_.check(lib.bigru_plan_create(B, T, F, H, L, C_, int(D == 2), CODE[prec], C.byref(plan)), "plan_create")
+    L_.check(lib.bigru_plan_create_rd(B, T, F, H, L, C_, int(D == 2), CODE[prec], rd_p, C.byref(plan)), "plan_create")
     try:
         sb, cb = C.c_size_t(), C.c_size_t()
         L_.check(lib.bigru_workspace_bytes(plan, C.byref(sb), C.byref(cb)), "workspace_bytes")
@@ -139,9 +149,10 @@ def kernel(s, prec, flat, x, h0, dl, p=0.0, spatial=False, seed=0, regions=False
         hn = torch.zeros(L * D, B, H, device=dev)
         st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
         ptr = L_.ptr
-        train = int(p > 0)
-        L_.check(lib.bigru_forward(plan, ptr(pd), ptr(xd), ptr(h0d), p, int(spatial), train, seed, ptr(stash), ptr(scratch),
-                                   ptr(logits), ptr(hn), st), "forward")
+        train = int(p > 0 or rd_p > 0)
+        lend = None if lens is None else torch.from_numpy(np.asarray(lens, np.int32)).to(dev)
+        L_.check(lib.bigru_forward_lengths(plan, ptr(pd), ptr(xd), ptr(h0d), p, int(spatial), train, seed, ptr(stash),
+                                           ptr(scratch), ptr(logits), ptr(hn), ptr(lend), st), "forward")
         off = C.c_size_t()
         ys = []
         for l in range(L):
@@ -153,11 +164,11 @@ def kernel(s, prec, flat, x, h0, dl, p=0.0, spatial=False, seed=0, regions=False
         dx = torch.zeros(B, T, F, device=dev)
         dh0 = torch.zeros(L * D, B, H, device=dev) if h0 is not None else None
         dld = torch.from_numpy(dl).to(dev)                      # alive until the synchronize below: the backward reads it
-        L_.check(lib.bigru_backward(plan, ptr(pd), ptr(xd), ptr(h0d), p, int(spatial), train, seed, ptr(stash), ptr(scratch),
-                                    ptr(dld), ptr(grads), ptr(dx), ptr(dh0), st), "backward")
+        L_.check(lib.bigru_backward_lengths(plan, ptr(pd), ptr(xd), ptr(h0d), p, int(spatial), train, seed, ptr(stash),
+                                            ptr(scratch), ptr(dld), ptr(grads), ptr(dx), ptr(dh0), ptr(lend), st), "backward")
         torch.cuda.synchronize()
         names = param_names(plan, s)
-        ws = _workspace(plan, s, prec, stash, scratch) if regions else None
+        ws = _workspace(plan, s, prec, stash, scratch, rd=rd_p > 0) if regions else None
         del stash, scratch
     finally:
         lib.bigru_plan_destroy(plan)
@@ -229,17 +240,28 @@ def rows64(p, sl, cols=slice(None)):
     return f64(p[0][sl, cols]), (None if p[1] is None else f64(p[1][sl, cols]))
 
 
-def stepwise(s, prec, flat, x, h0, dl, got, names, rows=None, gates=False):
+def _masked(m, v, prec):
+    """m * v as the kernels form the masked state: a float32 product (in float64 at "exact")."""
+    if prec == "exact":
+        return np.asarray(m, np.float64) * v
+    return (np.asarray(m, np.float32) * np.asarray(v, np.float32)).astype(np.float64)
+
+
+def stepwise(s, prec, flat, x, h0, dl, got, names, rows=None, gates=False, masks=None, lens=None, drops=None):
     """The model at `prec` (mm's) run one step at a time from the kernel's own state: every step of every layer starts
     from the kernel's h_{t-1} (its Y, or h0) and the kernel's layer input (x, or the previous layer's Y), the head from
     the kernel's top-layer Y.  Rounding flips cannot compound, so what is left of the kernel's distance is the arithmetic
     of one step.  At "fp32" every operation is float32.  Returns (name, class) -> array like `tensors`: Y per layer,
     direction and step, the logits and the lin_w gradient.  rows: the batch rows the layers are stepped for (all when
     None; the head always takes all).  gates: also G per layer, direction and step (class g_step), the model's r, z, n and
-    W_hn h_{t-1} + b_hn, which the forward scan stashes for the backward."""
+    W_hn h_{t-1} + b_hn, which the forward scan stashes for the backward.
+    masks: recurrent-dropout masks per layer [D, B, H] (DESIGN.md §4.8): gh and the carry take m * h_{t-1} (_masked).
+    lens: per-row lengths [B]: a padded (row, t) has Y = 0 and no G (0 in the zeroed stash); the head pools valid steps.
+    drops: per layer None or the float32 factor dropout_kernel multiplies that layer's input by."""
     B, T, H, L, C_, D = (s[k] for k in "BTHLCD")
     rows = np.arange(B) if rows is None else np.asarray(rows)
     B = len(rows)
+    valid = None if lens is None else (np.arange(T)[None, :] < np.asarray(lens)[rows][:, None])[..., None]
     dt = np.float32 if prec == "fp32" else np.float64
     one = dt(1)
     out = {}
@@ -247,6 +269,8 @@ def stepwise(s, prec, flat, x, h0, dl, got, names, rows=None, gates=False):
     inp = x[rows].astype(dt)
     for l in range(L):
         Y = got["ys"][l][rows].astype(dt)
+        if drops is not None and drops[l] is not None:
+            inp = (inp.astype(np.float32) * drops[l][rows]).astype(dt)
         I = inp.shape[2]
         for d in range(D):
             o = names[f"l{l}d{d}.w_ih"][0]
@@ -259,22 +283,33 @@ def stepwise(s, prec, flat, x, h0, dl, got, names, rows=None, gates=False):
                 hp = np.concatenate([start[:, None], y[:, :-1]], 1)
             else:
                 hp = np.concatenate([y[:, 1:], start[:, None]], 1)
+            if masks is not None:
+                hp = _masked(masks[l][d][rows][:, None, :], hp, prec).astype(dt)
             gi = (mm(inp.reshape(B * T, I), w_ih, prec) + b_ih).reshape(B, T, 3 * H)
             gh = (mm(hp.reshape(B * T, H), w_hh, prec) + b_hh).reshape(B, T, 3 * H)
             r = sig(gi[..., :H] + gh[..., :H])
             z = sig(gi[..., H:2 * H] + gh[..., H:2 * H])
             n = np.tanh(gi[..., 2 * H:] + r * gh[..., 2 * H:])
             h = (one - z) * n + z * hp
+            if valid is not None:
+                h = np.where(valid, h, dt(0))
             for t in range(T):
                 out[(f"step:y[l{l}d{d},t{t}]", "y_step")] = h[:, t].astype(np.float64)
                 if gates:
-                    out[(f"step:g[l{l}d{d},t{t}]", "g_step")] = np.concatenate(
-                        [r[:, t], z[:, t], n[:, t], gh[:, t, 2 * H:]], 1).astype(np.float64)
+                    g = np.concatenate([r[:, t], z[:, t], n[:, t], gh[:, t, 2 * H:]], 1).astype(np.float64)
+                    out[(f"step:g[l{l}d{d},t{t}]", "g_step")] = g if valid is None else np.where(valid[:, t], g, 0.0)
         inp = Y
     top = got["ys"][-1].astype(dt)
     pooled = top[..., :H] + top[..., H:] if D == 2 else top
-    last = top[:, T - 1, :H] + (top[:, 0, H:] if D == 2 else 0)
-    cat = np.concatenate([last, pooled.max(1), pooled.sum(1) / dt(T)], 1)
+    if lens is None:
+        last = top[:, T - 1, :H] + (top[:, 0, H:] if D == 2 else 0)
+        cat = np.concatenate([last, pooled.max(1), pooled.sum(1) / dt(T)], 1)
+    else:
+        # head_pool_kernel: the forward direction's last valid step, max and mean over the valid steps (padded Y is 0)
+        n_b = np.asarray(lens)
+        ok = (np.arange(T)[None, :] < n_b[:, None])[..., None]
+        last = top[np.arange(len(n_b)), n_b - 1, :H] + (top[:, 0, H:] if D == 2 else 0)
+        cat = np.concatenate([last, np.where(ok, pooled, -np.inf).max(1), pooled.sum(1) / n_b[:, None].astype(dt)], 1)
     o = names["lin_w"][0]
     lin_w = flat[o:o + C_ * 3 * H].reshape(C_, 3 * H).astype(dt)
     lin_b = flat[names["lin_b"][0]:names["lin_b"][0] + C_].astype(dt)
@@ -310,17 +345,23 @@ def head_dcat(s, prec, flat, dl, names):
     return pmm(split(dl, prec), split(_block(flat, names, "lin_w", (s["C"], 3 * s["H"])), prec))
 
 
-def head_dy(s, dcat, arg):
+def head_dy(s, dcat, arg, lens=None):
     """The top layer's upstream gradient [B, T, D*H] from d cat and the max-pool routing, as head_bwd_dy_kernel routes it:
     the mean's share at every step plus the max's at the arg-max step, the same for both directions.  (The `last` share
-    is the carry into the layer's last step, dcat[:, :H].)"""
+    is the carry into the layer's last step, dcat[:, :H].)  lens: the mean's share is over len valid steps, and padded
+    steps get 0 (the `last` share passes through them to t = len - 1 in the backward scan)."""
     B, T, H, D = (s[k] for k in "BTHD")
-    v = np.broadcast_to(dcat[:, None, 2 * H:] / T, (B, T, H)).copy()
+    if lens is None:
+        v = np.broadcast_to(dcat[:, None, 2 * H:] / T, (B, T, H)).copy()
+    else:
+        v = np.broadcast_to(dcat[:, None, 2 * H:] / np.asarray(lens)[:, None, None], (B, T, H)).copy()
     v += np.where(arg[:, None, :] == np.arange(T)[None, :, None], dcat[:, None, H:2 * H], 0.0)
+    if lens is not None:
+        v[np.arange(T)[None, :] >= np.asarray(lens)[:, None]] = 0.0
     return np.concatenate([v] * D, 2)
 
 
-def backward_steps(s, prec, flat, h0, ws, ys, names, own=False):
+def backward_steps(s, prec, flat, h0, ws, ys, names, own=False, masks=None, lens=None):
     """Layer 0's backward recurrence one step at a time in float64, following gru_scan_bwd_kernel (tc_hopper.cuh), per
     direction in the kernel's step order.  Each step takes the kernel's own operands: its dY (ws["DY"][0]), its gates
     (ws["G"][0]) and its h_{t-1} (ys[0], or h0), and
@@ -330,30 +371,47 @@ def backward_steps(s, prec, flat, h0, ws, ys, names, own=False):
     so rounding flips cannot compound.  It starts from the head's `last` share of the kernel's dcat when layer 0 is the
     top layer, else from zero.  own: P takes the model's own dgh instead, which makes this the oracle's free-running
     backward again.  Yields ("dg", d, t, dgi, dgh) per step ([B, 3H] each: dgi's n gate is dan, dgh's is dan r) and
-    ("dh0", d, None, dh_{-1}, None) after each direction's last step."""
+    ("dh0", d, None, dh_{-1}, None) after each direction's last step.
+    masks: layer 0's recurrent-dropout masks [D, B, H] (DESIGN.md §4.8): the gate math takes m * h_{t-1} (_masked), and
+    the carry leaving a valid step is m (dh z + P).  The dh0 item then ends in the carry before the last step's mask (the
+    fp32 path masks it into dh0 later; the scans' dh_{-1} is masked).  lens: a padded step has dgi = dgh = 0 and passes the
+    carry on unchanged and unmasked."""
     B, T, H, L, D = (s[k] for k in "BTHLD")
     for d in range(D):
         w = split(_block(flat, names, f"l0d{d}.w_hh", (3 * H, H)), prec)        # P[b, k] = sum_q dgh[b, q] W[q, k]
         G, y, dY = ws["G"][0][d], ys[0][:, :, d * H:(d + 1) * H], ws["DY"][0][:, :, d * H:(d + 1) * H]
         carry = ws["DCAT"][:, :H].astype(np.float64) if L == 1 else np.zeros((B, H))
         start = np.zeros((B, H)) if h0 is None else h0[d].astype(np.float64)
+        raw = None
         for st in range(T):
             t = T - 1 - st if d == 0 else st
             first = t == (0 if d == 0 else T - 1)
             g = G[:, t].astype(np.float64)
             r, z, n, hnv = g[:, :H], g[:, H:2 * H], g[:, 2 * H:3 * H], g[:, 3 * H:]
             hp = start if first else y[:, t - 1 if d == 0 else t + 1].astype(np.float64)
+            if masks is not None:
+                hp = _masked(masks[d], hp, prec)
             dh = carry + dY[:, t]
             dan = dh * (1 - z) * (1 - n * n)
             dar = dan * hnv * r * (1 - r)
             daz = dh * (hp - n) * z * (1 - z)
+            dgi = np.concatenate([dar, daz, dan], 1)
             dgh = np.concatenate([dar, daz, dan * r], 1)
-            yield "dg", d, t, np.concatenate([dar, daz, dan], 1), dgh
-            carry = dh * z + pmm(split(dgh if own else ws["DGH"][d][:, t], prec), w)
-        yield "dh0", d, None, carry, None
+            ok = None if lens is None else (np.asarray(lens) > t)[:, None]
+            if ok is not None:
+                dgi, dgh = np.where(ok, dgi, 0.0), np.where(ok, dgh, 0.0)
+            yield "dg", d, t, dgi, dgh
+            new = dh * z + pmm(split(dgh if own else ws["DGH"][d][:, t], prec), w)
+            if masks is not None:
+                raw, new = new, masks[d].astype(np.float64) * new
+            if ok is not None:
+                new = np.where(ok, new, carry)
+                raw = None if raw is None else np.where(ok, raw, carry)
+            carry = new
+        yield "dh0", d, None, carry, raw
 
 
-def gemm_steps(s, prec, flat, dl, h0, ops, names, arg):
+def gemm_steps(s, prec, flat, dl, h0, ops, names, arg, masks=None, lens=None):
     """Every backward GEMM of layer 0 and of the head in float64, from the operands the kernels read: `ops` holds the dgi
     and dgh planes (DGIP, DGHP: (hi, lo) [D, B, T, 3H]), the layer input's planes (XP [B, T, pitch]), the Y planes of layer
     0 (YP [B, T, D*H]), fp32 dgi and dgh (DGI, DGH [D, B, T, 3H]) and the kernel's dcat.  Returns (name, "gemm_step") ->
@@ -364,11 +422,13 @@ def gemm_steps(s, prec, flat, dl, h0, ops, names, arg):
       dx                 sum over d of dgi planes W_ih[d] (the kcat GEMM);
       dcat               dlogits lin_w;
       dy[l{L-1}]         the top layer's upstream gradient from the kernel's dcat and `arg` (when it survives the backward:
-                         layers 0 and 1)."""
+                         layers 0 and 1).
+    masks: layer 0's recurrent-dropout masks [D, B, H]: dW_hh takes the masked-state planes ops["RDS"] instead of the Y
+    planes, and its w0 term m * h0 (_masked).  lens: as head_dy."""
     B, T, F, H, L, D = (s[k] for k in "BTFHLD")
     BT = B * T
     flat2 = lambda p, d=None: tuple(None if a is None else (a if d is None else a[d]).reshape(BT, -1) for a in p)   # noqa: E731
-    xp, yp = flat2(ops["XP"]), flat2(ops["YP"])
+    xp, yp = flat2(ops["XP"]), flat2(ops["YP"] if masks is None else ops["RDS"])
     t_of = np.arange(BT) % T
     dx = np.zeros((BT, F))
     out = {}
@@ -390,7 +450,8 @@ def gemm_steps(s, prec, flat, dl, h0, ops, names, arg):
             dx[sl] += pmm(a, w_ih)
         if h0 is not None:
             tf = 0 if d == 0 else T - 1
-            dwhh += pmm(tr(split(ops["DGH"][d][:, tf], prec)), split(h0[d], prec))
+            h0d = h0[d] if masks is None else _masked(masks[d], h0[d], prec)
+            dwhh += pmm(tr(split(ops["DGH"][d][:, tf], prec)), split(h0d, prec))
         out[(f"gemm:grad:l0d{d}.w_ih", "gemm_step")] = dwih.ravel()
         out[(f"gemm:grad:l0d{d}.w_hh", "gemm_step")] = dwhh.ravel()
         out[(f"gemm:grad:l0d{d}.b_ih", "gemm_step")] = ops["DGI"][d].reshape(BT, 3 * H).astype(np.float64).sum(0)
@@ -398,7 +459,7 @@ def gemm_steps(s, prec, flat, dl, h0, ops, names, arg):
     out[("gemm:dx", "gemm_step")] = dx.reshape(B, T, F)
     out[("gemm:dcat", "gemm_step")] = head_dcat(s, prec, flat, dl, names)
     if L <= 2:
-        out[(f"gemm:dy[l{L - 1}]", "gemm_step")] = head_dy(s, ops["DCAT"].astype(np.float64), arg)
+        out[(f"gemm:dy[l{L - 1}]", "gemm_step")] = head_dy(s, ops["DCAT"].astype(np.float64), arg, lens)
     return out
 
 
@@ -423,29 +484,56 @@ def _split_bits(v32, prec):
     return bits(hi), (bits(bf16(v32 - hi)) if prec == "bf16x3" else None)
 
 
-def plane_checks(got, s, prec, x):
+def plane_checks(got, s, prec, x, masks=None, lens=None, drop=False):
     """Elements (hi and lo together) where a plane the kernels wrote differs bitwise from split_bf16 of its fp32 source:
-    the Y planes of every layer; layer 0's input planes (x, zero-padded to the pitch); the dgi planes; the dgh planes, zero
-    at each sequence's first step.  name -> count; all must be 0."""
-    ws, T, F = got["ws"], s["T"], s["F"]
+    the Y planes of every layer; layer 0's input planes (x, zero-padded to the pitch; the dropped x under dropout); the dgi
+    planes; the dgh planes, zero at each sequence's first step.  name -> count; all must be 0.
+    masks: the host restatement of the recurrent-dropout masks [L, D, B, H] (rd_masks).  Then the masks in the stash must
+    equal them, RDS[l] must be split_bf16 of fp32(m * Y) (at fp32 the float32 product itself; only these two at fp32), and
+    the Y planes exist only for a layer below the top whose next layer reads them (to_planes_kernel): not where that layer
+    owns its input planes, as every layer above 0 does under dropout (drop).  lens: the dgi and dgh planes are zero at
+    padded steps."""
+    ws, T, F, H, D = got["ws"], s["T"], s["F"], s["H"], s["D"]
     bad = lambda a, b: int((a != b).sum())                                       # noqa: E731
 
     def cmp(pl, want):
         n = bad(pl[0], want[0])
         return n + (bad(pl[1], want[1]) if prec == "bf16x3" else 0)
 
-    out = {f"Y_PLANES[l{l}]": cmp(ws["YP"][l], _split_bits(y.astype(np.float32), prec)) for l, y in enumerate(got["ys"])}
+    out = {}
+    if masks is not None:
+        for l, y in enumerate(got["ys"]):
+            out[f"RD_MASK[l{l}]"] = bad(ws["RDM"][l].view(np.uint32), np.asarray(masks[l], np.float32).view(np.uint32))
+            r = np.concatenate([np.asarray(masks[l][d], np.float32)[:, None, :] * y[..., d * H:(d + 1) * H].astype(np.float32)
+                                for d in range(D)], 2)
+            if prec == "fp32":
+                out[f"RD_STATE[l{l}]"] = bad(ws["RDS"][l][0].view(np.uint32), r.view(np.uint32))
+            else:
+                out[f"RD_STATE[l{l}]"] = cmp(ws["RDS"][l], _split_bits(r, prec))
+        if prec == "fp32":
+            return out
+    for l, y in enumerate(got["ys"]):
+        if masks is None or (l + 1 < s["L"] and not drop):
+            out[f"Y_PLANES[l{l}]"] = cmp(ws["YP"][l], _split_bits(y.astype(np.float32), prec))
     xw = np.zeros(ws["XP"][0].shape, np.float32)
     xw[..., :F] = x
     hi, lo = _split_bits(xw, prec)
     out["IN_PLANES[l0]"] = cmp(ws["XP"], (hi, lo))
-    out["DGI_PLANES"] = cmp(ws["DGIP"], _split_bits(ws["DGI"], prec))
+    padded = None if lens is None else np.arange(T)[None, :] >= np.asarray(lens)[:, None]
+    want = [p.copy() if p is not None else None for p in _split_bits(ws["DGI"], prec)]
+    if padded is not None:
+        for p in want:
+            if p is not None:
+                p[:, padded] = 0
+    out["DGI_PLANES"] = cmp(ws["DGIP"], want)
     want = [p.copy() if p is not None else None for p in _split_bits(ws["DGH"], prec)]
     for p in want:
         if p is not None:
             p[0, :, 0] = 0
             if s["D"] == 2:
                 p[1, :, T - 1] = 0
+            if padded is not None:
+                p[:, padded] = 0
     out["DGH_PLANES"] = cmp(ws["DGHP"], want)
     return out
 
