@@ -307,14 +307,7 @@ extern "C" int bigru_stash_output_offset(const bigru_plan* p, int layer, size_t*
 extern "C" int bigru_scan_geometry(const bigru_plan* p, int scan, int* R, int* n_split) {
     if (!p || !R || !n_split || (scan != 0 && scan != 1)) { bigru_set_error("scan_geometry: bad argument"); return BIGRU_ERR_ARG; }
     if (p->prec == BIGRU_PREC_FP32) { bigru_set_error("scan_geometry: BIGRU_PREC_FP32 runs no cluster scans"); return BIGRU_ERR_UNSUPPORTED; }
-    int geom[2] = {0, 0};
-    // a plan with recurrent dropout trains with the _rd scans: a non-null mask selects them (a placeholder, never read)
-    static const float placeholder = 0.f;
-    const float* mask = p->rp > 0.f ? &placeholder : nullptr;
-    if (scan == 0) TRY(tc_scan_fwd(*p, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, mask, 0, geom));
-    else TRY(tc_scan_bwd(*p, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, mask, 0, geom));
-    *R = geom[0]; *n_split = geom[1];
-    return BIGRU_OK;
+    return tc_scan_geometry(*p, scan, R, n_split);
 }
 
 // where a forward or backward intermediate lives inside the stash or the scratch (test support; see the header for the
@@ -462,14 +455,15 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
                 j.b.zsel = 1;
                 TRY(wg_gemm(j, xp, false, wp, false, p.prec, st));
             }
+            ScanFwdOps o{};
+            o.gi = buf.gi; o.Whh = params + p.off_whh(l, 0); o.bhh = params + p.off_bhh(l, 0); o.h0 = h0l;
+            o.Y = Y; o.G = G; o.hn = hnl; o.len = len; o.mask = ml;
             // the scan's planes: Y's, or with recurrent dropout the masked state's (dW_hh reads them)
-            float* sp = rd ? buf.R[l] : buf.YP[l];
-            htc::bf16_t *yh = nullptr, *yl = nullptr;
-            if (sp) {
+            if (float* sp = rd ? buf.R[l] : buf.YP[l]) {
                 const Planes yp = plan_planes(p, sp, 0, (int64_t)D * H, BT, 1, (int64_t)D * H);
-                yh = mut(yp); yl = mut_lo(yp);
+                o.yh = mut(yp); o.yl = mut_lo(yp);
             }
-            TRY(tc_scan_fwd(p, l, buf.gi, params + p.off_whh(l, 0), params + p.off_bhh(l, 0), h0l, Y, G, hnl, yh, yl, len, ml, st));
+            TRY(tc_scan_fwd(p, l, o, st));
             if (rd && l + 1 < p.L && !own_planes(p, do_drop, l + 1)) {
                 // the next layer's projection and dW_ih read Y's planes, split from the fp32 Y as the scan splits its tile
                 const Planes yp = plan_planes(p, buf.YP[l], 0, (int64_t)D * H, BT, 1, (int64_t)D * H);
@@ -506,12 +500,8 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
                 r.mask_period = 1; r.mask_skip = 0;                           // every k masked -> pure bias
                 TRY(sgemm_launch(r, st));
             }
-            if (rd)
-                KLAUNCH(KC_GATES_FWD, 0.0, 0.0, st, gru_gates_fwd_rd_kernel<<<nblk(DBH, 256), 256, 0, st>>>(buf.gi, buf.gh, h0l, Y, G, hnl, B, T, H,
-                                                                                               D, s, len, ml, buf.R[l]));
-            else
-                KLAUNCH(KC_GATES_FWD, 0.0, 0.0, st, gru_gates_fwd_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(buf.gi, buf.gh, h0l, Y, G,
-                                                                              hnl, B, T, H, D, s, len));
+            KLAUNCH(KC_GATES_FWD, 0.0, 0.0, st, (rd ? gru_gates_fwd_kernel<true> : gru_gates_fwd_kernel<false>)<<<nblk(DBH, 256), 256, 0, st>>>(
+                                                    buf.gi, buf.gh, h0l, Y, G, hnl, B, T, H, D, s, len, ml, rd ? buf.R[l] : nullptr));
         }
         inp = Y;
     }
@@ -580,13 +570,14 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
         const Planes ghp = plan_planes(p, scratch, W.dghP, H3, BT, D, H3);
         // recurrence: dgi, dgh [D][B*T][3H] and dh0 in dhc
         if (tc) {
-            TRY(tc_scan_bwd(p, l, G, Y, h0l, dY, dhc, dgi, dgh, params + p.off_whh(l, 0), mut(gip), mut_lo(gip), mut(ghp), mut_lo(ghp), len, ml, st));
+            ScanBwdOps o{};
+            o.G = G; o.Y = Y; o.h0 = h0l; o.dY = dY; o.dhc = dhc; o.dgi = dgi; o.dgh = dgh; o.Whh = params + p.off_whh(l, 0);
+            o.gih = mut(gip); o.gil = mut_lo(gip); o.ghh = mut(ghp); o.ghl = mut_lo(ghp); o.len = len; o.mask = ml;
+            TRY(tc_scan_bwd(p, l, o, st));
         } else {
             for (int s = 0; s < T; ++s) {
-                if (rd)
-                    KLAUNCH(KC_GATES_BWD, 0.0, 0.0, st, gru_gates_bwd_rd_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(G, Y, h0l, dY, dhc, dgi, dgh, B, T, H, D, s, len, ml));
-                else
-                    KLAUNCH(KC_GATES_BWD, 0.0, 0.0, st, gru_gates_bwd_kernel<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(G, Y, h0l, dY, dhc, dgi, dgh, B, T, H, D, s, len));
+                KLAUNCH(KC_GATES_BWD, 0.0, 0.0, st, (rd ? gru_gates_bwd_kernel<true> : gru_gates_bwd_kernel<false>)<<<nblk((int64_t)D * B * H, 256), 256, 0, st>>>(
+                                                        G, Y, h0l, dY, dhc, dgi, dgh, B, T, H, D, s, len, ml));
                 // dhc[d] += dgh_t[d] W_hh[d]   (rows t: dir0 -> T-1-s, dir1 -> s)
                 const int t0 = T - 1 - s, t1 = s;
                 GemmArgs r = gemm_args(dgh + (int64_t)t0 * 3 * H, params + p.off_whh(l, 0), dhc, B, H, 3 * H,

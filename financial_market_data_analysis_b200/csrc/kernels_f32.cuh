@@ -217,17 +217,13 @@ __device__ __forceinline__ void gru_gates_fwd(const float* __restrict__ gi, cons
     if (hn_out && (d == 0 ? t == n_b - 1 : s == T - 1)) hn_out[((int64_t)d * B + b) * H + j] = h;
 }
 
+// M and R are null without RD
+template <bool RD>
 __global__ void gru_gates_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ gh,
                                      const float* __restrict__ h0, float* __restrict__ Y, float* __restrict__ G,
                                      float* __restrict__ hn_out, int B, int T, int H, int D, int s,
-                                     const int* __restrict__ len) {
-    gru_gates_fwd<false>(gi, gh, h0, Y, G, hn_out, B, T, H, D, s, len, nullptr, nullptr);
-}
-__global__ void gru_gates_fwd_rd_kernel(const float* __restrict__ gi, const float* __restrict__ gh,
-                                        const float* __restrict__ h0, float* __restrict__ Y, float* __restrict__ G,
-                                        float* __restrict__ hn_out, int B, int T, int H, int D, int s,
-                                        const int* __restrict__ len, const float* __restrict__ M, float* __restrict__ R) {
-    gru_gates_fwd<true>(gi, gh, h0, Y, G, hn_out, B, T, H, D, s, len, M, R);
+                                     const int* __restrict__ len, const float* __restrict__ M, float* __restrict__ R) {
+    gru_gates_fwd<RD>(gi, gh, h0, Y, G, hn_out, B, T, H, D, s, len, M, R);
 }
 
 // backward gates for one step: consumes dh carry + dY_t, emits dgi/dgh rows and dh*z.  At a padded (row, t >= len[b]):
@@ -281,18 +277,14 @@ __device__ __forceinline__ void gru_gates_bwd(const float* __restrict__ G, const
     dhc[ci] = dh * z;
 }
 
+// M is null without RD
+template <bool RD>
 __global__ void gru_gates_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y,
                                      const float* __restrict__ h0, const float* __restrict__ dY,
                                      float* __restrict__ dhc, float* __restrict__ dgi, float* __restrict__ dgh,
-                                     int B, int T, int H, int D, int s, const int* __restrict__ len) {
-    gru_gates_bwd<false>(G, Y, h0, dY, dhc, dgi, dgh, B, T, H, D, s, len, nullptr);
-}
-__global__ void gru_gates_bwd_rd_kernel(const float* __restrict__ G, const float* __restrict__ Y,
-                                        const float* __restrict__ h0, const float* __restrict__ dY,
-                                        float* __restrict__ dhc, float* __restrict__ dgi, float* __restrict__ dgh,
-                                        int B, int T, int H, int D, int s, const int* __restrict__ len,
-                                        const float* __restrict__ M) {
-    gru_gates_bwd<true>(G, Y, h0, dY, dhc, dgi, dgh, B, T, H, D, s, len, M);
+                                     int B, int T, int H, int D, int s, const int* __restrict__ len,
+                                     const float* __restrict__ M) {
+    gru_gates_bwd<RD>(G, Y, h0, dY, dhc, dgi, dgh, B, T, H, D, s, len, M);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -635,38 +635,24 @@ __device__ __forceinline__ void gru_scan_fwd_tile(const float* __restrict__ gi, 
     cluster_wait();
 }
 
-template <int H, int NS, int OUT, bool LEN>
+// RD: recurrent dropout, in the training forward only (SCAN_TRAIN outputs): yh, yl receive the masked state, not Y.  mask is
+// null without RD
+template <int H, int NS, int OUT, bool LEN, bool RD>
 __global__ void __launch_bounds__(SCAN_THREADS, 1)
 gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh, const float* __restrict__ bhh, int64_t zW,
                     const float* __restrict__ h0, float* __restrict__ Y, float* __restrict__ G, float* __restrict__ hn_out,
-                    bf16_t* __restrict__ yh, bf16_t* __restrict__ yl, int B, int T, int D, int m2, const int* __restrict__ lens) {
+                    bf16_t* __restrict__ yh, bf16_t* __restrict__ yl, int B, int T, int D, int m2, const int* __restrict__ lens,
+                    const float* __restrict__ mask) {
+    static_assert(!RD || OUT == SCAN_TRAIN, "recurrent dropout runs in the training forward only");
     int d, bt0, nb;
     scan_tile(blockIdx.y, m2, B / SCAN_NB, D, d, bt0, nb);
     if constexpr (FwdSmem<H, NS>::NBMAX == 2 * SCAN_NB) {
         if (nb == 2 * SCAN_NB) {
-            gru_scan_fwd_tile<H, NS, OUT, LEN, 2>(gi, Whh, bhh, zW, h0, Y, G, hn_out, yh, yl, B, T, D, lens, d, bt0);
+            gru_scan_fwd_tile<H, NS, OUT, LEN, 2, RD>(gi, Whh, bhh, zW, h0, Y, G, hn_out, yh, yl, B, T, D, lens, d, bt0, mask);
             return;
         }
     }
-    gru_scan_fwd_tile<H, NS, OUT, LEN, 1>(gi, Whh, bhh, zW, h0, Y, G, hn_out, yh, yl, B, T, D, lens, d, bt0);
-}
-
-// the training forward with recurrent dropout (SCAN_TRAIN outputs): yh, yl receive the masked state, not Y
-template <int H, int NS, bool LEN>
-__global__ void __launch_bounds__(SCAN_THREADS, 1)
-gru_scan_fwd_rd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh, const float* __restrict__ bhh, int64_t zW,
-                       const float* __restrict__ h0, float* __restrict__ Y, float* __restrict__ G, float* __restrict__ hn_out,
-                       bf16_t* __restrict__ yh, bf16_t* __restrict__ yl, int B, int T, int D, int m2, const int* __restrict__ lens,
-                       const float* __restrict__ mask) {
-    int d, bt0, nb;
-    scan_tile(blockIdx.y, m2, B / SCAN_NB, D, d, bt0, nb);
-    if constexpr (FwdSmem<H, NS>::NBMAX == 2 * SCAN_NB) {
-        if (nb == 2 * SCAN_NB) {
-            gru_scan_fwd_tile<H, NS, SCAN_TRAIN, LEN, 2, true>(gi, Whh, bhh, zW, h0, Y, G, hn_out, yh, yl, B, T, D, lens, d, bt0, mask);
-            return;
-        }
-    }
-    gru_scan_fwd_tile<H, NS, SCAN_TRAIN, LEN, 1, true>(gi, Whh, bhh, zW, h0, Y, G, hn_out, yh, yl, B, T, D, lens, d, bt0, mask);
+    gru_scan_fwd_tile<H, NS, OUT, LEN, 1, RD>(gi, Whh, bhh, zW, h0, Y, G, hn_out, yh, yl, B, T, D, lens, d, bt0, mask);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -905,39 +891,23 @@ __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, c
 // tile) order; the last L8 tiles are split into two 8-row clusters each (scan_bwd_geometry), so a short last round of
 // clusters takes less time.  An 8-row cluster multiplies one n8 block with the same MMA sequence per element: a row's bits
 // do not depend on its tile.
-template <int H, int NS, bool LEN>
+// RD: the backward of the recurrent-dropout forward: Y is the unmasked output; the dgh planes pair with the masked-state
+// planes.  mask is null without RD
+template <int H, int NS, bool LEN, bool RD>
 __global__ void __launch_bounds__(SCAN_THREADS, 1)
 gru_scan_bwd_kernel(const float* __restrict__ G, const float* __restrict__ Y, const float* __restrict__ h0,
                     const float* __restrict__ dY, float* __restrict__ dhc, float* __restrict__ dgi, float* __restrict__ dgh,
                     const float* __restrict__ Whh, int64_t zW, bf16_t* __restrict__ gih, bf16_t* __restrict__ gil,
-                    bf16_t* __restrict__ ghh, bf16_t* __restrict__ ghl, int B, int T, int D, int L8, const int* __restrict__ lens) {
+                    bf16_t* __restrict__ ghh, bf16_t* __restrict__ ghl, int B, int T, int D, int L8, const int* __restrict__ lens,
+                    const float* __restrict__ mask) {
     const int ntd = B / SCAN_NB, n16 = D * ntd - L8, q = blockIdx.y;
     if (q < n16) {
-        gru_scan_bwd_tile<H, NS, LEN, SCAN_NB>(G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, lens, q / ntd,
-                                                (q % ntd) * SCAN_NB);
+        gru_scan_bwd_tile<H, NS, LEN, SCAN_NB, RD>(G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, lens,
+                                                    q / ntd, (q % ntd) * SCAN_NB, mask);
     } else {
         const int f = n16 + (q - n16) / 2;
-        gru_scan_bwd_tile<H, NS, LEN, SCAN_NB / 2>(G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, lens,
-                                                    f / ntd, (f % ntd) * SCAN_NB + ((q - n16) & 1) * (SCAN_NB / 2));
-    }
-}
-
-// the backward of gru_scan_fwd_rd_kernel: Y is the unmasked output; the dgh planes pair with the masked-state planes
-template <int H, int NS, bool LEN>
-__global__ void __launch_bounds__(SCAN_THREADS, 1)
-gru_scan_bwd_rd_kernel(const float* __restrict__ G, const float* __restrict__ Y, const float* __restrict__ h0,
-                       const float* __restrict__ dY, float* __restrict__ dhc, float* __restrict__ dgi, float* __restrict__ dgh,
-                       const float* __restrict__ Whh, int64_t zW, bf16_t* __restrict__ gih, bf16_t* __restrict__ gil,
-                       bf16_t* __restrict__ ghh, bf16_t* __restrict__ ghl, int B, int T, int D, int L8, const int* __restrict__ lens,
-                       const float* __restrict__ mask) {
-    const int ntd = B / SCAN_NB, n16 = D * ntd - L8, q = blockIdx.y;
-    if (q < n16) {
-        gru_scan_bwd_tile<H, NS, LEN, SCAN_NB, true>(G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, lens,
-                                                      q / ntd, (q % ntd) * SCAN_NB, mask);
-    } else {
-        const int f = n16 + (q - n16) / 2;
-        gru_scan_bwd_tile<H, NS, LEN, SCAN_NB / 2, true>(G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, lens,
-                                                          f / ntd, (f % ntd) * SCAN_NB + ((q - n16) & 1) * (SCAN_NB / 2), mask);
+        gru_scan_bwd_tile<H, NS, LEN, SCAN_NB / 2, RD>(G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, lens,
+                                                        f / ntd, (f % ntd) * SCAN_NB + ((q - n16) & 1) * (SCAN_NB / 2), mask);
     }
 }
 
@@ -1148,65 +1118,6 @@ static void scan_geometry(int R, bool two, int B, int D, int* m2, int* clusters)
     *clusters = n - n2;
 }
 
-template <int HH, int NS, bool LEN>
-static int scan_fwd_launch(int out, int cs, int B, int D, cudaStream_t st, const float* gi, const float* Whh, const float* bhh,
-                           int64_t zW, const float* h0, float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, int T,
-                           const int* len, const float* mask, int* geom) {
-    constexpr int smem = htc::FwdSmem<HH, NS>::TOTAL;
-    if (mask) {
-        if (out != htc::SCAN_TRAIN) { bigru_set_error("tc_scan_fwd: recurrent dropout runs in the training forward only"); return BIGRU_ERR_ARG; }
-        auto k = htc::gru_scan_fwd_rd_kernel<HH, NS, LEN>;
-        int R = 0, m2 = 0, clusters = 0;
-        TRY(cluster_residency(k, cs, smem, &R));
-        scan_geometry(R, htc::FwdSmem<HH, NS>::NBMAX == 2 * htc::SCAN_NB, B, D, &m2, &clusters);
-        if (geom) { geom[0] = R; geom[1] = D * m2; return BIGRU_OK; }
-        ProfScope ps(KC_TC_SCAN_FWD, 2.0 * D * B * (double)T * 3 * HH * HH, 0.0, st);
-        return launch_cluster(k, cs, clusters, 1, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D, m2, len, mask);
-    }
-    void (*k)(const float*, const float*, const float*, int64_t, const float*, float*, float*, float*, htc::bf16_t*, htc::bf16_t*,
-              int, int, int, int, const int*) = nullptr;
-    switch (out) {
-        case htc::SCAN_TRAIN: k = htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_TRAIN, LEN>; break;
-        case htc::SCAN_INFER_LOWER: k = htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_INFER_LOWER, LEN>; break;
-        case htc::SCAN_INFER_TOP: k = htc::gru_scan_fwd_kernel<HH, NS, htc::SCAN_INFER_TOP, LEN>; break;
-        default:
-            bigru_set_error("tc_scan_fwd: no kernel writes this set of outputs (Y %d, G %d, planes %d)", Y != nullptr, G != nullptr, yh != nullptr);
-            return BIGRU_ERR_ARG;
-    }
-    int R = 0, m2 = 0, clusters = 0;
-    TRY(cluster_residency(k, cs, smem, &R));
-    scan_geometry(R, htc::FwdSmem<HH, NS>::NBMAX == 2 * htc::SCAN_NB, B, D, &m2, &clusters);
-    if (geom) { geom[0] = R; geom[1] = D * m2; return BIGRU_OK; }
-    ProfScope ps(KC_TC_SCAN_FWD, 2.0 * D * B * (double)T * 3 * HH * HH, 0.0, st);
-    return launch_cluster(k, cs, clusters, 1, smem, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, B, T, D, m2, len);
-}
-
-// one layer's forward recurrence; shapes were validated by the plan (H in {128, 256, 512}, B % 16 == 0).  A null Y, G or yh:
-// that output is not written (the instantiations: all three, planes only, Y only).  len: per-row lengths [B] or null.
-// mask: the layer's recurrent-dropout masks [D][B][H] (training outputs only; yh, yl then get the masked state) or null.
-// geom non-null: launch nothing and return the training instantiation's residency R and two-tile cluster count n2 in
-// geom[0], geom[1] (test support); with a mask, those of the recurrent-dropout kernel (the mask is not read)
-static int tc_scan_fwd(const bigru_plan& p, int l, const float* gi, const float* Whh, const float* bhh, const float* h0,
-                       float* Y, float* G, float* hn, htc::bf16_t* yh, htc::bf16_t* yl, const int* len, const float* mask,
-                       cudaStream_t st, int* geom = nullptr) {
-    const int H = p.H, D = p.D, B = p.B, T = p.T, cs = H / htc::SCAN_U;
-    const int64_t zW = p.ld_block(l);
-    const int out = geom ? htc::SCAN_TRAIN : (Y ? htc::SCAN_Y : 0) | (G ? htc::SCAN_G : 0) | (yh ? htc::SCAN_PLANES : 0);
-#define FWD(HH, NS) return len ? scan_fwd_launch<HH, NS, true>(out, cs, B, D, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, T, len, mask, geom) \
-                               : scan_fwd_launch<HH, NS, false>(out, cs, B, D, st, gi, Whh, bhh, zW, h0, Y, G, hn, yh, yl, T, len, mask, geom)
-    if (p.prec == BIGRU_PREC_BF16X3) {
-        if (H == 128) FWD(128, 3);
-        if (H == 256) FWD(256, 3);
-    } else {
-        if (H == 128) FWD(128, 1);
-        if (H == 256) FWD(256, 1);
-        if (H == 512) FWD(512, 1);
-    }
-#undef FWD
-    bigru_set_error("tc_scan_fwd: no kernel for H=%d at precision %d", H, p.prec);
-    return BIGRU_ERR_UNSUPPORTED;
-}
-
 // Backward scan geometry.  n = D * B / 16 tiles; R clusters fit at once.  With rounds = ceil(n / R) > 1, the last round
 // holds L = n - (rounds - 1) * R tiles; when 2L <= R they run as 2L clusters of 8 rows, which take less time than L of 16.
 // Results do not depend on the geometry.  Returns L8 = the split tiles and the cluster count.
@@ -1216,47 +1127,112 @@ static void scan_bwd_geometry(int R, int B, int D, int* L8, int* clusters) {
     *clusters = n + *L8;
 }
 
+// the scan kernels of one (precision, H, forward outputs, lengths, recurrent dropout).  All instantiations of a direction
+// share one signature: the mask operand is null without recurrent dropout
+typedef decltype(&htc::gru_scan_fwd_kernel<128, 1, htc::SCAN_TRAIN, false, false>) ScanFwdFn;
+typedef decltype(&htc::gru_scan_bwd_kernel<128, 1, false, false>) ScanBwdFn;
+struct ScanKernels {
+    ScanFwdFn fwd; int fwd_smem; bool two;   // two: the forward has 32-row tiles
+    ScanBwdFn bwd; int bwd_smem;
+};
+
 template <int HH, int NS, bool LEN>
-static int scan_bwd_launch(int cs, int B, int D, cudaStream_t st, const float* G, const float* Y, const float* h0, const float* dY,
-                           float* dhc, float* dgi, float* dgh, const float* Whh, int64_t zW, htc::bf16_t* gih, htc::bf16_t* gil,
-                           htc::bf16_t* ghh, htc::bf16_t* ghl, int T, const int* len, const float* mask, int* geom) {
-    constexpr int smem = htc::BwdSmem<HH, NS>::TOTAL;
-    if (mask) {
-        auto k = htc::gru_scan_bwd_rd_kernel<HH, NS, LEN>;
-        int R = 0, L8 = 0, clusters = 0;
-        TRY(cluster_residency(k, cs, smem, &R));
-        scan_bwd_geometry(R, B, D, &L8, &clusters);
-        if (geom) { geom[0] = R; geom[1] = L8; return BIGRU_OK; }
-        ProfScope ps(KC_TC_SCAN_BWD, 2.0 * D * B * (double)T * 3 * HH * HH, 0.0, st);
-        return launch_cluster(k, cs, clusters, 1, smem, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, L8, len, mask);
-    }
-    auto k = htc::gru_scan_bwd_kernel<HH, NS, LEN>;
-    int R = 0, L8 = 0, clusters = 0;
-    TRY(cluster_residency(k, cs, smem, &R));
-    scan_bwd_geometry(R, B, D, &L8, &clusters);
-    if (geom) { geom[0] = R; geom[1] = L8; return BIGRU_OK; }
-    ProfScope ps(KC_TC_SCAN_BWD, 2.0 * D * B * (double)T * 3 * HH * HH, 0.0, st);
-    return launch_cluster(k, cs, clusters, 1, smem, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, B, T, D, L8, len);
+static ScanKernels scan_instance(int out, bool rd) {
+    using namespace htc;
+    const ScanFwdFn fwd = rd                        ? gru_scan_fwd_kernel<HH, NS, SCAN_TRAIN, LEN, true>
+                          : out == SCAN_TRAIN       ? gru_scan_fwd_kernel<HH, NS, SCAN_TRAIN, LEN, false>
+                          : out == SCAN_INFER_LOWER ? gru_scan_fwd_kernel<HH, NS, SCAN_INFER_LOWER, LEN, false>
+                                                    : gru_scan_fwd_kernel<HH, NS, SCAN_INFER_TOP, LEN, false>;
+    const ScanBwdFn bwd = rd ? gru_scan_bwd_kernel<HH, NS, LEN, true> : gru_scan_bwd_kernel<HH, NS, LEN, false>;
+    return {fwd, FwdSmem<HH, NS>::TOTAL, FwdSmem<HH, NS>::NBMAX == 2 * SCAN_NB, bwd, BwdSmem<HH, NS>::TOTAL};
 }
 
-// one layer's backward recurrence; mask as in tc_scan_fwd; geom as in tc_scan_fwd (geom[1]: the tiles split into two 8-row
-// clusters)
-static int tc_scan_bwd(const bigru_plan& p, int l, const float* G, const float* Y, const float* h0, const float* dY, float* dhc,
-                       float* dgi, float* dgh, const float* Whh, htc::bf16_t* gih, htc::bf16_t* gil, htc::bf16_t* ghh,
-                       htc::bf16_t* ghl, const int* len, const float* mask, cudaStream_t st, int* geom = nullptr) {
-    const int H = p.H, D = p.D, B = p.B, T = p.T, cs = H / htc::SCAN_U;
-    const int64_t zW = p.ld_block(l);
-#define BWD(HH, NS) return len ? scan_bwd_launch<HH, NS, true>(cs, B, D, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, T, len, mask, geom) \
-                           : scan_bwd_launch<HH, NS, false>(cs, B, D, st, G, Y, h0, dY, dhc, dgi, dgh, Whh, zW, gih, gil, ghh, ghl, T, len, mask, geom)
-    if (p.prec == BIGRU_PREC_BF16X3) {
-        if (H == 128) BWD(128, 3);
-        if (H == 256) BWD(256, 3);
-    } else {
-        if (H == 128) BWD(128, 1);
-        if (H == 256) BWD(256, 1);
-        if (H == 512) BWD(512, 1);
+// the scan kernels of plan p whose forward writes the outputs `out` (the backward's are those of SCAN_TRAIN); shapes were
+// validated by the plan (H in {128, 256, 512}, B % 16 == 0)
+static int scan_kernels(const bigru_plan& p, int out, bool len, bool rd, ScanKernels* k) {
+    using namespace htc;
+    if (rd && out != SCAN_TRAIN) { bigru_set_error("tc_scan: recurrent dropout runs in the training forward only"); return BIGRU_ERR_ARG; }
+    if (out != SCAN_TRAIN && out != SCAN_INFER_LOWER && out != SCAN_INFER_TOP) {
+        bigru_set_error("tc_scan: no kernel writes this set of outputs (Y %d, G %d, planes %d)", (out & SCAN_Y) != 0,
+                        (out & SCAN_G) != 0, (out & SCAN_PLANES) != 0);
+        return BIGRU_ERR_ARG;
     }
-#undef BWD
-    bigru_set_error("tc_scan_bwd: no kernel for H=%d at precision %d", H, p.prec);
-    return BIGRU_ERR_UNSUPPORTED;
+    const bool x3 = p.prec == BIGRU_PREC_BF16X3;
+    if (x3 && p.H == 128) *k = len ? scan_instance<128, 3, true>(out, rd) : scan_instance<128, 3, false>(out, rd);
+    else if (x3 && p.H == 256) *k = len ? scan_instance<256, 3, true>(out, rd) : scan_instance<256, 3, false>(out, rd);
+    else if (!x3 && p.H == 128) *k = len ? scan_instance<128, 1, true>(out, rd) : scan_instance<128, 1, false>(out, rd);
+    else if (!x3 && p.H == 256) *k = len ? scan_instance<256, 1, true>(out, rd) : scan_instance<256, 1, false>(out, rd);
+    else if (!x3 && p.H == 512) *k = len ? scan_instance<512, 1, true>(out, rd) : scan_instance<512, 1, false>(out, rd);
+    else {
+        bigru_set_error("tc_scan: no kernel for H=%d at precision %d", p.H, p.prec);
+        return BIGRU_ERR_UNSUPPORTED;
+    }
+    return BIGRU_OK;
+}
+
+// the operands of one layer's forward recurrence.  A null Y, G or yh: that output is not written (the instantiations: all
+// three, planes only, Y only).  len: per-row lengths [B] or null.  mask: the layer's recurrent-dropout masks [D][B][H]
+// (training outputs only; yh, yl then get the masked state) or null
+struct ScanFwdOps {
+    const float *gi, *Whh, *bhh, *h0;
+    float *Y, *G, *hn;
+    htc::bf16_t *yh, *yl;
+    const int* len;
+    const float* mask;
+};
+
+static int tc_scan_fwd(const bigru_plan& p, int l, const ScanFwdOps& o, cudaStream_t st) {
+    using namespace htc;
+    const int out = (o.Y ? SCAN_Y : 0) | (o.G ? SCAN_G : 0) | (o.yh ? SCAN_PLANES : 0);
+    ScanKernels k;
+    TRY(scan_kernels(p, out, o.len != nullptr, o.mask != nullptr, &k));
+    const int cs = p.H / SCAN_U;
+    int R = 0, m2 = 0, clusters = 0;
+    TRY(cluster_residency(k.fwd, cs, k.fwd_smem, &R));
+    scan_geometry(R, k.two, p.B, p.D, &m2, &clusters);
+    ProfScope ps(KC_TC_SCAN_FWD, 2.0 * p.D * p.B * (double)p.T * 3 * p.H * p.H, 0.0, st);
+    return launch_cluster(k.fwd, cs, clusters, 1, k.fwd_smem, st, o.gi, o.Whh, o.bhh, p.ld_block(l), o.h0, o.Y, o.G, o.hn, o.yh,
+                          o.yl, p.B, p.T, p.D, m2, o.len, o.mask);
+}
+
+// the operands of one layer's backward recurrence; len and mask as in ScanFwdOps
+struct ScanBwdOps {
+    const float *G, *Y, *h0, *dY;
+    float *dhc, *dgi, *dgh;
+    const float* Whh;
+    htc::bf16_t *gih, *gil, *ghh, *ghl;
+    const int* len;
+    const float* mask;
+};
+
+static int tc_scan_bwd(const bigru_plan& p, int l, const ScanBwdOps& o, cudaStream_t st) {
+    ScanKernels k;
+    TRY(scan_kernels(p, htc::SCAN_TRAIN, o.len != nullptr, o.mask != nullptr, &k));
+    const int cs = p.H / htc::SCAN_U;
+    int R = 0, L8 = 0, clusters = 0;
+    TRY(cluster_residency(k.bwd, cs, k.bwd_smem, &R));
+    scan_bwd_geometry(R, p.B, p.D, &L8, &clusters);
+    ProfScope ps(KC_TC_SCAN_BWD, 2.0 * p.D * p.B * (double)p.T * 3 * p.H * p.H, 0.0, st);
+    return launch_cluster(k.bwd, cs, clusters, 1, k.bwd_smem, st, o.G, o.Y, o.h0, o.dY, o.dhc, o.dgi, o.dgh, o.Whh, p.ld_block(l),
+                          o.gih, o.gil, o.ghh, o.ghl, p.B, p.T, p.D, L8, o.len, o.mask);
+}
+
+// plan p's layer scans without lengths, training outputs, with recurrent dropout when the plan has it (test support): the
+// clusters R the device holds at once, and n_split, the tiles in two-tile clusters (scan 0, forward) or split into two
+// 8-row clusters (scan 1, backward)
+static int tc_scan_geometry(const bigru_plan& p, int scan, int* R, int* n_split) {
+    ScanKernels k;
+    TRY(scan_kernels(p, htc::SCAN_TRAIN, false, p.rp > 0.f, &k));
+    const int cs = p.H / htc::SCAN_U;
+    int r = 0, m2 = 0, clusters = 0;
+    if (scan == 0) {
+        TRY(cluster_residency(k.fwd, cs, k.fwd_smem, &r));
+        scan_geometry(r, k.two, p.B, p.D, &m2, &clusters);
+        *n_split = p.D * m2;
+    } else {
+        TRY(cluster_residency(k.bwd, cs, k.bwd_smem, &r));
+        scan_bwd_geometry(r, p.B, p.D, n_split, &clusters);
+    }
+    *R = r;
+    return BIGRU_OK;
 }
