@@ -1,5 +1,6 @@
 """Drives the library's C ABI on one plan and takes the result apart tensor by tensor.  Test infrastructure, shared by
-test_gpu_rounding_model.py, test_gpu_fp32_path.py, test_gpu_tc_steps.py, test_gpu_scan_tiles.py and test_gpu_rd_steps.py.
+test_gpu_rounding_model.py, test_gpu_fp32_path.py, test_gpu_tc_steps.py, test_gpu_scan_tiles.py, test_gpu_rd_steps.py and
+test_gpu_gru_steps.py.
 
 A shape is a dict with B, T, F, H, L, C, D (1 or 2) and h0 (bool).  `kernel` runs bigru_forward and bigru_backward at a
 precision ("fp32", "bf16" or "bf16x3"), optionally with dropout, recurrent dropout and per-sequence lengths, and returns
@@ -8,7 +9,9 @@ backward's intermediates, read through bigru_workspace_region).  `tensors` / `ke
 recomputes one forward step from the kernel's own state, `backward_steps` / `gemm_steps` each backward step of layer 0
 and each backward GEMM from the kernel's own operands, `plane_checks` the bf16 planes bit for bit, `dist` measures two
 tensors.  The models take optional recurrent-dropout masks and lengths (DESIGN.md §4.8, §4.5); without them they are the
-models of the plain path, operation for operation."""
+models of the plain path, operation for operation.  With head=False the plan is a head-less one (bigru_gru_*, the nn.GRU
+drop-in): the top layer's output and upstream gradient are the caller's y and dy, each layer's carry starts from the
+caller's dhn, and there are no logits, pooling routing, dcat or head GEMMs."""
 import ctypes as C
 
 import numpy as np
@@ -43,12 +46,12 @@ def dropout_mask(seed, layer, B, T, I, p, spatial=False):
     return np.where(bigru_uniform(seed, layer, key).astype(np.float32) < p32, np.float32(0), scale).astype(np.float32)
 
 
-def param_names(plan, s):
-    """name -> (offset, size) of every parameter block, from bigru_param_offset."""
+def param_names(plan, s, head=True):
+    """name -> (offset, size) of every parameter block, from bigru_param_offset (head=False: a plan without lin_w, lin_b)."""
     lib = _pkg()._lib.load()
     out = {}
     off, rows, cols = C.c_int64(), C.c_int64(), C.c_int64()
-    for l in range(s["L"] + 1):
+    for l in range(s["L"] + int(head)):
         for d in range(s["D"] if l < s["L"] else 1):
             for which, nm in enumerate(("w_ih", "w_hh", "b_ih", "b_hh")):
                 if l == s["L"] and which in (1, 3):
@@ -91,11 +94,12 @@ def _bits_to_f32(u16):
     return (u16.astype(np.uint32) << np.uint32(16)).view(np.float32)
 
 
-def _workspace(plan, s, prec, stash, scratch, rd=False):
+def _workspace(plan, s, prec, stash, scratch, rd=False, head=True):
     """The backward's operands and intermediates (bigru_workspace_region) as host arrays: fp32 regions as float32, planes
     as (hi, lo) pairs of bf16 bit patterns (uint16; lo None at bf16; both None at fp32, which keeps no planes).  Rows are
     split into [B, T] (and a leading D where there is one).  rd: also every layer's recurrent-dropout masks RDM [D, B, H]
-    and masked state RDS [B, T, D*H] (planes, or float32 at fp32)."""
+    and masked state RDS [B, T, D*H] (planes, or float32 at fp32).  head=False: DCAT and the top layer's DY, which a
+    head-less plan refuses (its top layer's upstream gradient is the caller's dy), are None."""
     B, T, F, H, L, D = (s[k] for k in "BTFHLD")
     bufs = (stash, scratch)
 
@@ -119,8 +123,8 @@ def _workspace(plan, s, prec, stash, scratch, rd=False):
               XP=planes("IN_PLANES", 0, (B, T, pitch0)),
               DGI=f32("DGI", 0, (D, B, T, 3 * H)), DGH=f32("DGH", 0, (D, B, T, 3 * H)),
               DGIP=planes("DGI_PLANES", 0, (D, B, T, 3 * H)), DGHP=planes("DGH_PLANES", 0, (D, B, T, 3 * H)),
-              DY=[f32("DY", l, (B, T, D * H)) for l in range(min(L, 2))],
-              DHC=f32("DHC", 0, (D, B, H)), DCAT=f32("DCAT", L, (B, 3 * H)))
+              DY=[f32("DY", l, (B, T, D * H)) if head or l < L - 1 else None for l in range(min(L, 2))],
+              DHC=f32("DHC", 0, (D, B, H)), DCAT=f32("DCAT", L, (B, 3 * H)) if head else None)
     if rd:
         ws["RDM"] = [f32("RD_MASK", l, (D, B, H)) for l in range(L)]
         ws["RDS"] = [(f32("RD_STATE", l, (B, T, D * H)), None) if prec == "fp32" else planes("RD_STATE", l, (B, T, D * H))
@@ -128,15 +132,23 @@ def _workspace(plan, s, prec, stash, scratch, rd=False):
     return ws
 
 
-def kernel(s, prec, flat, x, h0, dl, p=0.0, spatial=False, seed=0, regions=False, rd_p=0.0, lens=None):
+def kernel(s, prec, flat, x, h0, dl, p=0.0, spatial=False, seed=0, regions=False, rd_p=0.0, lens=None, head=True, dy=None,
+           dhn=None):
     """bigru_forward_lengths + bigru_backward_lengths of shape s at precision prec on a bigru_plan_create_rd plan (p = 0:
     bigru_plan_create's plan); dropout p and recurrent dropout rd_p (training mode when either is on); lens: per-row
-    lengths [B] or None.  regions: the result also holds "ws", the intermediates of _workspace."""
+    lengths [B] or None.  regions: the result also holds "ws", the intermediates of _workspace.
+    head=False: bigru_gru_forward + bigru_gru_backward on a bigru_gru_plan_create_rd plan (flat is the recurrent prefix, dl
+    and spatial are unused, p drops only between layers).  dy [B, T, D*H] is the gradient of the top layer's output (None:
+    zeros, as GRU passes it), dhn [L*D, B, H] that of h_n (None: no gradient).  ys then takes the top layer from d_y, and
+    the result has no logits and no arg."""
     pkg = _pkg()
     lib, L_ = pkg._lib.load(), pkg._lib
     B, T, F, H, L, C_, D = (s[k] for k in "BTFHLCD")
     plan = C.c_void_p()
-    L_.check(lib.bigru_plan_create_rd(B, T, F, H, L, C_, int(D == 2), CODE[prec], rd_p, C.byref(plan)), "plan_create")
+    if head:
+        L_.check(lib.bigru_plan_create_rd(B, T, F, H, L, C_, int(D == 2), CODE[prec], rd_p, C.byref(plan)), "plan_create")
+    else:
+        L_.check(lib.bigru_gru_plan_create_rd(B, T, F, H, L, int(D == 2), CODE[prec], rd_p, C.byref(plan)), "gru_plan_create")
     try:
         sb, cb = C.c_size_t(), C.c_size_t()
         L_.check(lib.bigru_workspace_bytes(plan, C.byref(sb), C.byref(cb)), "workspace_bytes")
@@ -145,30 +157,45 @@ def kernel(s, prec, flat, x, h0, dl, p=0.0, spatial=False, seed=0, regions=False
         scratch = torch.zeros(cb.value // 4, dtype=torch.float32, device=dev)
         pd, xd = torch.from_numpy(flat).to(dev), torch.from_numpy(x).to(dev)
         h0d = None if h0 is None else torch.from_numpy(h0).to(dev)
-        logits = torch.zeros(B, C_, device=dev)
+        logits = torch.zeros(B, C_, device=dev) if head else None
+        y = None if head else torch.zeros(B, T, D * H, device=dev)
         hn = torch.zeros(L * D, B, H, device=dev)
         st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
         ptr = L_.ptr
         train = int(p > 0 or rd_p > 0)
         lend = None if lens is None else torch.from_numpy(np.asarray(lens, np.int32)).to(dev)
-        L_.check(lib.bigru_forward_lengths(plan, ptr(pd), ptr(xd), ptr(h0d), p, int(spatial), train, seed, ptr(stash),
-                                           ptr(scratch), ptr(logits), ptr(hn), ptr(lend), st), "forward")
+        if head:
+            L_.check(lib.bigru_forward_lengths(plan, ptr(pd), ptr(xd), ptr(h0d), p, int(spatial), train, seed, ptr(stash),
+                                               ptr(scratch), ptr(logits), ptr(hn), ptr(lend), st), "forward")
+        else:
+            L_.check(lib.bigru_gru_forward(plan, ptr(pd), ptr(xd), ptr(h0d), p, train, seed, ptr(stash), ptr(scratch), ptr(y),
+                                           ptr(hn), ptr(lend), st), "gru_forward")
         off = C.c_size_t()
         ys = []
-        for l in range(L):
+        for l in range(L if head else L - 1):
             L_.check(lib.bigru_stash_output_offset(plan, l, C.byref(off)), "stash_output_offset")
             ys.append(stash[off.value // 4: off.value // 4 + B * T * D * H].view(B, T, D * H).cpu().numpy().astype(np.float64))
-        L_.check(lib.bigru_stash_argmax_offset(plan, C.byref(off)), "stash_argmax_offset")
-        arg = stash.view(torch.int32)[off.value // 4: off.value // 4 + B * H].view(B, H).cpu().numpy().astype(np.int64)
+        arg = None
+        if head:
+            L_.check(lib.bigru_stash_argmax_offset(plan, C.byref(off)), "stash_argmax_offset")
+            arg = stash.view(torch.int32)[off.value // 4: off.value // 4 + B * H].view(B, H).cpu().numpy().astype(np.int64)
+        else:
+            ys.append(y.cpu().numpy().astype(np.float64))
         grads = torch.zeros(flat.size, device=dev)
         dx = torch.zeros(B, T, F, device=dev)
         dh0 = torch.zeros(L * D, B, H, device=dev) if h0 is not None else None
-        dld = torch.from_numpy(dl).to(dev)                      # alive until the synchronize below: the backward reads it
-        L_.check(lib.bigru_backward_lengths(plan, ptr(pd), ptr(xd), ptr(h0d), p, int(spatial), train, seed, ptr(stash),
-                                            ptr(scratch), ptr(dld), ptr(grads), ptr(dx), ptr(dh0), ptr(lend), st), "backward")
+        if head:
+            dld = torch.from_numpy(dl).to(dev)                  # alive until the synchronize below: the backward reads it
+            L_.check(lib.bigru_backward_lengths(plan, ptr(pd), ptr(xd), ptr(h0d), p, int(spatial), train, seed, ptr(stash),
+                                                ptr(scratch), ptr(dld), ptr(grads), ptr(dx), ptr(dh0), ptr(lend), st), "backward")
+        else:
+            dyd = torch.zeros(B, T, D * H, device=dev) if dy is None else torch.from_numpy(np.asarray(dy, np.float32)).to(dev)
+            dhnd = None if dhn is None else torch.from_numpy(np.asarray(dhn, np.float32)).to(dev)
+            L_.check(lib.bigru_gru_backward(plan, ptr(pd), ptr(xd), ptr(h0d), p, train, seed, ptr(stash), ptr(scratch), ptr(y),
+                                            ptr(dyd), ptr(dhnd), ptr(grads), ptr(dx), ptr(dh0), ptr(lend), st), "gru_backward")
         torch.cuda.synchronize()
-        names = param_names(plan, s)
-        ws = _workspace(plan, s, prec, stash, scratch, rd=rd_p > 0) if regions else None
+        names = param_names(plan, s, head)
+        ws = _workspace(plan, s, prec, stash, scratch, rd=rd_p > 0, head=head) if regions else None
         del stash, scratch
     finally:
         lib.bigru_plan_destroy(plan)
@@ -247,7 +274,7 @@ def _masked(m, v, prec):
     return (np.asarray(m, np.float32) * np.asarray(v, np.float32)).astype(np.float64)
 
 
-def stepwise(s, prec, flat, x, h0, dl, got, names, rows=None, gates=False, masks=None, lens=None, drops=None):
+def stepwise(s, prec, flat, x, h0, dl, got, names, rows=None, gates=False, masks=None, lens=None, drops=None, head=True):
     """The model at `prec` (mm's) run one step at a time from the kernel's own state: every step of every layer starts
     from the kernel's h_{t-1} (its Y, or h0) and the kernel's layer input (x, or the previous layer's Y), the head from
     the kernel's top-layer Y.  Rounding flips cannot compound, so what is left of the kernel's distance is the arithmetic
@@ -257,7 +284,8 @@ def stepwise(s, prec, flat, x, h0, dl, got, names, rows=None, gates=False, masks
     W_hn h_{t-1} + b_hn, which the forward scan stashes for the backward.
     masks: recurrent-dropout masks per layer [D, B, H] (DESIGN.md §4.8): gh and the carry take m * h_{t-1} (_masked).
     lens: per-row lengths [B]: a padded (row, t) has Y = 0 and no G (0 in the zeroed stash); the head pools valid steps.
-    drops: per layer None or the float32 factor dropout_kernel multiplies that layer's input by."""
+    drops: per layer None or the float32 factor dropout_kernel multiplies that layer's input by.  head=False: no logits and
+    no lin_w gradient (dl is unused)."""
     B, T, H, L, C_, D = (s[k] for k in "BTHLCD")
     rows = np.arange(B) if rows is None else np.asarray(rows)
     B = len(rows)
@@ -299,6 +327,8 @@ def stepwise(s, prec, flat, x, h0, dl, got, names, rows=None, gates=False, masks
                     g = np.concatenate([r[:, t], z[:, t], n[:, t], gh[:, t, 2 * H:]], 1).astype(np.float64)
                     out[(f"step:g[l{l}d{d},t{t}]", "g_step")] = g if valid is None else np.where(valid[:, t], g, 0.0)
         inp = Y
+    if not head:
+        return out
     top = got["ys"][-1].astype(dt)
     pooled = top[..., :H] + top[..., H:] if D == 2 else top
     if lens is None:
@@ -318,7 +348,7 @@ def stepwise(s, prec, flat, x, h0, dl, got, names, rows=None, gates=False, masks
     return out
 
 
-def kernel_steps(got, s, names, rows=None, gates=False):
+def kernel_steps(got, s, names, rows=None, gates=False, head=True):
     """The kernel's side of stepwise."""
     H = s["H"]
     rows = np.arange(s["B"]) if rows is None else np.asarray(rows)
@@ -329,6 +359,8 @@ def kernel_steps(got, s, names, rows=None, gates=False):
                 out[(f"step:y[l{l}d{d},t{t}]", "y_step")] = y[rows, t, d * H:(d + 1) * H]
                 if gates:
                     out[(f"step:g[l{l}d{d},t{t}]", "g_step")] = got["ws"]["G"][l][d][rows, t].astype(np.float64)
+    if not head:
+        return out
     out[("step:logits", "logits_step")] = got["logits"]
     o, k = names["lin_w"]
     out[("step:grad:lin_w", "w_step")] = got["grads"][o:o + k]
@@ -361,7 +393,7 @@ def head_dy(s, dcat, arg, lens=None):
     return np.concatenate([v] * D, 2)
 
 
-def backward_steps(s, prec, flat, h0, ws, ys, names, own=False, masks=None, lens=None):
+def backward_steps(s, prec, flat, h0, ws, ys, names, own=False, masks=None, lens=None, head=True, dy=None, dhn=None):
     """Layer 0's backward recurrence one step at a time in float64, following gru_scan_bwd_kernel (tc_hopper.cuh), per
     direction in the kernel's step order.  Each step takes the kernel's own operands: its dY (ws["DY"][0]), its gates
     (ws["G"][0]) and its h_{t-1} (ys[0], or h0), and
@@ -375,12 +407,21 @@ def backward_steps(s, prec, flat, h0, ws, ys, names, own=False, masks=None, lens
     masks: layer 0's recurrent-dropout masks [D, B, H] (DESIGN.md §4.8): the gate math takes m * h_{t-1} (_masked), and
     the carry leaving a valid step is m (dh z + P).  The dh0 item then ends in the carry before the last step's mask (the
     fp32 path masks it into dh0 later; the scans' dh_{-1} is masked).  lens: a padded step has dgi = dgh = 0 and passes the
-    carry on unchanged and unmasked."""
+    carry on unchanged and unmasked.
+    head=False (a head-less plan): the carry of direction d starts from the caller's dhn[0*D + d] (None: zero), and when
+    layer 0 is the top layer (L = 1) its dY is the caller's dy (None: zero) rather than a workspace region."""
     B, T, H, L, D = (s[k] for k in "BTHLD")
+    if head or L > 1:
+        dYall = ws["DY"][0]
+    else:
+        dYall = np.zeros((B, T, D * H)) if dy is None else dy
     for d in range(D):
         w = split(_block(flat, names, f"l0d{d}.w_hh", (3 * H, H)), prec)        # P[b, k] = sum_q dgh[b, q] W[q, k]
-        G, y, dY = ws["G"][0][d], ys[0][:, :, d * H:(d + 1) * H], ws["DY"][0][:, :, d * H:(d + 1) * H]
-        carry = ws["DCAT"][:, :H].astype(np.float64) if L == 1 else np.zeros((B, H))
+        G, y, dY = ws["G"][0][d], ys[0][:, :, d * H:(d + 1) * H], dYall[:, :, d * H:(d + 1) * H]
+        if not head:
+            carry = np.zeros((B, H)) if dhn is None else np.asarray(dhn[d], np.float64)
+        else:
+            carry = ws["DCAT"][:, :H].astype(np.float64) if L == 1 else np.zeros((B, H))
         start = np.zeros((B, H)) if h0 is None else h0[d].astype(np.float64)
         raw = None
         for st in range(T):
@@ -411,7 +452,7 @@ def backward_steps(s, prec, flat, h0, ws, ys, names, own=False, masks=None, lens
         yield "dh0", d, None, carry, raw
 
 
-def gemm_steps(s, prec, flat, dl, h0, ops, names, arg, masks=None, lens=None):
+def gemm_steps(s, prec, flat, dl, h0, ops, names, arg, masks=None, lens=None, head=True):
     """Every backward GEMM of layer 0 and of the head in float64, from the operands the kernels read: `ops` holds the dgi
     and dgh planes (DGIP, DGHP: (hi, lo) [D, B, T, 3H]), the layer input's planes (XP [B, T, pitch]), the Y planes of layer
     0 (YP [B, T, D*H]), fp32 dgi and dgh (DGI, DGH [D, B, T, 3H]) and the kernel's dcat.  Returns (name, "gemm_step") ->
@@ -424,7 +465,8 @@ def gemm_steps(s, prec, flat, dl, h0, ops, names, arg, masks=None, lens=None):
       dy[l{L-1}]         the top layer's upstream gradient from the kernel's dcat and `arg` (when it survives the backward:
                          layers 0 and 1).
     masks: layer 0's recurrent-dropout masks [D, B, H]: dW_hh takes the masked-state planes ops["RDS"] instead of the Y
-    planes, and its w0 term m * h0 (_masked).  lens: as head_dy."""
+    planes, and its w0 term m * h0 (_masked).  lens: as head_dy.  head=False: no dcat and no head dy (dl, arg and
+    ops["DCAT"] are unused); the top layer's upstream gradient is the caller's."""
     B, T, F, H, L, D = (s[k] for k in "BTFHLD")
     BT = B * T
     flat2 = lambda p, d=None: tuple(None if a is None else (a if d is None else a[d]).reshape(BT, -1) for a in p)   # noqa: E731
@@ -457,13 +499,15 @@ def gemm_steps(s, prec, flat, dl, h0, ops, names, arg, masks=None, lens=None):
         out[(f"gemm:grad:l0d{d}.b_ih", "gemm_step")] = ops["DGI"][d].reshape(BT, 3 * H).astype(np.float64).sum(0)
         out[(f"gemm:grad:l0d{d}.b_hh", "gemm_step")] = ops["DGH"][d].reshape(BT, 3 * H).astype(np.float64).sum(0)
     out[("gemm:dx", "gemm_step")] = dx.reshape(B, T, F)
+    if not head:
+        return out
     out[("gemm:dcat", "gemm_step")] = head_dcat(s, prec, flat, dl, names)
     if L <= 2:
         out[(f"gemm:dy[l{L - 1}]", "gemm_step")] = head_dy(s, ops["DCAT"].astype(np.float64), arg, lens)
     return out
 
 
-def kernel_gemm_steps(got, s, names):
+def kernel_gemm_steps(got, s, names, head=True):
     """The kernel's side of gemm_steps."""
     out = {}
     for d in range(s["D"]):
@@ -471,6 +515,8 @@ def kernel_gemm_steps(got, s, names):
             o, k = names[f"l0d{d}.{nm}"]
             out[(f"gemm:grad:l0d{d}.{nm}", "gemm_step")] = got["grads"][o:o + k]
     out[("gemm:dx", "gemm_step")] = got["dx"]
+    if not head:
+        return out
     out[("gemm:dcat", "gemm_step")] = got["ws"]["DCAT"].astype(np.float64)
     if s["L"] <= 2:
         out[(f"gemm:dy[l{s['L'] - 1}]", "gemm_step")] = got["ws"]["DY"][s["L"] - 1].astype(np.float64)
@@ -486,7 +532,8 @@ def _split_bits(v32, prec):
 
 def plane_checks(got, s, prec, x, masks=None, lens=None, drop=False):
     """Elements (hi and lo together) where a plane the kernels wrote differs bitwise from split_bf16 of its fp32 source:
-    the Y planes of every layer; layer 0's input planes (x, zero-padded to the pitch; the dropped x under dropout); the dgi
+    the Y planes of every layer; layer 0's input planes (x, zero-padded to the pitch; the dropped x under dropout with a
+    head, the undropped x on a head-less plan, whose dropout never touches x: pass that x); the dgi
     planes; the dgh planes, zero at each sequence's first step.  name -> count; all must be 0.
     masks: the host restatement of the recurrent-dropout masks [L, D, B, H] (rd_masks).  Then the masks in the stash must
     equal them, RDS[l] must be split_bf16 of fp32(m * Y) (at fp32 the float32 product itself; only these two at fp32), and
@@ -510,8 +557,8 @@ def plane_checks(got, s, prec, x, masks=None, lens=None, drop=False):
                 out[f"RD_STATE[l{l}]"] = bad(ws["RDS"][l][0].view(np.uint32), r.view(np.uint32))
             else:
                 out[f"RD_STATE[l{l}]"] = cmp(ws["RDS"][l], _split_bits(r, prec))
-        if prec == "fp32":
-            return out
+    if prec == "fp32":                                          # fp32 keeps no planes
+        return out
     for l, y in enumerate(got["ys"]):
         if masks is None or (l + 1 < s["L"] and not drop):
             out[f"Y_PLANES[l{l}]"] = cmp(ws["YP"][l], _split_bits(y.astype(np.float32), prec))
