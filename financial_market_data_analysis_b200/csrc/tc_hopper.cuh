@@ -92,9 +92,18 @@ __device__ __forceinline__ uint32_t cluster_rank() {
 //     STAGES-deep mbarrier ring and runs ahead across unit boundaries; two consumer warpgroups (64 rows each) multiply with
 //     wgmma.m64n128k16 (fp32 accumulation), keep one wgmma group in flight and release the previous stage;
 //     bf16x3 issues hi*hi + hi*lo + lo*hi per k-step;
-//   * split-K units write fp32 partials; splitk_reduce_kernel adds them in split order (no atomics: bit-reproducible).
+//   * split-K units write fp32 partials; splitk_reduce_kernel adds them in split order (no atomics: bit-reproducible);
+//   * jobs that overwrite a 16-byte-aligned C (WgJob::cmap) stage each warpgroup's 64 x 128 result, bias added, in shared
+//     memory as 64 x 32 boxes and send them with bulk tensor stores that drain while the next unit's mainloop runs; the
+//     others (beta accumulation, unaligned C) store straight from registers.
 // ------------------------------------------------------------------------------------------------------
 constexpr int WG_BM = 128, WG_BN = 128, WG_BK = 64;
+constexpr int WG_CBOX = 64 * 32 * 4;                          // one staging box: 64 rows x 32 fp32 (128-byte rows)
+// staging boxes per consumer warpgroup: a whole 64 x 128 result at bf16; at bf16x3 the 3-stage ring leaves room for two
+__host__ __device__ constexpr int wg_cboxes(int ns) { return ns == 1 ? 4 : 2; }
+__host__ __device__ constexpr int wg_smem_bytes(int ns, int stages) {
+    return 1024 + stages * 2 * (ns == 1 ? 1 : 2) * WG_BM * WG_BK * 2 + 2 * wg_cboxes(ns) * WG_CBOX + 2 * stages * 8;
+}
 
 // packs a small fp32 operand (weights, head activations) into a zero-padded K-major image [batch][Rp][Kp], hi and lo planes
 __global__ void tc_pack_kernel(const float* __restrict__ src, int64_t s_r, int64_t s_k, int64_t zsrc, int R, int K, int Rp, int Kp,
@@ -184,6 +193,17 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, 
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                  ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
+// one box from shared memory to global; TMA clips the rows and columns that fall outside the map
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(src), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still read shared memory
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 // wgmma shared-memory descriptor, 128-byte swizzle.  K-major: rows of 64 bf16 (128 B), 8-row groups 1024 B apart.
 // MN-major: lines of 64 MN elements per k, 8-k groups 1024 B apart (stride byte offset), 64-element MN blocks 8 KB apart
 // (leading byte offset: one 64 x 64 TMA box).
@@ -210,19 +230,22 @@ struct WgJob {
     int kblocks, kbd;                           // k-blocks per unit's full K range; per direction when kcat
     int kcat;                                   // 1: the K loop runs over direction 0, then direction 1 (dz = kb / kbd)
     int beta;
+    int cmap;                                   // 1: C (or part) goes out through the C tensor map, staged in shared memory
     int64_t ldc, zC, zBias;
 };
 
 template <int NS, int STAGES, int AMN, int BMN>
 __global__ void __launch_bounds__(384, 1)
 wg_gemm_kernel(const __grid_constant__ CUtensorMap ta_hi, const __grid_constant__ CUtensorMap ta_lo,
-               const __grid_constant__ CUtensorMap tb_hi, const __grid_constant__ CUtensorMap tb_lo, const WgJob j) {
+               const __grid_constant__ CUtensorMap tb_hi, const __grid_constant__ CUtensorMap tb_lo,
+               const __grid_constant__ CUtensorMap tc, const WgJob j) {
     constexpr int NH = NS == 1 ? 1 : 2;
     constexpr int PLANE = WG_BM * WG_BK * 2;                  // 16 KB: one 128 x 64 bf16 tile
     constexpr int STAGE = 2 * NH * PLANE;                     // A planes, then B planes
+    constexpr int CB = wg_cboxes(NS);
     extern __shared__ __align__(1024) uint8_t wg_smem_raw[];
     uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(wg_smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* full = reinterpret_cast<uint64_t*>(sm + STAGES * STAGE);
+    uint64_t* full = reinterpret_cast<uint64_t*>(sm + STAGES * STAGE + 2 * CB * WG_CBOX);
     uint64_t* empty = full + STAGES;
     const int wgi = threadIdx.x / 128, tid = threadIdx.x % 128;
     const int units = j.tm * j.tn * j.batch * j.splits;
@@ -313,6 +336,48 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap ta_hi, const __grid_constant_
         }
         asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
         if (prev >= 0 && tid == 0) mbar_arrive(empty + prev);
+        if (j.cmap) {
+            // box c holds columns 32c .. +32 of the warpgroup's 64 rows in staging slot c % CB.  Row r's 16-byte chunk k sits
+            // at chunk k ^ (r % 8), the 128-byte swizzle of the map, so a warp's v2 stores (8 rows x 32 B) hit every bank twice
+            const float* bias = j.splits == 1 && j.bias ? j.bias + zb * j.zBias : nullptr;
+            const int zc = j.splits > 1 ? s * j.batch + zb : zb;
+            const int q = l & 3, r8 = l >> 2;
+            float bv[32];
+#pragma unroll
+            for (int i = 0; i < 16; ++i)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int gn = n0 + 8 * i + 2 * q + e;
+                    bv[2 * i + e] = bias && gn < j.N ? bias[gn] : 0.f;
+                }
+            uint8_t* stg = sm + STAGES * STAGE + cg * CB * WG_CBOX;
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                const uint32_t box = smem_u32(stg + (c % CB) * WG_CBOX);
+                if (tid == 0) bulk_wait_read<CB - 1>();       // the store that last read this slot is done with it
+                named_sync(1 + cg, 128);
+#pragma unroll
+                for (int ii = 0; ii < 4; ++ii) {
+                    const int i = 4 * c + ii;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        float v0 = d[4 * i + 2 * h], v1 = d[4 * i + 2 * h + 1];
+                        if (bias) { v0 += bv[2 * i]; v1 += bv[2 * i + 1]; }
+                        const uint32_t a = box + (w * 16 + r8 + 8 * h) * 128 + (((2 * ii + (q >> 1)) ^ r8) << 4) + (q & 1) * 8;
+                        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(v0), "f"(v1) : "memory");
+                    }
+                }
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the writes, visible to the bulk copy
+                named_sync(1 + cg, 128);
+                if (tid == 0) {
+                    if (n0 + 32 * c < j.N) tma_store_3d(&tc, box, n0 + 32 * c, m0 + cg * 64, zc);
+                    bulk_commit();
+                }
+            }
+            continue;
+        }
+        // direct stores from registers: the only path for jobs that add to C (beta) and for a C whose base or row pitch is
+        // not 16-byte aligned, which a tensor map cannot describe (e.g. N = 13 features)
         float* C;
         int64_t ldc;
         const float* bias = nullptr;
@@ -338,6 +403,7 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap ta_hi, const __grid_constant_
                 else *c = v;
             }
     }
+    if (j.cmap && tid == 0) bulk_wait_all();
 }
 
 // C[z][m][n] (+)= sum over s = 0, 1, ... of part[s][z][m][n]: the split-K partial sums in a fixed order
@@ -944,9 +1010,9 @@ struct Planes {
 typedef CUresult (*PFN_encodeTiled_t)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                       const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                       CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-// 3-D tensor map over one plane with 128-byte swizzle and zero fill out of bounds: boxes of 64 (K) x 128 rows for a K-major
-// operand, 64 (MN) x 64 (K) rows for an MN-major one
-static int make_plane_map(CUtensorMap* m, const htc::bf16_t* base, const Planes& p, bool mn) {
+// 3-D tensor map [depth][rows][cols] with 128-byte swizzle; out-of-bounds elements read as zero and are not written
+static int encode_map(CUtensorMap* m, CUtensorMapDataType type, int esize, const void* base, int64_t cols, int64_t rows,
+                      int64_t depth, int64_t pitch, int64_t zstride, uint32_t box0, uint32_t box1) {
     static PFN_encodeTiled_t enc = nullptr;
     if (!enc) {
         void* f = nullptr;
@@ -957,23 +1023,29 @@ static int make_plane_map(CUtensorMap* m, const htc::bf16_t* base, const Planes&
         }
         enc = (PFN_encodeTiled_t)f;
     }
-    const cuuint64_t dims[3] = {(cuuint64_t)p.cols, (cuuint64_t)p.rows, (cuuint64_t)p.depth};
-    const cuuint64_t strides[2] = {(cuuint64_t)p.pitch * 2, (cuuint64_t)(p.pitch * p.rows) * 2};
-    const cuuint32_t box[3] = {64u, mn ? 64u : 128u, 1u}, es[3] = {1u, 1u, 1u};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<htc::bf16_t*>(base), dims, strides, box, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)depth};
+    const cuuint64_t strides[2] = {(cuuint64_t)(pitch * esize), (cuuint64_t)(zstride * esize)};
+    const cuuint32_t box[3] = {box0, box1, 1u}, es[3] = {1u, 1u, 1u};
+    CUresult r = enc(m, type, 3, const_cast<void*>(base), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { bigru_set_error("tc_gemm: cuTensorMapEncodeTiled failed (%d)", (int)r); return BIGRU_ERR_CUDA; }
     return BIGRU_OK;
 }
 
+// one plane: boxes of 64 (K) x 128 rows for a K-major operand, 64 (MN) x 64 (K) rows for an MN-major one
+static int make_plane_map(CUtensorMap* m, const htc::bf16_t* base, const Planes& p, bool mn) {
+    return encode_map(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, p.cols, p.rows, p.depth, p.pitch, p.pitch * p.rows, 64u,
+                      mn ? 64u : 128u);
+}
+
 template <int NS, int AMN, int BMN>
-static int wg_launch(const CUtensorMap (&tm)[4], const htc::WgJob& j, int grid, cudaStream_t st) {
+static int wg_launch(const CUtensorMap (&tm)[5], const htc::WgJob& j, int grid, cudaStream_t st) {
     constexpr int STAGES = NS == 1 ? 4 : 3;
-    const int smem = STAGES * 2 * (NS == 1 ? 1 : 2) * 16384 + 1024 + 2 * STAGES * 8;
+    constexpr int smem = htc::wg_smem_bytes(NS, STAGES);
+    static_assert(smem <= 232448, "wg_gemm_kernel: more shared memory than an sm_90 block may have");
     auto k = htc::wg_gemm_kernel<NS, STAGES, AMN, BMN>;
     CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    k<<<grid, 384, smem, st>>>(tm[0], tm[1], tm[2], tm[3], j);
+    k<<<grid, 384, smem, st>>>(tm[0], tm[1], tm[2], tm[3], tm[4], j);
     LAUNCH_CHECK();
     return BIGRU_OK;
 }
@@ -989,7 +1061,7 @@ static int wg_gemm(htc::WgJob j, const Planes& A, bool amn, const Planes& B, boo
     }
     j.tm = (int)cdiv64(j.M, htc::WG_BM);
     j.tn = (int)cdiv64(j.N, htc::WG_BN);
-    CUtensorMap tm[4];
+    CUtensorMap tm[5];
     TRY(make_plane_map(&tm[0], A.hi, A, amn));
     TRY(make_plane_map(&tm[2], B.hi, B, bmn));
     if (x3) {
@@ -998,6 +1070,15 @@ static int wg_gemm(htc::WgJob j, const Planes& A, bool amn, const Planes& B, boo
     } else {
         tm[1] = tm[0]; tm[3] = tm[2];
     }
+    // the kernel's output: part [splits * batch][M][N] for split jobs, else C [batch][M][ldc] with batch stride zC.  It goes
+    // through a tensor map when the job overwrites it and its base and strides are 16-byte aligned (a map's requirement)
+    const bool split = j.splits > 1;
+    float* const cbase = split ? j.part : j.C;
+    const int64_t depth = split ? (int64_t)j.splits * j.batch : j.batch, ldc = split ? j.N : j.ldc;
+    const int64_t zc = depth == 1 ? j.M * ldc : split ? (int64_t)j.M * j.N : j.zC;
+    j.cmap = (split || !j.beta) && reinterpret_cast<uintptr_t>(cbase) % 16 == 0 && ldc % 4 == 0 && zc % 4 == 0;
+    if (j.cmap) TRY(encode_map(&tm[4], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, cbase, j.N, j.M, depth, ldc, zc, 32u, 64u));
+    else tm[4] = tm[0];
     int dev = 0, nsm = 132;
     CUDA_TRY(cudaGetDevice(&dev));
     CUDA_TRY(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
