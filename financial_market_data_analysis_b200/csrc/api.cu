@@ -361,6 +361,84 @@ extern "C" int bigru_workspace_region(const bigru_plan* p, int which, int layer,
     return BIGRU_OK;
 }
 
+// One wg_gemm job on the caller's operands (test support; see the header).  Workspace (floats, offsets rounded to 64 floats
+// like the plans' planes): A's planes, B's planes, then the split-K partials [splits][batch][M][N].  K-major operands are
+// packed by tc_pack as tc_gemm_launch packs them; MN-major ones become [batch * K][rup(cols, 8)] planes through
+// to_planes_kernel, as the dW jobs' planes do.
+struct TcGemmWs {
+    int64_t a, b, part, total;
+    int splits;
+};
+static int tc_gemm_layout(int precision, int mn_major, int M, int N, int K, int batch, int splits, TcGemmWs* w) {
+    if ((precision != BIGRU_PREC_BF16 && precision != BIGRU_PREC_BF16X3) || (mn_major != 0 && mn_major != 1) || M < 1 ||
+        N < 1 || K < 1 || batch < 1 || splits < 0) {
+        bigru_set_error("tc_gemm: bad job precision=%d mn_major=%d M=%d N=%d K=%d batch=%d splits=%d", precision, mn_major, M, N,
+                        K, batch, splits);
+        return BIGRU_ERR_ARG;
+    }
+    const int64_t kb = cdiv64(K, htc::WG_BK);
+    const int s = splits ? splits : wg_splits(cdiv64(M, htc::WG_BM) * cdiv64(N, htc::WG_BN) * batch, kb);
+    if ((int64_t)(s - 1) * cdiv64(kb, s) >= kb) {
+        bigru_set_error("tc_gemm: %d splits of %lld k-blocks leave a split empty", s, (long long)kb);
+        return BIGRU_ERR_ARG;
+    }
+    const int64_t x = precision == BIGRU_PREC_BF16X3 ? 2 : 1;
+    auto planes = [&](int64_t rows) {
+        return mn_major ? rup(x * batch * K * rup(rows, 8), 128) / 2 : rup(tc_pack_elems(rows, K, batch, precision), 128) / 2;
+    };
+    w->splits = s;
+    w->a = 0;
+    w->b = w->a + planes(M);
+    w->part = w->b + planes(N);
+    w->total = w->part + (s > 1 ? (int64_t)s * batch * M * N : 0);
+    return BIGRU_OK;
+}
+
+extern "C" int bigru_tc_gemm_workspace_bytes(int precision, int mn_major, int M, int N, int K, int batch, int splits,
+                                             size_t* bytes) {
+    if (!bytes) { bigru_set_error("tc_gemm_workspace_bytes: null argument"); return BIGRU_ERR_ARG; }
+    TcGemmWs w;
+    TRY(tc_gemm_layout(precision, mn_major, M, N, K, batch, splits, &w));
+    *bytes = (size_t)w.total * sizeof(float);
+    return BIGRU_OK;
+}
+
+extern "C" int bigru_tc_gemm(int precision, int mn_major, int M, int N, int K, int batch, const float* d_a, const float* d_b,
+                             const float* d_bias, int64_t z_bias, float* d_c, int64_t ldc, int64_t z_c, int beta, int splits,
+                             void* d_workspace, int* staged, void* stream) {
+    if (!d_a || !d_b || !d_c || !d_workspace || !staged) { bigru_set_error("tc_gemm: null argument"); return BIGRU_ERR_ARG; }
+    TcGemmWs w;
+    TRY(tc_gemm_layout(precision, mn_major, M, N, K, batch, splits, &w));
+    if (ldc < N || (batch > 1 && z_c < (int64_t)(M - 1) * ldc + N) || (d_bias && z_bias < 0)) {
+        bigru_set_error("tc_gemm: rows or batches of C overlap (N=%d ldc=%lld z_c=%lld) or z_bias=%lld < 0", N, (long long)ldc,
+                        (long long)z_c, (long long)z_bias);
+        return BIGRU_ERR_ARG;
+    }
+    const int64_t kb = cdiv64(K, htc::WG_BK);
+    htc::WgJob j = wg_job(d_c, M, N, ldc, batch, kb);
+    j.bias = d_bias; j.zBias = z_bias; j.zC = z_c; j.beta = beta ? 1 : 0; j.splits = w.splits;
+    j.a.zsel = 1; j.b.zsel = 1;
+    TRY(wg_job_check(j));
+    float* ws = static_cast<float*>(d_workspace);
+    j.part = ws + w.part;
+    const cudaStream_t st = (cudaStream_t)stream;
+    htc::bf16_t* pa = reinterpret_cast<htc::bf16_t*>(ws + w.a);
+    htc::bf16_t* pb = reinterpret_cast<htc::bf16_t*>(ws + w.b);
+    const bool x3 = precision == BIGRU_PREC_BF16X3;
+    Planes A, B;
+    if (mn_major) {
+        const int64_t pma = rup(M, 8), pnb = rup(N, 8);
+        A = Planes{pa, x3 ? pa + (int64_t)batch * K * pma : nullptr, M, K, batch, pma};
+        B = Planes{pb, x3 ? pb + (int64_t)batch * K * pnb : nullptr, N, K, batch, pnb};
+        KLAUNCH(KC_PACK, 0.0, 0.0, st, htc::to_planes_kernel<<<132 * 8, 256, 0, st>>>(d_a, (int64_t)batch * K, M, (int)pma, mut(A), mut_lo(A)));
+        KLAUNCH(KC_PACK, 0.0, 0.0, st, htc::to_planes_kernel<<<132 * 8, 256, 0, st>>>(d_b, (int64_t)batch * K, N, (int)pnb, mut(B), mut_lo(B)));
+    } else {
+        TRY(tc_pack(d_a, K, 1, (int64_t)M * K, M, K, batch, precision, pa, &A, st));
+        TRY(tc_pack(d_b, K, 1, (int64_t)N * K, N, K, batch, precision, pb, &B, st));
+    }
+    return wg_gemm(j, A, mn_major != 0, B, mn_major != 0, precision, st, staged);
+}
+
 static inline unsigned nblk(int64_t n, int bs) { return (unsigned)cdiv64(n, bs); }
 
 // ------------------------------------------------------------------------------------------

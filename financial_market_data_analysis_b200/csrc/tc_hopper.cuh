@@ -93,9 +93,9 @@ __device__ __forceinline__ uint32_t cluster_rank() {
 //     wgmma.m64n128k16 (fp32 accumulation), keep one wgmma group in flight and release the previous stage;
 //     bf16x3 issues hi*hi + hi*lo + lo*hi per k-step;
 //   * split-K units write fp32 partials; splitk_reduce_kernel adds them in split order (no atomics: bit-reproducible);
-//   * jobs that overwrite a 16-byte-aligned C (WgJob::cmap) stage each warpgroup's 64 x 128 result, bias added, in shared
-//     memory as 64 x 32 boxes and send them with bulk tensor stores that drain while the next unit's mainloop runs; the
-//     others (beta accumulation, unaligned C) store straight from registers.
+//   * jobs that overwrite a 16-byte-aligned C with rows of whole 16-byte chunks (WgJob::cmap) stage each warpgroup's
+//     64 x 128 result, bias added, in shared memory as 64 x 32 boxes and send them with bulk tensor stores that drain while
+//     the next unit's mainloop runs; the others (beta accumulation, unaligned C, N % 4 != 0) store straight from registers.
 // ------------------------------------------------------------------------------------------------------
 constexpr int WG_BM = 128, WG_BN = 128, WG_BK = 64;
 constexpr int WG_CBOX = 64 * 32 * 4;                          // one staging box: 64 rows x 32 fp32 (128-byte rows)
@@ -376,8 +376,9 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap ta_hi, const __grid_constant_
             }
             continue;
         }
-        // direct stores from registers: the only path for jobs that add to C (beta) and for a C whose base or row pitch is
-        // not 16-byte aligned, which a tensor map cannot describe (e.g. N = 13 features)
+        // direct stores from registers: the only path for jobs that add to C (beta), for a C whose base or row pitch is not
+        // 16-byte aligned, which a tensor map cannot describe, and for rows that end inside a 16-byte chunk (e.g. N = 13
+        // features), which a bulk tensor store would overrun
         float* C;
         int64_t ldc;
         const float* bias = nullptr;
@@ -1050,9 +1051,22 @@ static int wg_launch(const CUtensorMap (&tm)[5], const htc::WgJob& j, int grid, 
     return BIGRU_OK;
 }
 
+// what wg_gemm refuses before it touches the device.  A bias with split-K: neither epilogue adds it to the partials and
+// splitk_reduce_kernel has no bias, so the result would silently lack it (no plan asks for the combination)
+static int wg_job_check(const htc::WgJob& j) {
+    if (j.bias && j.splits > 1) {
+        bigru_set_error("tc_gemm: a bias together with split-K (%d splits) is not supported", j.splits);
+        return BIGRU_ERR_ARG;
+    }
+    return BIGRU_OK;
+}
+
 // runs j (M, N, batch, kblocks, kbd, kcat, C, bias, beta, ldc, zC, zBias, a/b coordinates set; tm, tn, part filled here)
-// over planes A and B; split-K partials (j.splits > 1) go to j.part and are reduced into C in split order
-static int wg_gemm(htc::WgJob j, const Planes& A, bool amn, const Planes& B, bool bmn, int prec, cudaStream_t st) {
+// over planes A and B; split-K partials (j.splits > 1) go to j.part and are reduced into C in split order.  staged (nullable)
+// receives j.cmap, the epilogue the kernel runs
+static int wg_gemm(htc::WgJob j, const Planes& A, bool amn, const Planes& B, bool bmn, int prec, cudaStream_t st,
+                   int* staged = nullptr) {
+    TRY(wg_job_check(j));
     if (j.M <= 0 || j.N <= 0) return BIGRU_OK;
     const bool x3 = prec == BIGRU_PREC_BF16X3;
     if (x3 != (A.lo != nullptr) || x3 != (B.lo != nullptr) || amn != bmn) {
@@ -1071,14 +1085,17 @@ static int wg_gemm(htc::WgJob j, const Planes& A, bool amn, const Planes& B, boo
         tm[1] = tm[0]; tm[3] = tm[2];
     }
     // the kernel's output: part [splits * batch][M][N] for split jobs, else C [batch][M][ldc] with batch stride zC.  It goes
-    // through a tensor map when the job overwrites it and its base and strides are 16-byte aligned (a map's requirement)
+    // through a tensor map when the job overwrites it, its base and strides are 16-byte aligned (a map's requirement) and
+    // its rows are whole 16-byte chunks: the bulk tensor store clips a box at the map's column extent only to 16 bytes, so
+    // N = 13 at ldc = 16 would overwrite columns 13..15 of every row (seen on the H100; tests/test_gpu_tc_gemm.py)
     const bool split = j.splits > 1;
     float* const cbase = split ? j.part : j.C;
     const int64_t depth = split ? (int64_t)j.splits * j.batch : j.batch, ldc = split ? j.N : j.ldc;
     const int64_t zc = depth == 1 ? j.M * ldc : split ? (int64_t)j.M * j.N : j.zC;
-    j.cmap = (split || !j.beta) && reinterpret_cast<uintptr_t>(cbase) % 16 == 0 && ldc % 4 == 0 && zc % 4 == 0;
+    j.cmap = (split || !j.beta) && reinterpret_cast<uintptr_t>(cbase) % 16 == 0 && ldc % 4 == 0 && zc % 4 == 0 && j.N % 4 == 0;
     if (j.cmap) TRY(encode_map(&tm[4], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, cbase, j.N, j.M, depth, ldc, zc, 32u, 64u));
     else tm[4] = tm[0];
+    if (staged) *staged = j.cmap;
     int dev = 0, nsm = 132;
     CUDA_TRY(cudaGetDevice(&dev));
     CUDA_TRY(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));

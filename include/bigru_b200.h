@@ -11,6 +11,10 @@
  *    library never frees caller memory and keeps no reference to it after the call returns;
  *  - `stream` is a cudaStream_t passed as void*; all calls are asynchronous on that stream and
  *    never synchronise; a plan may be used from one stream at a time;
+ *  - a d_* array needs only the alignment of its element type (4 bytes for float and int32): where a kernel has a
+ *    vector or bulk-tensor path (the tensor-core GEMMs' staged epilogue, bigru_window_gather_norm) it checks the actual
+ *    address and strides and otherwise stores element by element, with bitwise the same results.  The workspaces
+ *    (d_stash, d_scratch, d_workspace) hold bf16 planes that TMA reads and must be 16-byte aligned (cudaMalloc: 256);
  *  - every function returns 0 on success, <0 on error (BIGRU_ERR_*); bigru_last_error() returns
  *    a thread-local message.  There is no CPU fallback anywhere: without an sm_90 (H100)
  *    device every compute call fails with BIGRU_ERR_DEVICE.
@@ -140,6 +144,25 @@ int  bigru_workspace_region(const bigru_plan* plan, int which, int layer, int* i
  *  recurrent_p > 0 both describe the recurrent-dropout scans, which that plan's training calls launch.
  *  BIGRU_PREC_FP32: BIGRU_ERR_UNSUPPORTED; another scan: BIGRU_ERR_ARG. */
 int  bigru_scan_geometry(const bigru_plan* plan, int scan, int* R, int* n_split);
+
+/* --- One tensor-core GEMM job (test support): the persistent wgmma GEMM every projection and gradient of the tensor-core
+ *  plans runs, on the caller's fp32 operands, through the same host code as the plans' jobs.
+ *      C[z][m][n] (+)= sum_k A[z][m][k] * B[z][n][k] (+ d_bias[z * z_bias + n]),   z < batch, m < M, n < N, k < K
+ *  precision BIGRU_PREC_BF16 or BIGRU_PREC_BF16X3 (operands split into bf16 hi, and lo, as the plans split them; fp32
+ *  accumulation).  mn_major 0: d_a [batch][M][K], d_b [batch][N][K], packed into K-major planes (as the head's operands);
+ *  mn_major 1: d_a [batch][K][M], d_b [batch][K][N], MN-major planes (as the weight gradients' operands).  C element
+ *  (z, m, n) is d_c[z * z_c + m * ldc + n]; beta != 0 adds to it.  d_bias nullable.  splits: split-K count, 0 = the plans'
+ *  own rule for the shape.  *staged: 1 when the output tile went out through shared memory and bulk tensor stores, 0
+ *  when it was stored element by element; the library decides it as for every plan job, from beta and the alignment of
+ *  the output (C, or with splits > 1 the partials in d_workspace): base, ldc and z_c multiples of 16 bytes and N of 4 (a
+ *  row ending inside a 16-byte chunk is stored element by element).  d_workspace:
+ *  bigru_tc_gemm_workspace_bytes bytes, 16-byte aligned.  BIGRU_ERR_ARG, before any device work: an unknown precision or
+ *  mn_major, M, N, K or batch < 1, a null operand, ldc < N, z_c < (M-1)*ldc + N when batch > 1, z_bias < 0, a split
+ *  count that leaves a split empty, and a bias with more than one split (split-K has no bias). */
+int  bigru_tc_gemm_workspace_bytes(int precision, int mn_major, int M, int N, int K, int batch, int splits, size_t* bytes);
+int  bigru_tc_gemm(int precision, int mn_major, int M, int N, int K, int batch, const float* d_a, const float* d_b,
+                   const float* d_bias, int64_t z_bias, float* d_c, int64_t ldc, int64_t z_c, int beta, int splits,
+                   void* d_workspace, int* staged, void* stream);
 
 /* --- BiGRU.forward (biGRU_model.py:63-138): dropout :87-94, nn.GRU :102, head :111-137.
  *  d_x[B,T,F]; d_h0 nullable [L*D,B,H] (the `hidden` argument); d_logits[B,C];

@@ -48,6 +48,14 @@ def wg_splits(tiles, kblocks):
     return cdiv(kblocks, cdiv(kblocks, s))
 
 
+def wg_staged(splits, beta, base_bytes, ldc, zc, N):
+    """Restates the epilogue decision of wg_gemm (tc_hopper.cuh): whether a job's output goes out through shared memory and
+    bulk tensor stores (1) or element by element (0).  base_bytes, ldc, zc (elements) describe the kernel's output: C with
+    its batch stride (M * ldc at batch 1), or with splits > 1 the partials [splits][batch][M][N] (ldc = N, zc = M * N).
+    Rows must be whole 16-byte chunks (N % 4 == 0): a bulk tensor store clips columns only to 16 bytes."""
+    return int((splits > 1 or not beta) and base_bytes % 16 == 0 and ldc % 4 == 0 and zc % 4 == 0 and N % 4 == 0)
+
+
 def dw0_gemms(s):
     """(splits, units, short last split) of layer 0's dW_ih and dW_hh launches: M = 3H, N = F or H, K = B*T, 128 x 128
     tiles, one batch per direction."""
