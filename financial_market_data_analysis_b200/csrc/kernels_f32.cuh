@@ -442,8 +442,11 @@ __global__ void clip_adam_dev_kernel(float* __restrict__ p, float* __restrict__ 
 }
 
 // ------------------------------------------------------------------------------------------
-// Window collation (sql_pytorch_dataloader.py:239-245): coalesced, float4 when F % 4 == 0
+// Window collation (sql_pytorch_dataloader.py:239-245): coalesced, float4 when F % 4 == 0.  A NaN source element (SQL NULL
+// in a bulk-loaded table) is read as 0 before normalising: the SQL path selects IFNULL(field, 0)
 // ------------------------------------------------------------------------------------------
+__device__ __forceinline__ float ifnull0(float v) { return isnan(v) ? 0.f : v; }
+
 template <int VEC>
 __global__ void window_gather_kernel(const float* __restrict__ src, const float* __restrict__ xmin,
                                      const float* __restrict__ xmax, int64_t start, int B, int T, int F,
@@ -458,6 +461,7 @@ __global__ void window_gather_kernel(const float* __restrict__ src, const float*
         const int64_t srow = start + b + t;
         if (VEC == 4) {
             float4 v = *reinterpret_cast<const float4*>(src + srow * F + fv * 4);
+            v.x = ifnull0(v.x); v.y = ifnull0(v.y); v.z = ifnull0(v.z); v.w = ifnull0(v.w);
             if (xmin) {
                 const float4 mn = *reinterpret_cast<const float4*>(xmin + fv * 4);
                 const float4 mx = *reinterpret_cast<const float4*>(xmax + fv * 4);
@@ -466,7 +470,7 @@ __global__ void window_gather_kernel(const float* __restrict__ src, const float*
             }
             __stcs(reinterpret_cast<float4*>(out + bt * F + fv * 4), v);
         } else {
-            float v = src[srow * F + fv];
+            float v = ifnull0(src[srow * F + fv]);
             if (xmin) v = (v - xmin[fv]) / (xmax[fv] - xmin[fv]);
             out[bt * F + fv] = v;
         }

@@ -8,7 +8,11 @@ import torch
 
 
 class DevicePrefetcher:
-    """Iterate (x, target) host batches as device tensors, double-buffered through a copy stream."""
+    """Iterate (x, target) host batches as device tensors, double-buffered through a copy stream.
+
+    ``x`` arrives as float32, ``target`` in its own dtype.  A yielded pair lives in one of ``depth`` reused device slots
+    and is valid until the consumer asks for the next pair: the copy of a later batch into that slot is issued as soon
+    as the iteration resumes.  Use (or clone) each pair before advancing."""
 
     def __init__(self, batches, device, depth: int = 2):
         self.batches, self.device, self.depth = batches, torch.device(device), max(2, depth)

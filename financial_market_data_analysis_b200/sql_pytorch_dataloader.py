@@ -52,7 +52,11 @@ def _split_query(db_x_query: str):
 
 
 def chunk_id_ranges(db_length: int, chunk_size: int, window: int):
-    """ID ranges of the chunks; neighbours overlap by window-1 rows so every window appears once."""
+    """ID ranges of the chunks; neighbours overlap by window-1 rows so every window appears once.
+
+    When db_length < chunk_size the one chunk is range(window, db_length + 1), where the reference has
+    range(window, chunk_size): its IDs past the table's end select no row, so both fetch the same rows and get the
+    same MIN/MAX, and every range here stays inside the table (MySQLChunkLoader.from_table needs that)."""
     n_full = db_length // chunk_size
     ranges = []
     for c in range(n_full + 1):
@@ -127,7 +131,8 @@ class MySQLChunkLoader(Dataset):
         """Same object, built from a bulk-loaded feature table resident in HBM instead of 2 SQL aggregates per chunk
         (SURVEY.md 8(f) N3): ``table[i]`` is the row with database ID ``i + 1``, NaN = SQL NULL.  Per-chunk MIN/MAX come
         from one reduction kernel (``bigru_chunk_minmax``); the min==max guard, order-book sharing and the
-        ``norm_params`` pickle are the reference's host rules, unchanged."""
+        ``norm_params`` pickle are the reference's host rules, unchanged.  A column that is NULL in every row of a chunk
+        raises ValueError, as the SQL path cannot build that chunk either (its MIN is NULL)."""
         if not table.is_cuda:
             raise RuntimeError("from_table needs the table on a CUDA device (no CPU fallback)")
         self = cls.__new__(cls)
@@ -140,11 +145,15 @@ class MySQLChunkLoader(Dataset):
         lib = _lib.load()
         mn = torch.empty(F, device=table.device, dtype=torch.float32)
         mx = torch.empty(F, device=table.device, dtype=torch.float32)
-        for ids in self.chunk_indices:
+        for c, ids in enumerate(self.chunk_indices):
             with torch.cuda.device(table.device):
                 _lib.check(lib.bigru_chunk_minmax(_lib.ptr(table), db_length, F, ids[0] - 1, ids[-1], _lib.ptr(mn), _lib.ptr(mx),
                                                   torch.cuda.current_stream(table.device).cuda_stream), "bigru_chunk_minmax")
             x_min, x_max = mn.cpu().reshape(1, F).clone(), mx.cpu().reshape(1, F).clone()
+            empty = (x_min[0] > x_max[0]).nonzero().flatten().tolist()      # the kernel's +inf / -inf: no non-NULL value
+            if empty:
+                raise ValueError(f"from_table: column {self.x_fields[empty[0]]!r} is NULL in every row of chunk {c} "
+                                 f"(IDs {ids[0]}..{ids[-1]})")
             x_min[0], x_max[0] = widen_degenerate(x_min[0], x_max[0])
             self.norm_params.append((x_min, x_max))
         for x_min, x_max in self.norm_params:
@@ -209,7 +218,9 @@ class MySQLBatchLoader(Dataset):
     def from_tensors(cls, x_rows, y_rows, norm_params, window, device=None):
         """The same dataset over a chunk that is already in memory (x_rows [N, F] raw features, y_rows [N, C] targets,
         norm_params = (min [1, F], max [1, F]) as MySQLChunkLoader yields them) - no cursor, no SQL.  Used when the table
-        has been bulk-loaded (MySQLChunkLoader.from_table) and by the loader arm of bench.py."""
+        has been bulk-loaded (MySQLChunkLoader.from_table) and by the loader arm of bench.py.  NaN in x_rows is SQL NULL:
+        the gather kernel reads it as 0 before normalising, the IFNULL(field, 0) the SQL path selects, so both paths give
+        the same batches."""
         self = cls.__new__(cls)
         Dataset.__init__(self)
         if device is None:

@@ -284,8 +284,10 @@ int  bigru_clip_adam_step_dev(float* d_params, float* d_grads, float* d_m, float
                               const int* d_step, float grad_scale, void* stream);
 
 /* --- MySQLBatchLoader collation (sql_pytorch_dataloader.py:239-245 + default_collate):
- *  out[b,t,f] = (src[start+b+t, f] - xmin[f]) / (xmax[f] - xmin[f]);  src is [N,F], start+B+T-1 <= N.
- *  xmin/xmax nullable (then a plain gather).  targets: out[b,0,c] = y[start+b+T-1, c]. */
+ *  out[b,t,f] = (s - xmin[f]) / (xmax[f] - xmin[f]), an IEEE float division, with s = src[start+b+t, f] and a NaN s
+ *  (SQL NULL) read as 0, the IFNULL(field, 0) of the SQL path;  src is [N,F], start+B+T-1 <= N.
+ *  xmin/xmax nullable together (then a plain gather, NaN still read as 0).  B = 0 writes nothing.
+ *  targets: out[b,0,c] = y[start+b+T-1, c]. */
 int  bigru_window_gather_norm(const float* d_src, const float* d_xmin, const float* d_xmax,
                               int64_t start, int64_t N, int B, int T, int F, float* d_out, void* stream);
 int  bigru_window_targets(const float* d_y, int64_t start, int64_t N, int B, int T, int C,
@@ -293,7 +295,8 @@ int  bigru_window_targets(const float* d_y, int64_t start, int64_t N, int B, int
 
 /* --- SURVEY.md 8(f) N3, chunk statistics on the GPU: per-feature MIN / MAX over rows [row_lo, row_hi) of a
  *  table[N,F] (NaN = SQL NULL, ignored), i.e. the two aggregate queries of MySQLChunkLoader
- *  (sql_pytorch_dataloader.py:96-105).  The min==max guard and order-book sharing stay on the host. */
+ *  (sql_pytorch_dataloader.py:96-105).  A column with no non-NaN value in the range gets min = +inf, max = -inf
+ *  (SQL would give NULL).  The min==max guard and order-book sharing stay on the host. */
 int  bigru_chunk_minmax(const float* d_table, int64_t N, int F, int64_t row_lo, int64_t row_hi, float* d_min,
                         float* d_max, void* stream);
 

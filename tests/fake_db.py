@@ -35,6 +35,7 @@ class FakeCursor:
             self._rows = [(self.n,)]
             return
         rows = np.array(self._ids(s), dtype=np.int64) - 1
+        rows = rows[(rows >= 0) & (rows < self.n)]          # WHERE ID IN (...) skips IDs the table does not have
         head = s[len("SELECT"):s.index(" FROM ")]
         if "FROM target" in s:
             names = [w.strip() for w in head.split(",")]
@@ -57,8 +58,13 @@ class FakeCursor:
         return list(self._rows)
 
 
-def make_table(n_rows=250, n_plain=3, levels=2, n_targets=4, seed=7, with_nulls=True, const_col=True):
-    """A small synthetic joined table with order-book size columns, a constant column and NULLs."""
+def make_table(n_rows=250, n_plain=3, levels=2, n_targets=4, seed=7, with_nulls=True, const_col=True, null_rows=None):
+    """A small synthetic joined table with order-book size columns, a constant column and NULLs.
+
+    Columns: ``levels`` bid/ask size pairs, ``n_plain`` normal columns ``sd.f<i>``, then (``const_col``) a constant
+    non-zero and a constant zero column.  ``with_nulls`` puts NULL (NaN) in about 5 % of ``sd.f0``; ``null_rows``
+    ({field: 0-based row numbers}) adds NULLs at chosen rows, e.g. at chunk edges.  The defaults reproduce
+    tests/golden/loader.npz's table bit for bit."""
     rng = np.random.default_rng(seed)
     cols = {}
     for i in range(levels):
@@ -73,6 +79,8 @@ def make_table(n_rows=250, n_plain=3, levels=2, n_targets=4, seed=7, with_nulls=
         nul = rng.random(n_rows) < 0.05
         cols["sd.f0"] = np.where(nul, np.nan, cols["sd.f0"])
     targets = {f"t{i}": (rng.random(n_rows) < 0.3).astype(np.float64) for i in range(n_targets)}
+    for name, rows in (null_rows or {}).items():
+        cols[name][list(rows)] = np.nan
     fields = list(cols.keys())
     query = "SELECT " + ", ".join(fields) + " FROM stock_data_joined sd JOIN other o ON sd.ID = o.ID;"
     return cols, targets, fields, query

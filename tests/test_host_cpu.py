@@ -209,6 +209,42 @@ def test_chunk_loader_host_logic(pkg, golden_dir, tmp_path):
             L.MySQLBatchLoader(ids, norm, cur, "stock_data_joined", query, "t0, t1, t2, t3", 30)
 
 
+@pytest.mark.parametrize("name", ["current", "divisible", "window1", "one_window", "exact_fill", "short"])
+def test_chunk_loader_host_logic_at_table_edges(pkg, golden_dir, tmp_path, monkeypatch, name):
+    """The SQL-path MySQLChunkLoader over every table shape of loader_edges.npz (NULLs at chunk edges, 1-3 book levels,
+    db_length % chunk_size == 0, window 1, one-window chunks): chunk IDs, norm params, the pickle and the split equal the
+    unmodified reference's.  For db_length < chunk_size ("short") the reference's IDs run past the table: the ranges
+    differ on purpose and select the same rows."""
+    import json
+    import pickle
+    import financial_market_data_analysis_b200.sql_pytorch_dataloader as L
+    z = np.load(os.path.join(golden_dir, "loader_edges.npz"))
+    spec = json.loads(str(z[name + "__spec"]))
+    g = lambda key: z[f"{name}__{key}"]                                        # noqa: E731
+    monkeypatch.setattr(L, "bid_levels", spec["table"].get("levels", 2))
+    monkeypatch.setattr(L, "ask_levels", spec["table"].get("levels", 2))
+    cols, targets, fields, query = fake_db.make_table(**spec["table"])
+    assert fields == list(g("fields"))
+    npath = str(tmp_path / "norm_params")
+    cl = L.MySQLChunkLoader(fake_db.FakeCursor(cols, targets), "stock_data_joined", query, spec["chunk_size"], spec["window"],
+                            norm_params_path=npath)
+    assert len(cl) == int(g("n_chunks"))
+    n = len(cols[fields[0]])
+    for i in range(len(cl)):
+        ids, (mn, mx) = cl[i]
+        ref_ids = g(f"chunk{i}_ids")
+        if name == "short":
+            assert n < spec["chunk_size"] and ids == tuple(range(spec["window"], n + 1)) and len(ref_ids) > len(ids)
+            ref_ids = ref_ids[ref_ids <= n]
+        assert np.array_equal(np.array(ids), ref_ids), i
+        assert np.array_equal(mn.numpy(), g(f"chunk{i}_min")) and np.array_equal(mx.numpy(), g(f"chunk{i}_max")), i
+    assert [len(list(s)) for s in L.TrainValTestSplit(cl, 0.1, 0.1).get_sets()] == list(g("split"))
+    saved = pickle.load(open(npath, "rb"))
+    assert list(saved) == fields
+    assert np.array_equal(np.array([float(saved[f]["MIN"]) for f in fields], np.float32), g("pickle_min"))
+    assert np.array_equal(np.array([float(saved[f]["MAX"]) for f in fields], np.float32), g("pickle_max"))
+
+
 def test_metric_arithmetic_matches_sklearn(pkg):
     from sklearn.metrics import accuracy_score, fbeta_score, hamming_loss
     rng = np.random.default_rng(0)
