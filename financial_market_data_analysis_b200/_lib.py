@@ -15,6 +15,9 @@ LIB_PATH = os.path.join(_HERE, "libbigru_b200.so")
 PREC_FP32, PREC_BF16, PREC_BF16X3 = 0, 1, 2
 SQNORM_WS = 528                     # BIGRU_SQNORM_WS: floats of scratch bigru_sqnorm needs
 LOSS_CE, LOSS_BCE, LOSS_MLSM = 0, 1, 2
+LOSS_CE_WEIGHTED, LOSS_MSE, LOSS_L1, LOSS_SMOOTH_L1, LOSS_HUBER = 3, 4, 5, 6, 7
+ADAM_MAX_GROUPS = 64                # BIGRU_ADAM_MAX_GROUPS
+ADAM_GROUP_FIELDS = 6               # bigru_adam_group: lr, beta1, beta2, eps, weight_decay, decoupled (float32 each)
 ERR_ARG, ERR_CUDA, ERR_DEVICE, ERR_UNSUPPORTED = -1, -2, -3, -4
 
 _vp, _i, _i64, _f, _u64, _d = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_uint64, C.c_double
@@ -52,9 +55,11 @@ SIGNATURES = {
     "bigru_cell_forward": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_cell_backward": (_i, [_i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "bigru_loss": (_i, [_i, _vp, _vp, _vp, _vp, _i, _i, _d, _vp, _vp, _vp]),
+    "bigru_loss_param": (_i, [_i, _vp, _vp, _vp, _vp, _i, _i, _d, _f, _vp, _vp, _vp]),
     "bigru_sqnorm": (_i, [_vp, _i64, _vp, _vp, _vp]),
     "bigru_adam_tick": (_i, [_vp, _vp, _vp]),
     "bigru_clip_adam_step_dev": (_i, [_vp, _vp, _vp, _vp, _i64, _vp, _f, _f, _f, _f, _f, _vp, _f, _vp]),
+    "bigru_clip_adam_groups_dev": (_i, [_vp, _vp, _vp, _vp, _i64, _vp, _f, _vp, _i, _vp, _i, _vp, _f, _vp]),
     "bigru_launch_count_add": (None, [C.c_longlong]),
     "bigru_window_gather_norm": (_i, [_vp, _vp, _vp, _i64, _i64, _i, _i, _i, _vp, _vp]),
     "bigru_window_targets": (_i, [_vp, _i64, _i64, _i, _i, _i, _vp, _vp]),

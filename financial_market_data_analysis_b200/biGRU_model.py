@@ -41,9 +41,12 @@ else:
 class _AdamState:
     """Optimiser state of the fused step.  The flat gradient and the scalar loss share one buffer (``gext`` = P gradients + 1
     loss), so that data parallelism needs exactly one all-reduce per step.  Adam's step count lives on the device too
-    (``dstep``), so that a captured CUDA graph of the step stays valid from one step to the next; ``step`` counts on the host."""
+    (``dstep``), so that a captured CUDA graph of the step stays valid from one step to the next; ``step`` counts on the host.
+    So do the hyperparameters of each parameter group (``hyper``, bigru_adam_group rows) and the group of each parameter
+    tensor (``segs``, bigru_adam_segment rows over the flat vector): a learning-rate schedule changes a table entry, not
+    the captured graph."""
 
-    def __init__(self, flat, pad):
+    def __init__(self, flat, pad, n_tensors):
         P, dev = flat.numel(), flat.device
         self.gext = torch.empty(P + 1, device=dev, dtype=torch.float32)
         self.grad, self.loss = self.gext[:P], self.gext[P:P + 1]
@@ -55,6 +58,19 @@ class _AdamState:
         self.pflat = pad.params(flat)
         self.pgrad = torch.empty_like(self.pflat) if pad.padded else self.grad
         self.mirror_steps = []           # optimizer.state[p]["step"] tensors, kept equal to `step`
+        self.hyper = torch.zeros(_lib.ADAM_MAX_GROUPS, _lib.ADAM_GROUP_FIELDS, device=dev, dtype=torch.float32)
+        self.segs = torch.zeros(n_tensors, 3, device=dev, dtype=torch.int64)
+        self.hyper_rows = self.seg_rows = None   # what the last load_tables enqueued
+
+    def load_tables(self, hyper_rows, seg_rows):
+        """Enqueue on the current stream a copy of each table that differs from what the previous call enqueued.  The
+        host rows go through pinned memory, which torch keeps alive until the asynchronous copy has read it: no host
+        synchronisation, and the copy runs before whatever the stream runs next (the step, or its graph replay)."""
+        for rows, dst, dt, attr in ((hyper_rows, self.hyper, torch.float32, "hyper_rows"),
+                                    (seg_rows, self.segs, torch.int64, "seg_rows")):
+            if rows != getattr(self, attr):
+                dst[:len(rows)].copy_(torch.tensor(rows, dtype=dt).pin_memory(), non_blocking=True)
+                setattr(self, attr, rows)
 
     def __getitem__(self, name):
         """Read access by name (``st["grad"]``) for callers that index the state like a dict."""
@@ -324,17 +340,28 @@ class BiGRU(_FlatModel):
 
     # ------------------------------------------------------------------ fused training step
     def _loss_spec(self):
+        """(loss kind, weight, pos_weight, scalar parameter) of a loss the fused step computes, else None."""
         fn = self.loss_fn
+        if getattr(fn, "reduction", None) != "mean":
+            return None
         if isinstance(fn, nn.CrossEntropyLoss):
-            if fn.weight is None and fn.reduction == "mean" and getattr(fn, "label_smoothing", 0.0) == 0.0 \
-                    and fn.ignore_index == -100:
-                return _lib.LOSS_CE, None, None
+            if getattr(fn, "label_smoothing", 0.0) == 0.0 and fn.ignore_index == -100:
+                if fn.weight is None:
+                    return _lib.LOSS_CE, None, None, 0.0
+                if fn.weight.dim() == 1 and fn.weight.numel() == self.output_size:
+                    return _lib.LOSS_CE_WEIGHTED, fn.weight, None, 0.0
         elif isinstance(fn, nn.BCEWithLogitsLoss):
-            if fn.reduction == "mean" and self._per_class(fn.weight) and self._per_class(fn.pos_weight):
-                return _lib.LOSS_BCE, fn.weight, fn.pos_weight
+            if self._per_class(fn.weight) and self._per_class(fn.pos_weight):
+                return _lib.LOSS_BCE, fn.weight, fn.pos_weight, 0.0
         elif isinstance(fn, nn.MultiLabelSoftMarginLoss):
-            if fn.weight is None and fn.reduction == "mean":
-                return _lib.LOSS_MLSM, None, None
+            if fn.weight is None:
+                return _lib.LOSS_MLSM, None, None, 0.0
+        elif type(fn) in (nn.MSELoss, nn.L1Loss):
+            return (_lib.LOSS_MSE if type(fn) is nn.MSELoss else _lib.LOSS_L1), None, None, 0.0
+        elif type(fn) is nn.SmoothL1Loss and fn.beta >= 0:
+            return _lib.LOSS_SMOOTH_L1, None, None, float(fn.beta)
+        elif type(fn) is nn.HuberLoss and fn.delta > 0:
+            return _lib.LOSS_HUBER, None, None, float(fn.delta)
         return None
 
     def _per_class(self, w):
@@ -346,16 +373,29 @@ class BiGRU(_FlatModel):
         return w.dim() >= 1 and w.shape[-1] == self.output_size and all(s == 1 for s in w.shape[:-1])
 
     def _adam_spec(self):
+        """The param_groups of a torch.optim.Adam / AdamW (AdamW is Adam with decoupled weight decay) whose groups hold
+        exactly this model's parameters, each once, else None."""
         opt = self.optimizer
-        if not isinstance(opt, torch.optim.Adam) or len(opt.param_groups) != 1:
+        if not isinstance(opt, torch.optim.Adam) or not 1 <= len(opt.param_groups) <= _lib.ADAM_MAX_GROUPS:
             return None
-        g = opt.param_groups[0]
-        if g.get("weight_decay", 0) != 0 or g.get("amsgrad", False) or g.get("maximize", False):
+        groups = opt.param_groups
+        if any(g.get("amsgrad", False) or g.get("maximize", False) for g in groups):
             return None
         mine = {id(p) for p in self._ordered_params()}
-        if {id(p) for p in g["params"]} != mine:
+        theirs = [id(p) for g in groups for p in g["params"]]
+        if len(theirs) != len(mine) or set(theirs) != mine:
             return None
-        return g
+        return groups
+
+    def _adam_tables(self, groups):
+        """(bigru_adam_group rows, bigru_adam_segment rows) of the optimizer's current param_groups: one row per group, and
+        (offset, count, group) per parameter tensor in the flat vector's order (``_views``)."""
+        hyper = tuple((float(g["lr"]), float(g["betas"][0]), float(g["betas"][1]), float(g["eps"]),
+                       float(g.get("weight_decay", 0.0)), float(bool(g.get("decoupled_weight_decay", False))))
+                      for g in groups)
+        group_of = {id(p): k for k, g in enumerate(groups) for p in g["params"]}
+        segs = tuple((off, n, group_of[id(p)]) for p, (off, n, _) in zip(self._ordered_params(), self._views))
+        return hyper, segs
 
     def can_fuse_step(self) -> bool:
         return self._loss_spec() is not None and self._adam_spec() is not None
@@ -380,13 +420,13 @@ class BiGRU(_FlatModel):
 
     def _fused_state(self):
         if self._adam is None:
-            self._adam = _AdamState(self._flat, self._pad)
+            self._adam = _AdamState(self._flat, self._pad, len(self._views))
             self._import_optimizer_state(self._adam)
             self._mirror_optimizer_state()
         return self._adam
 
     def _import_optimizer_state(self, st):
-        """Moments the user's torch.optim.Adam already holds (generic steps taken before, or a loaded optimizer.state_dict())
+        """Moments the user's torch.optim.Adam / AdamW already holds (generic steps taken before, or a loaded optimizer.state_dict())
         become the fused step's flat moments."""
         opt = getattr(self, "optimizer", None)
         if opt is None:
@@ -408,7 +448,7 @@ class BiGRU(_FlatModel):
         st.dstep.fill_(steps[0])
 
     def _mirror_optimizer_state(self):
-        """optimizer.state[p] = views of the flat moments + a step tensor, in torch.optim.Adam's own format: optimizer.state_dict()
+        """optimizer.state[p] = views of the flat moments + a step tensor, in torch.optim.Adam's (and AdamW's) own format: optimizer.state_dict()
         checkpoints carry the fused step's moments, and a later generic optimizer.step() continues from them (in place)."""
         opt, st = getattr(self, "optimizer", None), self._adam
         if opt is None or st is None or self._adam_spec() is None:
@@ -422,13 +462,13 @@ class BiGRU(_FlatModel):
         """Forward, loss and backward of one step on stream `s`: the loss into st.loss and the gradient of the real parameters
         into st.grad."""
         lib = _lib.load()
-        c, (kind, wv, pwv, denom) = buf.c, buf.loss
+        c, (kind, wv, pwv, denom, param) = buf.c, buf.loss
         pflat = self._plan_params(st.pflat)
         # the loss sees the real batch rows (tgt's); logits / dlogits may carry zero-padded rows behind them
         B, C = buf.tgt.shape[0], buf.logits.shape[1]
         self._forward_c(c.plan, pflat, c.x, c.h0, c.lengths, c.training, c.seed, buf.stash, buf.logits, None, s)
-        _lib.check(lib.bigru_loss(kind, _lib.ptr(buf.logits), _lib.ptr(buf.tgt), _lib.ptr(wv), _lib.ptr(pwv), B, C, denom,
-                                  _lib.ptr(st.loss), _lib.ptr(buf.dlogits), s), "bigru_loss")
+        _lib.check(lib.bigru_loss_param(kind, _lib.ptr(buf.logits), _lib.ptr(buf.tgt), _lib.ptr(wv), _lib.ptr(pwv), B, C, denom,
+                                        param, _lib.ptr(st.loss), _lib.ptr(buf.dlogits), s), "bigru_loss_param")
         self._backward_c(c.plan, pflat, c.x, c.h0, c.lengths, c.training, c.seed, buf.stash, buf.dlogits, st.pgrad, None, None, s)
         self._plan_grads(st.pgrad, st.grad)
 
@@ -448,16 +488,25 @@ class BiGRU(_FlatModel):
                    "bigru_backward_lengths")
 
     def _launch_update(self, g, st, s):
-        """clip_grad_norm_(clip) + Adam on the flat buffers on stream `s`; Adam's step counter is incremented on the device."""
+        """clip_grad_norm_(clip) + Adam / AdamW of the param_groups `g` on the flat buffers on stream `s`, with each group's
+        hyperparameters read from st.hyper on the device; Adam's step counter is incremented on the device."""
         lib = _lib.load()
         sq = st.scal[1:2]
         _lib.check(lib.bigru_adam_tick(_lib.ptr(st.dstep), _lib.ptr(sq), s), "bigru_adam_tick")
         _lib.check(lib.bigru_sqnorm(_lib.ptr(st.grad), st.grad.numel(), _lib.ptr(sq), _lib.ptr(st.sqws), s), "bigru_sqnorm")
-        b1, b2 = g["betas"]
-        _lib.check(lib.bigru_clip_adam_step_dev(_lib.ptr(self._flat), _lib.ptr(st.grad), _lib.ptr(st.m),
-                                                _lib.ptr(st.v), self._flat.numel(), _lib.ptr(sq), float(self.clip),
-                                                float(g["lr"]), float(b1), float(b2), float(g["eps"]), _lib.ptr(st.dstep),
-                                                1.0, s), "bigru_clip_adam_step_dev")
+        _lib.check(lib.bigru_clip_adam_groups_dev(_lib.ptr(self._flat), _lib.ptr(st.grad), _lib.ptr(st.m), _lib.ptr(st.v),
+                                                  self._flat.numel(), _lib.ptr(sq), float(self.clip), _lib.ptr(st.hyper),
+                                                  len(g), _lib.ptr(st.segs), st.segs.shape[0], _lib.ptr(st.dstep), 1.0, s),
+                   "bigru_clip_adam_groups_dev")
+
+    def _graph_key(self, B, T, loss, n_groups, dev, has_lengths):
+        """Key of the captured step graph.  It holds no optimizer hyperparameter: the update reads those from the device
+        table (_AdamState.hyper), so a schedule replays one graph.  clip stays a kernel argument, as the model's own
+        attribute (the reference's constructor argument) that no scheduler touches.  The last element is whether the step
+        has per-row lengths."""
+        kind, wv, pwv, denom, param = loss
+        return (B, T, self.precision, kind, id(wv), id(pwv), denom, param, n_groups, float(self.clip), self._dp_world,
+                dev.index, has_lengths)
 
     def _capture(self, key, buf, st, g):
         """CUDA graph(s) of the step on the static buffers `buf` (SURVEY.md 8(f) N5): one graph at world size 1; with data
@@ -502,19 +551,22 @@ class BiGRU(_FlatModel):
         be checked on the host)."""
         spec, g = self._loss_spec(), self._adam_spec()
         if spec is None or g is None:
-            raise RuntimeError("train_step needs add_loss_fn(CrossEntropyLoss | BCEWithLogitsLoss | "
-                               "MultiLabelSoftMarginLoss, mean reduction) and add_optimizer(torch.optim.Adam(model.parameters()))")
+            raise RuntimeError("train_step needs add_loss_fn(CrossEntropyLoss [weight=] | BCEWithLogitsLoss | "
+                               "MultiLabelSoftMarginLoss | MSELoss | L1Loss | SmoothL1Loss | HuberLoss, mean reduction) and "
+                               "add_optimizer(torch.optim.Adam or AdamW over model.parameters(), any parameter groups, "
+                               "no amsgrad / maximize)")
         lib = _lib.load()
         x, h0 = self._prepare_input(input_seq, hidden)
         lens = self._prepare_lengths(lengths, x, hidden)
         dev = x.device
-        kind, w, pw = spec
+        kind, w, pw, param = spec
         B, C = x.shape[0], self.output_size
-        if kind == _lib.LOSS_CE:
+        if kind in (_lib.LOSS_CE, _lib.LOSS_CE_WEIGHTED):
             tgt = target.to(device=dev, dtype=torch.int64, non_blocking=True).contiguous()
             if tgt.shape != (B,):
                 raise ValueError(f"CrossEntropyLoss target must be [{B}] class indices")
-            denom = float(B * self._dp_world)
+            # weighted CE: each rank's weighted mean (the kernel divides by its own weight sum), averaged over the ranks
+            denom = float((B if kind == _lib.LOSS_CE else 1) * self._dp_world)
         else:
             tgt = target.to(device=dev, dtype=torch.float32, non_blocking=True).contiguous()
             if tuple(tgt.shape) != (B, C):
@@ -525,11 +577,11 @@ class BiGRU(_FlatModel):
             graphed = self.use_cuda_graph and not training and h0 is None and not torch.cuda.is_current_stream_capturing()
             wv, pwv = self._loss_vec(w, C), self._loss_vec(pw, C)
             st = self._fused_state()
+            st.load_tables(*self._adam_tables(g))
             s = _stream_ptr(dev)
             key = ent = None
             if graphed:
-                key = (B, int(x.shape[1]), self.precision, kind, id(wv), id(pwv), denom, float(g["lr"]), tuple(g["betas"]),
-                       float(g["eps"]), float(self.clip), self._dp_world, dev.index, lens is not None)
+                key = self._graph_key(B, int(x.shape[1]), (kind, wv, pwv, denom, param), len(g), dev, lens is not None)
                 ent = self._graphs.get(key)
             if ent is not None:
                 buf, ga, gb, launches = ent
@@ -544,13 +596,14 @@ class BiGRU(_FlatModel):
                 if graphed:                               # a new graph key: this step runs on the graph's static buffers
                     c.x, tgt = c.x.clone(), tgt.clone()
                     c.lengths = None if c.lengths is None else c.lengths.clone()
-                buf = _StepBuffers(c, tgt, (kind, wv, pwv, denom), C)
+                buf = _StepBuffers(c, tgt, (kind, wv, pwv, denom, param), C)
                 compute, update = (lambda: self._launch_compute(buf, st, s)), (lambda: self._launch_update(g, st, s))
             compute()
             if self._dp_world > 1:
                 allreduce_flat_(st.gext, self._dp_group)  # ONE all-reduce: shard gradients of the global-mean loss + the loss
             update()
             st.advance()
+            self.optimizer._opt_called = True                 # torch's mark of a stepped optimizer, which lr schedulers check
             if not graphed:
                 buf.c.plan.release_stash(buf.stash)
             elif ent is None:
@@ -593,10 +646,11 @@ class BiGRU(_FlatModel):
         Returns (loss, logits)."""
         spec = self._loss_spec()
         if spec is None or self._adam_spec() is None:
-            raise RuntimeError("train_step_windows needs a fusable loss and torch.optim.Adam (see train_step)")
+            raise RuntimeError("train_step_windows needs a fusable loss and torch.optim.Adam or AdamW (see train_step)")
         self._window_args(dataset, start, count)
         x, y = dataset.collate(start, count)
-        tgt = y.reshape(count, -1)[:, 0].to(torch.int64) if spec[0] == _lib.LOSS_CE else y.reshape(count, self.output_size)
+        ce = spec[0] in (_lib.LOSS_CE, _lib.LOSS_CE_WEIGHTED)
+        tgt = y.reshape(count, -1)[:, 0].to(torch.int64) if ce else y.reshape(count, self.output_size)
         return self.train_step(x, tgt)
 
     def _generic_step(self, x, target):

@@ -1014,19 +1014,36 @@ extern "C" int bigru_infer_window(const float* d_params, const float* d_x, const
     return BIGRU_OK;
 }
 
-extern "C" int bigru_loss(int kind, const float* d_logits, const void* d_target, const float* d_weight,
-                          const float* d_pos_weight, int B, int C, double denom, float* d_loss, float* d_dlogits,
-                          void* stream) {
-    if (!d_logits || !d_target || !d_loss || B <= 0 || C <= 0 || denom <= 0 || kind < 0 || kind > 2) {
-        bigru_set_error("loss: bad argument");
+extern "C" int bigru_loss_param(int kind, const float* d_logits, const void* d_target, const float* d_weight,
+                                const float* d_pos_weight, int B, int C, double denom, float param, float* d_loss,
+                                float* d_dlogits, void* stream) {
+    if (!d_logits || !d_target || !d_loss || B <= 0 || C <= 0 || denom <= 0 || kind < 0 || kind > BIGRU_LOSS_HUBER ||
+        (kind == BIGRU_LOSS_CE_WEIGHTED && !d_weight) || (kind == BIGRU_LOSS_SMOOTH_L1 && !(param >= 0.f && std::isfinite(param))) ||
+        (kind == BIGRU_LOSS_HUBER && !(param > 0.f && std::isfinite(param)))) {
+        bigru_set_error("loss: bad argument (kind %d, B %d, C %d, param %g)", kind, B, C, (double)param);
         return BIGRU_ERR_ARG;
     }
     cudaStream_t st = (cudaStream_t)stream;
     CUDA_TRY(cudaMemsetAsync(d_loss, 0, sizeof(float), st));
-    if (kind == BIGRU_LOSS_MLSM) { d_weight = nullptr; d_pos_weight = nullptr; }
-    KLAUNCH(KC_LOSS, 0.0, 0.0, st, loss_kernel<<<1, 256, 0, st>>>(kind, d_logits, d_target, d_weight, d_pos_weight, B, C,
-                                             (float)(1.0 / denom), d_loss, d_dlogits));
+    if (kind <= BIGRU_LOSS_MLSM) {
+        if (kind == BIGRU_LOSS_MLSM) { d_weight = nullptr; d_pos_weight = nullptr; }
+        KLAUNCH(KC_LOSS, 0.0, 0.0, st, loss_kernel<<<1, 256, 0, st>>>(kind, d_logits, d_target, d_weight, d_pos_weight, B, C,
+                                                 (float)(1.0 / denom), d_loss, d_dlogits));
+    } else {
+        KLAUNCH(KC_LOSS, 0.0, 0.0, st, loss_param_kernel<<<1, 256, 0, st>>>(kind, d_logits, d_target, d_weight, B, C, param,
+                                                       (float)(1.0 / denom), d_loss, d_dlogits));
+    }
     return BIGRU_OK;
+}
+
+extern "C" int bigru_loss(int kind, const float* d_logits, const void* d_target, const float* d_weight,
+                          const float* d_pos_weight, int B, int C, double denom, float* d_loss, float* d_dlogits,
+                          void* stream) {
+    if (kind < 0 || kind > BIGRU_LOSS_MLSM) {
+        bigru_set_error("loss: bad argument (kind %d; the other kinds are bigru_loss_param's)", kind);
+        return BIGRU_ERR_ARG;
+    }
+    return bigru_loss_param(kind, d_logits, d_target, d_weight, d_pos_weight, B, C, denom, 0.f, d_loss, d_dlogits, stream);
 }
 
 extern "C" int bigru_sqnorm(const float* d_g, int64_t n, float* d_out, float* d_ws, void* stream) {
@@ -1044,6 +1061,16 @@ extern "C" int bigru_adam_tick(int* d_step, float* d_sqnorm, void* stream) {
     return BIGRU_OK;
 }
 
+static int clip_adam_launch(float* d_params, float* d_grads, float* d_m, float* d_v, int64_t n, const float* d_sqnorm,
+                            float clip, const bigru_adam_group* d_groups, int n_groups, bigru_adam_group one,
+                            const bigru_adam_segment* d_segments, int n_segments, const int* d_step, float grad_scale,
+                            void* stream) {
+    const unsigned blocks = (unsigned)min((int64_t)132 * 8, cdiv64(n, 256));
+    KLAUNCH(KC_OPTIM, 0.0, 0.0, (cudaStream_t)stream, clip_adam_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d_params, d_grads, d_m, d_v, n, d_sqnorm, clip,
+                                                                    d_groups, n_groups, one, d_segments, n_segments, d_step, grad_scale));
+    return BIGRU_OK;
+}
+
 extern "C" int bigru_clip_adam_step_dev(float* d_params, float* d_grads, float* d_m, float* d_v, int64_t n,
                                         const float* d_sqnorm, float clip, float lr, float b1, float b2, float eps,
                                         const int* d_step, float grad_scale, void* stream) {
@@ -1051,10 +1078,23 @@ extern "C" int bigru_clip_adam_step_dev(float* d_params, float* d_grads, float* 
         bigru_set_error("clip_adam_step_dev: bad argument");
         return BIGRU_ERR_ARG;
     }
-    const unsigned blocks = (unsigned)min((int64_t)132 * 8, cdiv64(n, 256));
-    KLAUNCH(KC_OPTIM, 0.0, 0.0, (cudaStream_t)stream, clip_adam_dev_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d_params, d_grads, d_m, d_v, n, d_sqnorm, clip,
-                                                                    lr, b1, b2, eps, d_step, grad_scale));
-    return BIGRU_OK;
+    const bigru_adam_group one = {lr, b1, b2, eps, 0.f, 0.f};
+    return clip_adam_launch(d_params, d_grads, d_m, d_v, n, d_sqnorm, clip, nullptr, 1, one, nullptr, 0, d_step, grad_scale,
+                            stream);
+}
+
+extern "C" int bigru_clip_adam_groups_dev(float* d_params, float* d_grads, float* d_m, float* d_v, int64_t n,
+                                          const float* d_sqnorm, float clip, const bigru_adam_group* d_groups, int n_groups,
+                                          const bigru_adam_segment* d_segments, int n_segments, const int* d_step,
+                                          float grad_scale, void* stream) {
+    if (!d_params || !d_grads || !d_m || !d_v || !d_sqnorm || !d_step || !d_groups || !d_segments || n <= 0 ||
+        n_groups < 1 || n_groups > BIGRU_ADAM_MAX_GROUPS || n_segments < 1) {
+        bigru_set_error("clip_adam_groups_dev: bad argument (n %lld, %d groups, %d segments)", (long long)n, n_groups,
+                        n_segments);
+        return BIGRU_ERR_ARG;
+    }
+    return clip_adam_launch(d_params, d_grads, d_m, d_v, n, d_sqnorm, clip, d_groups, n_groups, bigru_adam_group{},
+                            d_segments, n_segments, d_step, grad_scale, stream);
 }
 
 extern "C" int bigru_window_gather_norm(const float* d_src, const float* d_xmin, const float* d_xmax, int64_t start,

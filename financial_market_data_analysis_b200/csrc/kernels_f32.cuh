@@ -387,6 +387,81 @@ __global__ void loss_kernel(int kind, const float* __restrict__ logits, const vo
     }
 }
 
+// The kinds bigru_loss_param adds, in a kernel of their own so that loss_kernel's arithmetic stays as it was.  Weighted CE
+// first sums the targets' weights (every thread needs the sum for dlogits), in the fixed order of the loss's own sum.
+__device__ __forceinline__ float block_sum_fixed(float v, float* sm) {       // the total is in warp 0
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float t = 0.f;
+    if (threadIdx.x < 32) {
+        t = threadIdx.x < (blockDim.x >> 5) ? sm[threadIdx.x] : 0.f;
+        for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    }
+    return t;
+}
+
+__global__ void loss_param_kernel(int kind, const float* __restrict__ logits, const void* __restrict__ target,
+                                  const float* __restrict__ weight, int B, int C, float param, float inv_denom,
+                                  float* __restrict__ loss, float* __restrict__ dlogits) {
+    __shared__ float sm[32];
+    __shared__ float wsum;
+    if (kind == BIGRU_LOSS_CE_WEIGHTED) {
+        float ws = 0.f;
+        for (int b = threadIdx.x; b < B; b += blockDim.x) {
+            const long long tg = ((const long long*)target)[b];
+            ws += tg >= 0 && tg < C ? weight[tg] : nanf("");
+        }
+        ws = block_sum_fixed(ws, sm);
+        if (threadIdx.x == 0) wsum = ws;
+        __syncthreads();
+        inv_denom = inv_denom / wsum;                           // 0 / 0 = NaN when every target weight is 0, as torch
+    }
+    // SmoothL1 with beta 0 is L1 (torch calls l1_loss for it)
+    const int k = kind == BIGRU_LOSS_SMOOTH_L1 && param == 0.f ? BIGRU_LOSS_L1 : kind;
+    float l = 0.f;
+    for (int b = threadIdx.x; b < B; b += blockDim.x) {
+        const float* lg = logits + (int64_t)b * C;
+        if (k == BIGRU_LOSS_CE_WEIGHTED) {
+            // a target outside [0, C) poisons its row with NaN, as in loss_kernel
+            const long long tg = ((const long long*)target)[b];
+            const bool valid = tg >= 0 && tg < C;
+            float m = lg[0];
+            for (int c = 1; c < C; ++c) m = fmaxf(m, lg[c]);
+            float s = 0.f;
+            for (int c = 0; c < C; ++c) s += expf(lg[c] - m);
+            const float lse = m + logf(s);
+            const float w = valid ? weight[tg] : nanf("");
+            l += w * (lse - (valid ? lg[tg] : nanf("")));
+            if (dlogits)
+                for (int c = 0; c < C; ++c)
+                    dlogits[(int64_t)b * C + c] = valid ? (expf(lg[c] - lse) - (c == tg ? 1.f : 0.f)) * (w * inv_denom) : nanf("");
+            continue;
+        }
+        // the regressions: torch's forward and backward formulas branch for branch, so the kinks take torch's gradient
+        const float* tg = (const float*)target + (int64_t)b * C;
+        for (int c = 0; c < C; ++c) {
+            const float d = lg[c] - tg[c], ad = fabsf(d);
+            float val, gr;
+            if (k == BIGRU_LOSS_MSE) {
+                val = d * d; gr = 2.f * d;
+            } else if (k == BIGRU_LOSS_L1) {
+                val = ad; gr = d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f);
+            } else if (k == BIGRU_LOSS_SMOOTH_L1) {
+                val = ad < param ? 0.5f * d * d / param : ad - 0.5f * param;
+                gr = d < -param ? -1.f : (d > param ? 1.f : d / param);
+            } else {                                            // Huber
+                val = ad < param ? 0.5f * d * d : param * (ad - 0.5f * param);
+                gr = d < -param ? -param : (d > param ? param : d);
+            }
+            l += val;
+            if (dlogits) dlogits[(int64_t)b * C + c] = gr * inv_denom;
+        }
+    }
+    const float v = block_sum_fixed(l, sm);
+    if (threadIdx.x == 0) *loss += v * inv_denom;
+}
+
 // ------------------------------------------------------------------------------------------
 // clip_grad_norm_ + Adam over the flat buffers
 // ------------------------------------------------------------------------------------------
@@ -421,23 +496,52 @@ __global__ void sqnorm_finish_kernel(const float* __restrict__ ws, int nblocks, 
 __global__ void adam_tick_kernel(int* __restrict__ step, float* __restrict__ sqnorm) {
     if (threadIdx.x == 0 && blockIdx.x == 0) { *step += 1; *sqnorm = 0.f; }
 }
-__global__ void clip_adam_dev_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
-                                     float* __restrict__ v, int64_t n, const float* __restrict__ sqnorm, float clip,
-                                     float lr, float b1, float b2, float eps, const int* __restrict__ step_p, float gscale) {
+// clip coefficient, then Adam / AdamW per parameter group.  Each block forms every group's step-dependent constants once
+// (in double, as before) into shared memory.  Without a table (groups == nullptr) the one group is `one` and the one
+// segment is [0, n).  A thread walks its grid-stride elements in increasing order, so its segment cursor only moves on.
+__global__ void clip_adam_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m,
+                                 float* __restrict__ v, int64_t n, const float* __restrict__ sqnorm, float clip,
+                                 const bigru_adam_group* __restrict__ groups, int G, bigru_adam_group one,
+                                 const bigru_adam_segment* __restrict__ seg, int S, const int* __restrict__ step_p,
+                                 float gscale) {
+    __shared__ bigru_adam_group h_s[BIGRU_ADAM_MAX_GROUPS];
+    __shared__ float step_s[BIGRU_ADAM_MAX_GROUPS], bc2_s[BIGRU_ADAM_MAX_GROUPS], decay_s[BIGRU_ADAM_MAX_GROUPS];
     const int step_i = *step_p;
-    const float bc1 = (float)(1.0 - pow((double)b1, (double)step_i));
-    const float bc2_sqrt = (float)sqrt(1.0 - pow((double)b2, (double)step_i));
+    for (int k = threadIdx.x; k < G; k += blockDim.x) {
+        const bigru_adam_group h = groups ? groups[k] : one;
+        const float bc1 = (float)(1.0 - pow((double)h.beta1, (double)step_i));
+        bc2_s[k] = (float)sqrt(1.0 - pow((double)h.beta2, (double)step_i));
+        step_s[k] = h.lr / bc1;
+        decay_s[k] = (float)(1.0 - (double)h.lr * (double)h.weight_decay);
+        h_s[k] = h;
+    }
+    __syncthreads();
     const float norm = sqrtf(*sqnorm) * gscale;
     const float coef = fminf(1.f, clip / (norm + 1e-6f)) * gscale;
-    const float step = lr / bc1;
+    int s = 0;
+    int64_t lo = 0, hi = n, gi = 0;                               // the current segment [lo, hi) and its group
+    if (seg) { lo = seg[0].offset; hi = lo + seg[0].count; gi = seg[0].group; }
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        if (seg) {
+            while (i >= hi && s + 1 < S) { ++s; lo = seg[s].offset; hi = lo + seg[s].count; gi = seg[s].group; }
+            if (i < lo || i >= hi || gi < 0 || gi >= G) continue;
+        }
+        const bigru_adam_group& h = h_s[gi];
         const float gq = g[i] * coef;
         g[i] = gq;
-        const float mi = m[i] + (gq - m[i]) * (1.f - b1);        // lerp, as torch.optim.Adam does
-        const float vi = v[i] * b2 + (1.f - b2) * gq * gq;
+        float pi = p[i], ge = gq;
+        if (h.weight_decay != 0.f) {
+            if (h.decoupled != 0.f) pi = pi * decay_s[gi];            // AdamW, as torch.optim.AdamW
+            else ge = gq + h.weight_decay * pi;                       // L2 into the gradient, as torch.optim.Adam
+        }
+        // the roundings of the single-group kernel this one replaced, spelled out with intrinsics so that the compiler's
+        // contraction choices cannot change them: m + (g - m)(1 - b1) (a lerp, as torch.optim.Adam),
+        // v b2 + ((1 - b2) g) g with one rounding after the last product, p - step (m / denom)
+        const float mi = __fmaf_rn(ge - m[i], 1.f - h.beta1, m[i]);
+        const float vi = __fmaf_rn(__fmul_rn(1.f - h.beta2, ge), ge, __fmul_rn(v[i], h.beta2));
         m[i] = mi; v[i] = vi;
-        const float denom = sqrtf(vi) / bc2_sqrt + eps;
-        p[i] = p[i] - step * (mi / denom);
+        const float denom = sqrtf(vi) / bc2_s[gi] + h.eps;
+        p[i] = __fmaf_rn(mi / denom, -step_s[gi], pi);
     }
 }
 

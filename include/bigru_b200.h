@@ -59,6 +59,12 @@ extern "C" {
 #define BIGRU_LOSS_CE   0          /* torch.nn.CrossEntropyLoss (BASELINE.json configs) */
 #define BIGRU_LOSS_BCE  1          /* torch.nn.BCEWithLogitsLoss(weight,pos_weight) notebook raw :1192 */
 #define BIGRU_LOSS_MLSM 2          /* torch.nn.MultiLabelSoftMarginLoss  predict.py:94 */
+/* bigru_loss_param only: */
+#define BIGRU_LOSS_CE_WEIGHTED 3   /* torch.nn.CrossEntropyLoss(weight=w) */
+#define BIGRU_LOSS_MSE         4   /* torch.nn.MSELoss */
+#define BIGRU_LOSS_L1          5   /* torch.nn.L1Loss */
+#define BIGRU_LOSS_SMOOTH_L1   6   /* torch.nn.SmoothL1Loss(beta = param) */
+#define BIGRU_LOSS_HUBER       7   /* torch.nn.HuberLoss(delta = param) */
 
 typedef struct bigru_plan bigru_plan;
 
@@ -268,6 +274,18 @@ int  bigru_cell_backward(int B, int I, int H, int precision, const float* d_para
 int  bigru_loss(int kind, const float* d_logits, const void* d_target, const float* d_weight,
                 const float* d_pos_weight, int B, int C, double denom, float* d_loss,
                 float* d_dlogits, void* stream);
+/*  bigru_loss_param: every kind above, with the scalar `param` of the kinds that have one (SmoothL1's beta >= 0,
+ *  Huber's delta > 0; ignored otherwise).  Kinds 0-2 compute bitwise what bigru_loss computes (which calls this).
+ *  CE_WEIGHTED: d_target int64[B] as CE, d_weight [C] required; loss = sum_b w[y_b] nll_b / (W * denom) with
+ *  W = sum_b w[y_b] formed in the same launch in a fixed order, i.e. torch's weighted mean when denom = 1.  Under data
+ *  parallelism pass denom = world size: the all-reduced sum is then the mean over ranks of each rank's weighted mean.
+ *  W = 0 (every target weight zero) gives a NaN loss and NaN dlogits, as torch does.  Targets outside [0, C) as CE.
+ *  MSE / L1 / SMOOTH_L1 / HUBER: d_target float[B,C], mean over denom (B*C, times the world size under data
+ *  parallelism), d_weight / d_pos_weight ignored.  The gradient at the kinks is torch's: L1 gives 0 where x == y,
+ *  SmoothL1 with beta = 0 is L1, and at |x - y| == beta (delta) both take the quadratic side's value. */
+int  bigru_loss_param(int kind, const float* d_logits, const void* d_target, const float* d_weight,
+                      const float* d_pos_weight, int B, int C, double denom, float param, float* d_loss,
+                      float* d_dlogits, void* stream);
 
 /* --- nn.utils.clip_grad_norm_ + optimizer.step() (biGRU_model.py:208-210, Adam, notebook raw :1194)
  *  bigru_sqnorm accumulates sum(g^2) into *d_out (caller zeroes it first); d_ws: BIGRU_SQNORM_WS floats of
@@ -282,6 +300,24 @@ int  bigru_adam_tick(int* d_step, float* d_sqnorm, void* stream);
 int  bigru_clip_adam_step_dev(float* d_params, float* d_grads, float* d_m, float* d_v, int64_t n,
                               const float* d_sqnorm, float clip, float lr, float b1, float b2, float eps,
                               const int* d_step, float grad_scale, void* stream);
+
+/* --- the same clip + update with its hyperparameters in device memory, one set per parameter group
+ *  (torch.optim.Adam / AdamW param_groups), so that a captured CUDA graph of the step follows a learning-rate schedule.
+ *  d_groups [n_groups] (1 <= n_groups <= BIGRU_ADAM_MAX_GROUPS); d_segments [n_segments] (>= 1): ranges of the flat
+ *  vector sorted by offset and disjoint, each updated with the hyperparameters of its group.  An element outside every
+ *  segment, or in a segment whose group is outside [0, n_groups), is left as it is (p, g, m and v).  Per element,
+ *  after the clip of bigru_clip_adam_step_dev:
+ *    weight_decay != 0 and decoupled (AdamW):  p *= 1 - lr * weight_decay   (formed in double), then Adam on g;
+ *    weight_decay != 0, not decoupled (Adam):  Adam on g + weight_decay * p  (g itself keeps the clipped gradient);
+ *  and the Adam update and bias corrections of bigru_clip_adam_step_dev.  bigru_clip_adam_step_dev is this update with
+ *  one group (lr, b1, b2, eps, no weight decay) and one segment [0, n).  No atomics, each element written once. */
+#define BIGRU_ADAM_MAX_GROUPS 64
+typedef struct { float lr, beta1, beta2, eps, weight_decay, decoupled; } bigru_adam_group;  /* decoupled: 0 or 1 */
+typedef struct { int64_t offset, count, group; } bigru_adam_segment;
+int  bigru_clip_adam_groups_dev(float* d_params, float* d_grads, float* d_m, float* d_v, int64_t n,
+                                const float* d_sqnorm, float clip, const bigru_adam_group* d_groups, int n_groups,
+                                const bigru_adam_segment* d_segments, int n_segments, const int* d_step,
+                                float grad_scale, void* stream);
 
 /* --- MySQLBatchLoader collation (sql_pytorch_dataloader.py:239-245 + default_collate):
  *  out[b,t,f] = (s - xmin[f]) / (xmax[f] - xmin[f]), an IEEE float division, with s = src[start+b+t, f] and a NaN s
