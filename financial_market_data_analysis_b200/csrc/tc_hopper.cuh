@@ -184,10 +184,16 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         }
     }
 }
-// bytes from this CTA's shared memory to CTA `cta` of the cluster, at the same offsets; completes on that CTA's mbarrier
-__device__ __forceinline__ void bulk_copy_to_peer(uint32_t src, uint32_t bytes, uint64_t* bar, uint32_t cta) {
+// bytes from this CTA's shared memory at src to CTA `cta` of the cluster at dst (an offset in this CTA's shared window,
+// mapped to the peer's); completes on that CTA's mbarrier.  Only the peer's mbarrier tracks the copy: no bulk group does, so
+// the source may be rewritten only once the peer has reported the phase complete
+__device__ __forceinline__ void bulk_copy_to_peer_at(uint32_t dst, uint32_t src, uint32_t bytes, uint64_t* bar, uint32_t cta) {
     asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(mapa(src, cta)), "r"(src), "r"(bytes), "r"(mapa(smem_u32(bar), cta)) : "memory");
+                 ::"r"(mapa(dst, cta)), "r"(src), "r"(bytes), "r"(mapa(smem_u32(bar), cta)) : "memory");
+}
+// the same at the same offset in the peer
+__device__ __forceinline__ void bulk_copy_to_peer(uint32_t src, uint32_t bytes, uint64_t* bar, uint32_t cta) {
+    bulk_copy_to_peer_at(src, src, bytes, bar, cta);
 }
 __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
@@ -727,23 +733,46 @@ gru_scan_fwd_kernel(const float* __restrict__ gi, const float* __restrict__ Whh,
 // forward; dY [B][T][D*H]; dhc [D][B][H] carries dh into the layer's last step (head / zero) and returns dh_{-1};
 // dgi, dgh [D][B*T][3H], and their bf16 planes gih/gil, ghh/ghl in the same layout for the GEMMs.  The dgh planes hold
 // zeros at each sequence's first step (t = 0 for d = 0, t = T-1 for d = 1): that row pairs with h0 (covered from fp32 dgh),
-// so dW_hh = dgh^T H_prev needs no row mask.  Shared memory: W^T rows (H) x own gate rows (192) | dgh tile [16][192] | receive slots of the
-// peers' partial sums [CS-1][64][16] fp32 (k-major, xslot; this CTA's own partial goes into the dgh tile's space, which is free by then).
-// Cluster barrier phases per step: (1) partials of the step have landed; (2) every CTA has read its receive slots, so
-// the next step's partials may be written.
+// so dW_hh = dgh^T H_prev needs no row mask.  Shared memory: W^T rows (H) x own gate rows (192) | region X | receive slots of
+// the peers' partial sums [CS-1][64][16] fp32 (k-major, xslot) | (BULK) full and empty mbarriers.  X holds the dgh tile
+// [NH][16][192] bf16 from the gate math to the multiply, then the step's partial sums.
+// BULK (H <= 256): X holds this CTA's partial for every owner CTA, block X[dst] = [U][NB] fp32 in xslot order (the own one
+// at X[c]), written with local stores; one thread sends block X[dst] to dst's receive slot of source c with one bulk copy
+// per peer, completing on dst's "full" mbarrier, and a CTA waits on its own full before it reads its slots.  After reading
+// them, threads 0 .. CS - 2 each arrive on one peer's "empty" mbarrier; a CTA waits on its own empty (phase s - 1 at step
+// s) after the gate math, before it writes the dgh tile into X.  There is no cluster barrier per step.
+//   * No peer copies into a receive slot that is still being read: a peer's step-s copy into this CTA follows the peer's
+//     empty wait of phase s - 1, which needs this CTA's arrive, which follows the __syncthreads after which every thread of
+//     this CTA has read its step-(s - 1) slots.
+//   * No complete_tx lands in the wrong phase of full: this CTA waits on phase s - 1 and then (thread 0) arms phase s
+//     with its (CS - 1) * SLOT bytes before that __syncthreads and arrive, so every step-s copy into this CTA is issued
+//     after phase s - 1 completed and phase s expects it.  Phase 0 is armed before the starting cluster barrier.
+//   * X is rewritten only after the copies out of it are done: those copies are tracked by the peers' full barriers alone
+//     (no bulk group), so the empty wait before the dgh tile write is what shows it: every peer arrived after its full
+//     wait of phase s - 1, which completed when this CTA's step-(s - 1) copy into it had landed.  The own block X[c] is read
+//     before the __syncthreads that precedes that write.
+//   Arrives release and waits acquire at cluster scope; the copies' complete_tx does the same.
+// At H = 512 the 28 KB of receive slots and 32 KB of outgoing blocks next to the 192 KB of W^T exceed the 227 KB a block may
+// use, so there the partials go out as remote stores and two cluster barrier phases per step keep order: (1) partials of
+// the step have landed; (2) every CTA has read its receive slots, so the next step's partials may be written.  The own
+// partial then sits at the start of X.
 // LEN: at a padded (row, t >= lens[b]) dgi and dgh are 0 (fp32 and planes) and dh passes through unchanged: its dgh row
 // adds exact zeros to the partial sums.  The barriers and the exchange are those of every step.
 // ------------------------------------------------------------------------------------------------------
 template <int H, int NS>
 struct BwdSmem {
     static constexpr int NH = NS == 1 ? 1 : 2;
+    static constexpr int CS = H / SCAN_U;
     static constexpr int Q = 3 * SCAN_U;                   // own gate rows
     static constexpr int WP = Q * 2;                        // W^T row pitch (bytes)
     static constexpr int WBYTES = H * WP;
     static constexpr int DBYTES = SCAN_NB * Q * 2;
     static constexpr int SLOT = SCAN_NB * SCAN_U * 4;
-    static constexpr int TOTAL = NH * WBYTES + NH * DBYTES + (H / SCAN_U - 1) * SLOT;
+    static constexpr bool BULK = H <= 256;                  // outgoing blocks in X fit next to W^T (see above)
+    static constexpr int XBYTES = BULK && CS * SLOT > NH * DBYTES ? CS * SLOT : NH * DBYTES;
+    static constexpr int TOTAL = NH * WBYTES + XBYTES + (CS - 1) * SLOT + (BULK ? 2 * 8 : 0);
     static_assert(NH * DBYTES >= SLOT, "own partial sums alias the dgh tile");
+    static_assert(TOTAL <= 232448, "an H100 block's shared memory");
 };
 
 // float index of the partial sum for (unit kl, batch column b) in a receive slot: k-major [U][NB], so a thread's two
@@ -774,12 +803,14 @@ __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, c
     constexpr int NBLK = NR / 8;                             // n8 blocks of the tile
     extern __shared__ __align__(128) uint8_t smem[];
     uint8_t* Wsm = smem;                                     // [NH][H rows][Q]
-    uint8_t* Dsm = smem + NH * S::WBYTES;                    // [NH][NB rows][Q]; also this CTA's own partial [U][NB] fp32
-    float* recv = reinterpret_cast<float*>(Dsm + NH * S::DBYTES);   // [CS-1][U][NB] (xslot)
+    uint8_t* Dsm = smem + NH * S::WBYTES;                    // X: [NH][NB rows][Q] dgh tile; then partials [CS or 1][U][NB] fp32
+    float* recv = reinterpret_cast<float*>(Dsm + S::XBYTES);   // [CS-1][U][NB] (xslot)
+    uint64_t* full = reinterpret_cast<uint64_t*>(recv + (CS - 1) * NB * U);   // BULK
+    uint64_t* empty = full + 1;
     const int c = (int)cluster_rank();
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const float* W = Whh + d * zW;
-    float* own = reinterpret_cast<float*>(Dsm);
+    float* own = reinterpret_cast<float*>(Dsm + (S::BULK ? c * S::SLOT : 0));
     auto slot = [&](int src) -> float* { return src == c ? own : recv + (src < c ? src : src - 1) * NB * U; };
 
     for (int i = tid; i < Q * H; i += SCAN_THREADS) {
@@ -800,16 +831,21 @@ __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, c
         plen[i] = LEN ? lens[bt0 + b] : T;
         if constexpr (RD) mk[i] = mask[((int64_t)d * B + bt0 + b) * H + c * U + u];
     }
+    if (S::BULK && tid == 0) {
+        mbar_init(full, 1);
+        mbar_init(empty, CS - 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_arrive_expect_tx(full, (CS - 1) * S::SLOT);     // phase 0: step 0's partials
+    }
+    // every CTA of the cluster has started and initialised its barriers before any remote store, bulk copy or arrive
     cluster_arrive();
     cluster_wait();
 
     const int DH = D * H;
     // the step's operands from global memory: G (r, z, n, W_hn h + b_hn), h_{t-1} (Y, or h0 at the first step) and dY.
     // Step s + 1's are loaded during step s, so their latency hides behind the rest of the step and the dgh tile waits only
-    // for the incoming dh.  Where they are issued was measured per precision at configs[1] (per-phase clock64 stamps on an
-    // H100): at bf16x3 after the multiply, when the step's dgi / dgh / plane stores have drained (about 600 cycles per step
-    // less than right after the gate math); at bf16 right after the gate math (about 500 cycles less than after the
-    // multiply, where the loads delay the partial-sum exchange).
+    // for the incoming dh.  They are issued right after the gate math at both precisions: at configs[1] on an H100 that
+    // ran the backward scan 0.03 ms faster at bf16x3 than issuing them after the multiply, and 0.2 ms faster at bf16.
     float gr[PAIRS], gz[PAIRS], gn[PAIRS], ghn[PAIRS], hprev[PAIRS], dyv[PAIRS];
     auto load_step = [&](int s) {
         const int t = d == 0 ? T - 1 - s : s;
@@ -831,6 +867,10 @@ __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, c
         const int t = d == 0 ? T - 1 - s : s;
         const bool first = d == 0 ? t == 0 : t == T - 1;
         if (s > 0) {
+            if constexpr (S::BULK) {
+                mbar_wait<true>(full, (s - 1) & 1);          // the peers' partials of step s - 1 have landed
+                if (tid == 0) mbar_arrive_expect_tx(full, (CS - 1) * S::SLOT);   // phase s: this step's
+            }
 #pragma unroll
             for (int i = 0; i < PAIRS; ++i) {
                 const int p = tid + i * SCAN_THREADS, x = xslot(p % U, p / U);
@@ -842,8 +882,11 @@ __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, c
                 dhr[i] = v;
             }
         }
-        cluster_arrive();                                    // phase (2): this CTA's receive slots are read
+        if constexpr (!S::BULK) cluster_arrive();            // phase (2): this CTA's receive slots are read
         __syncthreads();                                     // own partial read before the dgh tile is rewritten
+        // this CTA's receive slots are read: tell every peer (threads 0 .. CS - 2, one peer each)
+        if (S::BULK && s > 0 && tid < CS - 1) mbar_arrive_peer(empty, (c + 1 + tid) % CS);
+        float gv[PAIRS][3];
 #pragma unroll
         for (int i = 0; i < PAIRS; ++i) {
             const int p = tid + i * SCAN_THREADS, u = p % U, bl = p / U, b = bt0 + bl, j = c * U + u;
@@ -861,14 +904,7 @@ __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, c
             a[0] = dar; a[H] = daz; a[2 * H] = dan;
             cg[0] = dar; cg[H] = daz; cg[2 * H] = dgn;
             dhz[i] = pad ? dhr[i] : dh * z;
-            const float gv[3] = {dar, daz, dgn};
-#pragma unroll
-            for (int gte = 0; gte < 3; ++gte) {
-                bf16_t hi, lo;
-                split_bf16(gv[gte], hi, lo);
-                *reinterpret_cast<bf16_t*>(Dsm + swz<S::WP>(bl, gte * U + u)) = hi;
-                if (NH == 2) *reinterpret_cast<bf16_t*>(Dsm + S::DBYTES + swz<S::WP>(bl, gte * U + u)) = lo;
-            }
+            gv[i][0] = dar; gv[i][1] = daz; gv[i][2] = dgn;
             // dgi's n gate is dan (dgh's is dgn = dan * r); its r and z gates equal dgh's and leave from the dgh tile below
             bf16_t hi, lo;
             split_bf16(dan, hi, lo);
@@ -876,7 +912,21 @@ __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, c
             gih[po] = hi;
             if (NH == 2) gil[po] = lo;
         }
-        if (NS == 1 && s + 1 < T) load_step(s + 1);
+        // every peer has read its slots of step s - 1, so this CTA's copies of that step out of X are done, and the
+        // peers' slots are free for this step's
+        if (S::BULK && s > 0) mbar_wait<true>(empty, (s - 1) & 1);
+#pragma unroll
+        for (int i = 0; i < PAIRS; ++i) {
+            const int p = tid + i * SCAN_THREADS, u = p % U, bl = p / U;
+#pragma unroll
+            for (int gte = 0; gte < 3; ++gte) {
+                bf16_t hi, lo;
+                split_bf16(gv[i][gte], hi, lo);
+                *reinterpret_cast<bf16_t*>(Dsm + swz<S::WP>(bl, gte * U + u)) = hi;
+                if (NH == 2) *reinterpret_cast<bf16_t*>(Dsm + S::DBYTES + swz<S::WP>(bl, gte * U + u)) = lo;
+            }
+        }
+        if (s + 1 < T) load_step(s + 1);
         __syncthreads();
         // planes of this step's rows from the dgh tile, 16-byte stores: dgh (zeros at a sequence's first step) and dgi's r, z
         for (int i = tid; i < NH * NR * (Q / 8); i += SCAN_THREADS) {
@@ -918,9 +968,8 @@ __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, c
                 }
             }
         }
-        if (NS != 1 && s + 1 < T) load_step(s + 1);
-        __syncthreads();                                     // dgh tile consumed: its space takes the own partial
-        cluster_wait();                                      // phase (2) complete: peers' receive slots are free
+        __syncthreads();                                     // dgh tile consumed: its space takes the partials
+        if constexpr (!S::BULK) cluster_wait();              // phase (2) complete: peers' receive slots are free
         // accumulators e = 0, 1 (and 2, 3) are adjacent batch columns of one unit: one 8-byte store each
 #pragma unroll
         for (int m = 0; m < MT; ++m)
@@ -932,7 +981,9 @@ __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, c
                     const int bl = n * 8 + 2 * (lane & 3);
                     const int dst = k / U, x = xslot(k % U, bl);
                     const float2 v = make_float2(acc[m][n][e], acc[m][n][e + 1]);
-                    if (dst == c) {
+                    if (S::BULK) {
+                        *reinterpret_cast<float2*>(Dsm + dst * S::SLOT + x * 4) = v;
+                    } else if (dst == c) {
                         *reinterpret_cast<float2*>(own + x) = v;
                     } else {
                         // at CTA dst, the slot of source c is (c < dst ? c : c - 1)
@@ -940,9 +991,26 @@ __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, c
                         st_cluster_v2_f32(mapa(smem_u32(rs), dst), v);
                     }
                 }
-        cluster_arrive();                                    // phase (1): this step's partial sums are delivered
-        cluster_wait();
+        if constexpr (S::BULK) {
+            // the blocks of X are complete; make them visible to the bulk copies (async proxy), then send one to each peer:
+            // all of its slot, also from an 8-row tile (xslot spreads its columns over all 16).  The last step's go to the
+            // final dh_{-1} sum below
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            __syncthreads();
+            if (tid == 0) {
+#pragma unroll
+                for (int p = 1; p < CS; ++p) {
+                    const int dst = (c + p) % CS;
+                    bulk_copy_to_peer_at(smem_u32(recv + (c < dst ? c : c - 1) * NB * U), smem_u32(Dsm + dst * S::SLOT),
+                                         S::SLOT, full, dst);
+                }
+            }
+        } else {
+            cluster_arrive();                                // phase (1): this step's partial sums are delivered
+            cluster_wait();
+        }
     }
+    if constexpr (S::BULK) mbar_wait<true>(full, (T - 1) & 1);   // the peers' partials of the last step have landed
 #pragma unroll
     for (int i = 0; i < PAIRS; ++i) {
         const int p = tid + i * SCAN_THREADS, u = p % U, b = p / U, x = xslot(u, b);
@@ -951,6 +1019,11 @@ __device__ __forceinline__ void gru_scan_bwd_tile(const float* __restrict__ G, c
         for (int src = 0; src < CS; ++src) v += slot(src)[x];
         if constexpr (RD) v = LEN && (d == 0 ? 0 : T - 1) >= plen[i] ? v : mk[i] * v;
         dhc[((int64_t)d * B + bt0 + b) * H + c * U + u] = v;
+    }
+    if constexpr (S::BULK) {
+        // no CTA leaves while a bulk copy out of its shared memory may be in flight
+        cluster_arrive();
+        cluster_wait();
     }
 }
 
