@@ -36,6 +36,7 @@ SIGNATURES = {
     "bigru_stash_output_offset": (_i, [_vp, _i, C.POINTER(C.c_size_t)]),
     "bigru_workspace_region": (_i, [_vp, _i, _i, C.POINTER(_i), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(_i64)]),
     "bigru_scan_geometry": (_i, [_vp, _i, C.POINTER(_i), C.POINTER(_i)]),
+    "bigru_plan_set_backward_stop": (_i, [_vp, _i]),
     "bigru_tc_gemm_workspace_bytes": (_i, [_i, _i, _i, _i, _i, _i, _i, C.POINTER(C.c_size_t)]),
     "bigru_tc_gemm": (_i, [_i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _i64, _vp, _i64, _i64, _i, _i, _vp, C.POINTER(_i), _vp]),
     "bigru_forward": (_i, [_vp, _vp, _vp, _vp, _f, _i, _i, _u64, _vp, _vp, _vp, _vp, _vp]),

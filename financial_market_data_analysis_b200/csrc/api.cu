@@ -310,6 +310,16 @@ extern "C" int bigru_scan_geometry(const bigru_plan* p, int scan, int* R, int* n
     return tc_scan_geometry(*p, scan, R, n_split);
 }
 
+// the lowest layer the backward runs (test support; see the header): the scratch then holds that layer's intermediates
+extern "C" int bigru_plan_set_backward_stop(bigru_plan* p, int layer) {
+    if (!p || layer < 0 || layer >= p->L) {
+        bigru_set_error("plan_set_backward_stop: bad plan or layer %d", layer);
+        return BIGRU_ERR_ARG;
+    }
+    p->bwd_stop = layer;
+    return BIGRU_OK;
+}
+
 // where a forward or backward intermediate lives inside the stash or the scratch (test support; see the header for the
 // regions and when each is valid)
 extern "C" int bigru_workspace_region(const bigru_plan* p, int which, int layer, int* in_scratch, size_t* byte_offset,
@@ -322,12 +332,14 @@ extern "C" int bigru_workspace_region(const bigru_plan* p, int which, int layer,
                         which == BIGRU_WS_DGH_PLANES || (which == BIGRU_WS_RD_STATE && p->prec != BIGRU_PREC_FP32);
     const bool rd = which == BIGRU_WS_RD_MASK || which == BIGRU_WS_RD_STATE;    // plans with recurrent dropout only
     const bool stashed = which == BIGRU_WS_GATES || which == BIGRU_WS_Y_PLANES || which == BIGRU_WS_IN_PLANES || rd;
-    // stash regions exist for every layer; the scratch keeps layer 0's recurrence gradients, the upstream gradients of layers
-    // 0 and 1 and the head's dcat (layer L, as in bigru_param_offset).  A head-less plan has no dcat, and its top layer's
-    // upstream gradient is the caller's d_dy
+    // stash regions exist for every layer; the scratch keeps the recurrence gradients of the last layer the backward ran (its
+    // stop s), the upstream gradients of the two layers whose ping-pong buffers survive ({0, 1} at stop 0, else {s-1, s}) and
+    // the head's dcat (layer L, as in bigru_param_offset).  A head-less plan has no dcat, and its top layer's upstream
+    // gradient is the caller's d_dy
+    const int s = p->bwd_stop, dy_lo = s > 0 ? s - 1 : 0;
     const bool layer_ok = stashed ? layer >= 0 && layer < p->L
-                        : which == BIGRU_WS_DY ? layer >= 0 && layer < p->L && layer < 2 && (has_head(*p) || layer < p->L - 1)
-                        : which == BIGRU_WS_DCAT ? layer == p->L && has_head(*p) : layer == 0;
+                        : which == BIGRU_WS_DY ? layer >= dy_lo && layer <= dy_lo + 1 && layer < p->L && (has_head(*p) || layer < p->L - 1)
+                        : which == BIGRU_WS_DCAT ? layer == p->L && has_head(*p) : layer == s;
     if (which < 0 || which >= BIGRU_WS_COUNT || !layer_ok || (rd && !(p->rp > 0.f))) {
         bigru_set_error("workspace_region: bad region %d or layer %d", which, layer);
         return BIGRU_ERR_ARG;
@@ -592,7 +604,8 @@ static int forward_plan(const bigru_plan& p, const float* params, const float* x
 }
 
 // ------------------------------------------------------------------------------------------
-// backward: the head, then layers L-1 .. 0.  The upstream gradient of layer l lives in dYa when L-1-l is even, else in dYb.
+// backward: the head, then layers L-1 .. 0 (.. bwd_stop: layers below keep zero gradients and write no dx, no dh0).  The
+// upstream gradient of layer l lives in dYa when L-1-l is even, else in dYb.
 // A plan without a head skips the head: its top layer reads its output from y and its upstream gradient from dy, and
 // layer l's carry starts from dhn's slice l (the gradient of h_n; null: zero) instead of the head's d(last) or zero.
 // ------------------------------------------------------------------------------------------
@@ -628,7 +641,7 @@ static int backward_plan(const bigru_plan& p, const float* params, const float* 
         TRY(colsum_launch(dlogits, grads + p.off_linb(), B, C, C, 1, 0, 0, scratch + W.csum, st));
         KLAUNCH(KC_HEAD, 0.0, 0.0, st, head_bwd_dy_kernel<<<nblk(BT * H, 256), 256, 0, st>>>(scratch + W.dcat, (const int*)(stash + S.arg), scratch + W.dYa, dhc, B, T, H, D, len));
     }
-    for (int l = p.L - 1; l >= 0; --l) {
+    for (int l = p.L - 1; l >= p.bwd_stop; --l) {
         const int I = (int)p.in_size(l);
         const bool even = (p.L - 1 - l) % 2 == 0;
         const bool drop_l = input_dropped(p, do_drop, l);

@@ -30,6 +30,7 @@ static inline int64_t cdiv64(int64_t a, int64_t b) { return (a + b - 1) / b; }
 struct bigru_plan {
     int B, T, F, H, L, C, D, prec;
     float rp;                      // recurrent dropout p (bigru_plan_create_rd); 0: none
+    int bwd_stop = 0;              // lowest layer the backward runs (bigru_plan_set_backward_stop, test support); 0: all
     int64_t nparams;
     int64_t layer_dir_stride[8];   // unused for L>8; offsets are computed on demand
     size_t stash_bytes, scratch_bytes;

@@ -115,12 +115,14 @@ int  bigru_stash_output_offset(const bigru_plan* plan, int layer, size_t* byte_o
  *   BIGRU_WS_Y_PLANES       stash    0..L-1     planes of Y [B*T][D*H]; bigru_forward
  *   BIGRU_WS_IN_PLANES      stash    0..L-1     planes of the layer's own input [B*T][rup(I_l, 8)], zero-padded columns;
  *                                               bigru_forward, layer 0 always, layers above only in training with dropout
- *   BIGRU_WS_DGI, _DGH      scratch  0          dgi, dgh [D][B*T][3H] fp32 of layer 0; bigru_backward (each layer reuses them)
- *   BIGRU_WS_DGI_PLANES,    scratch  0          their planes; dgi's n-gate rows hold dan, the dgh rows are zero at each
+ *   BIGRU_WS_DGI, _DGH      scratch  s          dgi, dgh [D][B*T][3H] fp32 of layer s, the backward stop (0 unless
+ *                                               bigru_plan_set_backward_stop set it); bigru_backward (each layer reuses them)
+ *   BIGRU_WS_DGI_PLANES,    scratch  s          their planes; dgi's n-gate rows hold dan, the dgh rows are zero at each
  *   BIGRU_WS_DGH_PLANES                         sequence's first step (t = 0 forward, t = T-1 reverse); bigru_backward.
  *                                               With lengths, these and the Y planes are zero at padded steps
- *   BIGRU_WS_DY             scratch  0, 1       upstream gradient of the layer's output [B*T][D*H]; bigru_backward
- *   BIGRU_WS_DHC            scratch  0          dh_{-1} of layer 0 [D][B][H]; bigru_backward
+ *   BIGRU_WS_DY             scratch  0, 1       upstream gradient of the layer's output [B*T][D*H]; bigru_backward.  The
+ *                                               two ping-pong buffers: at a stop s > 0 they hold layers s-1 and s instead
+ *   BIGRU_WS_DHC            scratch  s          dh_{-1} of layer s [D][B][H]; bigru_backward
  *   BIGRU_WS_DCAT           scratch  L (head)   d cat [B][3H] (last | max | mean); bigru_backward
  *   BIGRU_WS_RD_MASK        stash    0..L-1     recurrent-dropout masks m [D][B][H] fp32; training bigru_forward, plans with
  *                                               recurrent_p > 0 only
@@ -142,6 +144,12 @@ int  bigru_stash_output_offset(const bigru_plan* plan, int layer, size_t* byte_o
 #define BIGRU_WS_COUNT      12
 int  bigru_workspace_region(const bigru_plan* plan, int which, int layer, int* in_scratch, size_t* byte_offset,
                             size_t* lo_byte_offset, int64_t* pitch);
+
+/* --- Backward stop (test support): every later backward call on the plan (bigru_backward*, bigru_gru_backward) runs the
+ *  head and layers L-1 .. layer, then returns, so that the scratch regions above hold layer `layer`'s intermediates.
+ *  d_grads is still zeroed first: the gradients of the layers below stay 0, and d_dx and their d_dh0 slices are not
+ *  written.  Plans start at 0, the whole backward.  A null plan or a layer outside [0, L): BIGRU_ERR_ARG. */
+int  bigru_plan_set_backward_stop(bigru_plan* plan, int layer);
 
 /* --- Recurrence scan geometry of a tensor-core plan on the current device (test support).  *R: clusters of the scan the
  *  device holds at once.  scan 0, the forward (training instantiation): *n_split = clusters that take two 16-row batch

@@ -1,6 +1,6 @@
 """Drives the library's C ABI on one plan and takes the result apart tensor by tensor.  Test infrastructure, shared by
-test_gpu_rounding_model.py, test_gpu_fp32_path.py, test_gpu_tc_steps.py, test_gpu_scan_tiles.py, test_gpu_rd_steps.py and
-test_gpu_gru_steps.py.
+test_gpu_rounding_model.py, test_gpu_fp32_path.py, test_gpu_tc_steps.py, test_gpu_scan_tiles.py, test_gpu_rd_steps.py,
+test_gpu_gru_steps.py and test_gpu_layer_steps.py.
 
 A shape is a dict with B, T, F, H, L, C, D (1 or 2) and h0 (bool).  `kernel` runs bigru_forward and bigru_backward at a
 precision ("fp32", "bf16" or "bf16x3"), optionally with dropout, recurrent dropout and per-sequence lengths, and returns
@@ -11,7 +11,8 @@ and each backward GEMM from the kernel's own operands, `plane_checks` the bf16 p
 tensors.  The models take optional recurrent-dropout masks and lengths (DESIGN.md §4.8, §4.5); without them they are the
 models of the plain path, operation for operation.  With head=False the plan is a head-less one (bigru_gru_*, the nn.GRU
 drop-in): the top layer's output and upstream gradient are the caller's y and dy, each layer's carry starts from the
-caller's dhn, and there are no logits, pooling routing, dcat or head GEMMs."""
+caller's dhn, and there are no logits, pooling routing, dcat or head GEMMs.  With layer=l (kernel: the backward stops after
+layer l) the backward models are those of layer l, fed that layer's operands."""
 import ctypes as C
 
 import numpy as np
@@ -94,12 +95,21 @@ def _bits_to_f32(u16):
     return (u16.astype(np.uint32) << np.uint32(16)).view(np.float32)
 
 
-def _workspace(plan, s, prec, stash, scratch, rd=False, head=True):
+def dy_layers(L, layer):
+    """The layers whose upstream gradient survives a backward stopped at `layer` (BIGRU_WS_DY of include/bigru_b200.h):
+    the two ping-pong buffers hold layers 0 and 1 at stop 0, layers layer-1 and layer above it."""
+    lo = layer - 1 if layer > 0 else 0
+    return [l for l in (lo, lo + 1) if l < L]
+
+
+def _workspace(plan, s, prec, stash, scratch, rd=False, head=True, layer=0):
     """The backward's operands and intermediates (bigru_workspace_region) as host arrays: fp32 regions as float32, planes
     as (hi, lo) pairs of bf16 bit patterns (uint16; lo None at bf16; both None at fp32, which keeps no planes).  Rows are
     split into [B, T] (and a leading D where there is one).  rd: also every layer's recurrent-dropout masks RDM [D, B, H]
     and masked state RDS [B, T, D*H] (planes, or float32 at fp32).  head=False: DCAT and the top layer's DY, which a
-    head-less plan refuses (its top layer's upstream gradient is the caller's dy), are None."""
+    head-less plan refuses (its top layer's upstream gradient is the caller's dy), are None.  layer: the layer the backward
+    stopped at, whose dgi, dgh, their planes and dh_{-1} the scratch holds; XP is that layer's own input planes and DY[l]
+    is None for every layer but those of dy_layers."""
     B, T, F, H, L, D = (s[k] for k in "BTFHLD")
     bufs = (stash, scratch)
 
@@ -117,14 +127,16 @@ def _workspace(plan, s, prec, stash, scratch, rd=False, head=True):
         get = lambda o: v[o // 2: o // 2 + n].view(*shape).cpu().numpy().view(np.uint16)   # noqa: E731
         return get(off), (get(lo) if prec == "bf16x3" else None)
 
-    pitch0 = region(plan, "IN_PLANES", 0)[4]
+    pitch = region(plan, "IN_PLANES", layer)[4]
+    keep = dy_layers(L, layer)
     ws = dict(G=[f32("GATES", l, (D, B, T, 4 * H)) for l in range(L)],
               YP=[planes("Y_PLANES", l, (B, T, D * H)) for l in range(L)],
-              XP=planes("IN_PLANES", 0, (B, T, pitch0)),
-              DGI=f32("DGI", 0, (D, B, T, 3 * H)), DGH=f32("DGH", 0, (D, B, T, 3 * H)),
-              DGIP=planes("DGI_PLANES", 0, (D, B, T, 3 * H)), DGHP=planes("DGH_PLANES", 0, (D, B, T, 3 * H)),
-              DY=[f32("DY", l, (B, T, D * H)) if head or l < L - 1 else None for l in range(min(L, 2))],
-              DHC=f32("DHC", 0, (D, B, H)), DCAT=f32("DCAT", L, (B, 3 * H)) if head else None)
+              XP=planes("IN_PLANES", layer, (B, T, pitch)),
+              DGI=f32("DGI", layer, (D, B, T, 3 * H)), DGH=f32("DGH", layer, (D, B, T, 3 * H)),
+              DGIP=planes("DGI_PLANES", layer, (D, B, T, 3 * H)), DGHP=planes("DGH_PLANES", layer, (D, B, T, 3 * H)),
+              DY=[f32("DY", l, (B, T, D * H)) if l in keep and (head or l < L - 1) else None
+                  for l in range(L if layer else min(L, 2))],
+              DHC=f32("DHC", layer, (D, B, H)), DCAT=f32("DCAT", L, (B, 3 * H)) if head else None)
     if rd:
         ws["RDM"] = [f32("RD_MASK", l, (D, B, H)) for l in range(L)]
         ws["RDS"] = [(f32("RD_STATE", l, (B, T, D * H)), None) if prec == "fp32" else planes("RD_STATE", l, (B, T, D * H))
@@ -133,10 +145,12 @@ def _workspace(plan, s, prec, stash, scratch, rd=False, head=True):
 
 
 def kernel(s, prec, flat, x, h0, dl, p=0.0, spatial=False, seed=0, regions=False, rd_p=0.0, lens=None, head=True, dy=None,
-           dhn=None):
+           dhn=None, layer=0):
     """bigru_forward_lengths + bigru_backward_lengths of shape s at precision prec on a bigru_plan_create_rd plan (p = 0:
     bigru_plan_create's plan); dropout p and recurrent dropout rd_p (training mode when either is on); lens: per-row
-    lengths [B] or None.  regions: the result also holds "ws", the intermediates of _workspace.
+    lengths [B] or None.  regions: the result also holds "ws", the intermediates of _workspace.  layer > 0: the backward
+    stops after that layer (bigru_plan_set_backward_stop), so that "ws" holds its intermediates; the gradients of the
+    layers below are 0, and dx and their dh0 slices stay zero.
     head=False: bigru_gru_forward + bigru_gru_backward on a bigru_gru_plan_create_rd plan (flat is the recurrent prefix, dl
     and spatial are unused, p drops only between layers).  dy [B, T, D*H] is the gradient of the top layer's output (None:
     zeros, as GRU passes it), dhn [L*D, B, H] that of h_n (None: no gradient).  ys then takes the top layer from d_y, and
@@ -150,6 +164,8 @@ def kernel(s, prec, flat, x, h0, dl, p=0.0, spatial=False, seed=0, regions=False
     else:
         L_.check(lib.bigru_gru_plan_create_rd(B, T, F, H, L, int(D == 2), CODE[prec], rd_p, C.byref(plan)), "gru_plan_create")
     try:
+        if layer:
+            L_.check(lib.bigru_plan_set_backward_stop(plan, layer), "plan_set_backward_stop")
         sb, cb = C.c_size_t(), C.c_size_t()
         L_.check(lib.bigru_workspace_bytes(plan, C.byref(sb), C.byref(cb)), "workspace_bytes")
         dev = torch.device("cuda")
@@ -195,7 +211,7 @@ def kernel(s, prec, flat, x, h0, dl, p=0.0, spatial=False, seed=0, regions=False
                                             ptr(dyd), ptr(dhnd), ptr(grads), ptr(dx), ptr(dh0), ptr(lend), st), "gru_backward")
         torch.cuda.synchronize()
         names = param_names(plan, s, head)
-        ws = _workspace(plan, s, prec, stash, scratch, rd=rd_p > 0, head=head) if regions else None
+        ws = _workspace(plan, s, prec, stash, scratch, rd=rd_p > 0, head=head, layer=layer) if regions else None
         del stash, scratch
     finally:
         lib.bigru_plan_destroy(plan)
@@ -393,7 +409,8 @@ def head_dy(s, dcat, arg, lens=None):
     return np.concatenate([v] * D, 2)
 
 
-def backward_steps(s, prec, flat, h0, ws, ys, names, own=False, masks=None, lens=None, head=True, dy=None, dhn=None):
+def backward_steps(s, prec, flat, h0, ws, ys, names, own=False, masks=None, lens=None, head=True, dy=None, dhn=None,
+                   layer=0):
     """Layer 0's backward recurrence one step at a time in float64, following gru_scan_bwd_kernel (tc_hopper.cuh), per
     direction in the kernel's step order.  Each step takes the kernel's own operands: its dY (ws["DY"][0]), its gates
     (ws["G"][0]) and its h_{t-1} (ys[0], or h0), and
@@ -409,20 +426,23 @@ def backward_steps(s, prec, flat, h0, ws, ys, names, own=False, masks=None, lens
     fp32 path masks it into dh0 later; the scans' dh_{-1} is masked).  lens: a padded step has dgi = dgh = 0 and passes the
     carry on unchanged and unmasked.
     head=False (a head-less plan): the carry of direction d starts from the caller's dhn[0*D + d] (None: zero), and when
-    layer 0 is the top layer (L = 1) its dY is the caller's dy (None: zero) rather than a workspace region."""
+    layer 0 is the top layer (L = 1) its dY is the caller's dy (None: zero) rather than a workspace region.
+    layer: the same for layer l: its dY ws["DY"][l] (on a head-less plan's top layer the caller's dy), its gates ws["G"][l],
+    its h_{t-1} from ys[l] or h0[l*D + d], W_hh of layer l; the carry starts from the head's `last` share when l = L-1, from
+    dhn[l*D + d] on a head-less plan, else from zero.  masks are then layer l's."""
     B, T, H, L, D = (s[k] for k in "BTHLD")
-    if head or L > 1:
-        dYall = ws["DY"][0]
+    if head or layer < L - 1:
+        dYall = ws["DY"][layer]
     else:
         dYall = np.zeros((B, T, D * H)) if dy is None else dy
     for d in range(D):
-        w = split(_block(flat, names, f"l0d{d}.w_hh", (3 * H, H)), prec)        # P[b, k] = sum_q dgh[b, q] W[q, k]
-        G, y, dY = ws["G"][0][d], ys[0][:, :, d * H:(d + 1) * H], dYall[:, :, d * H:(d + 1) * H]
+        w = split(_block(flat, names, f"l{layer}d{d}.w_hh", (3 * H, H)), prec)   # P[b, k] = sum_q dgh[b, q] W[q, k]
+        G, y, dY = ws["G"][layer][d], ys[layer][:, :, d * H:(d + 1) * H], dYall[:, :, d * H:(d + 1) * H]
         if not head:
-            carry = np.zeros((B, H)) if dhn is None else np.asarray(dhn[d], np.float64)
+            carry = np.zeros((B, H)) if dhn is None else np.asarray(dhn[layer * D + d], np.float64)
         else:
-            carry = ws["DCAT"][:, :H].astype(np.float64) if L == 1 else np.zeros((B, H))
-        start = np.zeros((B, H)) if h0 is None else h0[d].astype(np.float64)
+            carry = ws["DCAT"][:, :H].astype(np.float64) if layer == L - 1 else np.zeros((B, H))
+        start = np.zeros((B, H)) if h0 is None else h0[layer * D + d].astype(np.float64)
         raw = None
         for st in range(T):
             t = T - 1 - st if d == 0 else st
@@ -452,7 +472,7 @@ def backward_steps(s, prec, flat, h0, ws, ys, names, own=False, masks=None, lens
         yield "dh0", d, None, carry, raw
 
 
-def gemm_steps(s, prec, flat, dl, h0, ops, names, arg, masks=None, lens=None, head=True):
+def gemm_steps(s, prec, flat, dl, h0, ops, names, arg, masks=None, lens=None, head=True, layer=0, drop=None):
     """Every backward GEMM of layer 0 and of the head in float64, from the operands the kernels read: `ops` holds the dgi
     and dgh planes (DGIP, DGHP: (hi, lo) [D, B, T, 3H]), the layer input's planes (XP [B, T, pitch]), the Y planes of layer
     0 (YP [B, T, D*H]), fp32 dgi and dgh (DGI, DGH [D, B, T, 3H]) and the kernel's dcat.  Returns (name, "gemm_step") ->
@@ -466,23 +486,29 @@ def gemm_steps(s, prec, flat, dl, h0, ops, names, arg, masks=None, lens=None, he
                          layers 0 and 1).
     masks: layer 0's recurrent-dropout masks [D, B, H]: dW_hh takes the masked-state planes ops["RDS"] instead of the Y
     planes, and its w0 term m * h0 (_masked).  lens: as head_dy.  head=False: no dcat and no head dy (dl, arg and
-    ops["DCAT"] are unused); the top layer's upstream gradient is the caller's."""
+    ops["DCAT"] are unused); the top layer's upstream gradient is the caller's.
+    layer: the GEMMs of layer l: XP is then its input's planes (the Y planes of layer l-1 [B, T, D*H], or its own input
+    planes when its input was dropped), YP (or RDS) layer l's, h0 the whole [L*D, B, H] state (its slices l*D + d enter
+    the w0 term) and masks layer l's.  Its dX is grad "dy[l{l-1}]" instead of dx.  drop: the float32 factor dropout_kernel
+    multiplied the layer's input by (dropout_mask), or None: the dX GEMM's result is multiplied by it, as the in-place
+    dropout backward does.  The head's dy[l{L-1}] is compared only when that layer is one of dy_layers."""
     B, T, F, H, L, D = (s[k] for k in "BTFHLD")
     BT = B * T
+    I = F if layer == 0 else D * H
     flat2 = lambda p, d=None: tuple(None if a is None else (a if d is None else a[d]).reshape(BT, -1) for a in p)   # noqa: E731
     xp, yp = flat2(ops["XP"]), flat2(ops["YP"] if masks is None else ops["RDS"])
     t_of = np.arange(BT) % T
-    dx = np.zeros((BT, F))
+    dx = np.zeros((BT, I))
     out = {}
     for d in range(D):
         gi, gh = flat2(ops["DGIP"], d), flat2(ops["DGHP"], d)
-        w_ih = split(_block(flat, names, f"l0d{d}.w_ih", (3 * H, F)), prec)
-        dwih, dwhh = np.zeros((3 * H, F)), np.zeros((3 * H, H))
+        w_ih = split(_block(flat, names, f"l{layer}d{d}.w_ih", (3 * H, I)), prec)
+        dwih, dwhh = np.zeros((3 * H, I)), np.zeros((3 * H, H))
         # K = B*T in chunks of rows, so that no float64 copy of a whole plane is made
         for r0 in range(0, BT, 8192):
             sl = slice(r0, min(BT, r0 + 8192))
             a, c = rows64(gi, sl), rows64(gh, sl)
-            dwih += pmm(tr(a), rows64(xp, sl, slice(0, F)))
+            dwih += pmm(tr(a), rows64(xp, sl, slice(0, I)))
             # H_prev(b, t) = Y(b, t - 1) forward, Y(b, t + 1) reverse: rows shifted by one; where that leaves the sequence
             # the dgh planes are zero (and so is H_prev here)
             src = np.arange(sl.start, sl.stop) + (-1 if d == 0 else 1)
@@ -492,34 +518,45 @@ def gemm_steps(s, prec, flat, dl, h0, ops, names, arg, masks=None, lens=None, he
             dx[sl] += pmm(a, w_ih)
         if h0 is not None:
             tf = 0 if d == 0 else T - 1
-            h0d = h0[d] if masks is None else _masked(masks[d], h0[d], prec)
+            h0l = h0[layer * D + d]
+            h0d = h0l if masks is None else _masked(masks[d], h0l, prec)
             dwhh += pmm(tr(split(ops["DGH"][d][:, tf], prec)), split(h0d, prec))
-        out[(f"gemm:grad:l0d{d}.w_ih", "gemm_step")] = dwih.ravel()
-        out[(f"gemm:grad:l0d{d}.w_hh", "gemm_step")] = dwhh.ravel()
-        out[(f"gemm:grad:l0d{d}.b_ih", "gemm_step")] = ops["DGI"][d].reshape(BT, 3 * H).astype(np.float64).sum(0)
-        out[(f"gemm:grad:l0d{d}.b_hh", "gemm_step")] = ops["DGH"][d].reshape(BT, 3 * H).astype(np.float64).sum(0)
-    out[("gemm:dx", "gemm_step")] = dx.reshape(B, T, F)
+        pre = f"gemm:grad:l{layer}d{d}"
+        out[(f"{pre}.w_ih", "gemm_step")] = dwih.ravel()
+        out[(f"{pre}.w_hh", "gemm_step")] = dwhh.ravel()
+        out[(f"{pre}.b_ih", "gemm_step")] = ops["DGI"][d].reshape(BT, 3 * H).astype(np.float64).sum(0)
+        out[(f"{pre}.b_hh", "gemm_step")] = ops["DGH"][d].reshape(BT, 3 * H).astype(np.float64).sum(0)
+    dx = dx.reshape(B, T, I)
+    if drop is not None:
+        dx = dx * drop
+    out[(_dx_name(layer), "gemm_step")] = dx
     if not head:
         return out
     out[("gemm:dcat", "gemm_step")] = head_dcat(s, prec, flat, dl, names)
-    if L <= 2:
+    if L - 1 in dy_layers(L, layer):
         out[(f"gemm:dy[l{L - 1}]", "gemm_step")] = head_dy(s, ops["DCAT"].astype(np.float64), arg, lens)
     return out
 
 
-def kernel_gemm_steps(got, s, names, head=True):
+def _dx_name(layer):
+    """The gradient layer l's dX GEMM writes: dx at layer 0, else the upstream gradient of layer l-1."""
+    return "gemm:dx" if layer == 0 else f"gemm:dy[l{layer - 1}]"
+
+
+def kernel_gemm_steps(got, s, names, head=True, layer=0):
     """The kernel's side of gemm_steps."""
     out = {}
+    L = s["L"]
     for d in range(s["D"]):
         for nm in ("w_ih", "w_hh", "b_ih", "b_hh"):
-            o, k = names[f"l0d{d}.{nm}"]
-            out[(f"gemm:grad:l0d{d}.{nm}", "gemm_step")] = got["grads"][o:o + k]
-    out[("gemm:dx", "gemm_step")] = got["dx"]
+            o, k = names[f"l{layer}d{d}.{nm}"]
+            out[(f"gemm:grad:l{layer}d{d}.{nm}", "gemm_step")] = got["grads"][o:o + k]
+    out[(_dx_name(layer), "gemm_step")] = got["dx"] if layer == 0 else got["ws"]["DY"][layer - 1].astype(np.float64)
     if not head:
         return out
     out[("gemm:dcat", "gemm_step")] = got["ws"]["DCAT"].astype(np.float64)
-    if s["L"] <= 2:
-        out[(f"gemm:dy[l{s['L'] - 1}]", "gemm_step")] = got["ws"]["DY"][s["L"] - 1].astype(np.float64)
+    if L - 1 in dy_layers(L, layer):
+        out[(f"gemm:dy[l{L - 1}]", "gemm_step")] = got["ws"]["DY"][L - 1].astype(np.float64)
     return out
 
 
@@ -530,11 +567,21 @@ def _split_bits(v32, prec):
     return bits(hi), (bits(bf16(v32 - hi)) if prec == "bf16x3" else None)
 
 
-def plane_checks(got, s, prec, x, masks=None, lens=None, drop=False):
+def dropped(v, factor):
+    """dropout_kernel's output restated: +0 where the element is dropped (factor 0), else the float32 product v * factor."""
+    v32 = np.asarray(v, np.float32)
+    return np.where(factor == 0, np.float32(0), v32 * factor).astype(np.float32)
+
+
+def plane_checks(got, s, prec, x, masks=None, lens=None, drop=False, layer=0):
     """Elements (hi and lo together) where a plane the kernels wrote differs bitwise from split_bf16 of its fp32 source:
     the Y planes of every layer; layer 0's input planes (x, zero-padded to the pitch; the dropped x under dropout with a
     head, the undropped x on a head-less plan, whose dropout never touches x: pass that x); the dgi
     planes; the dgh planes, zero at each sequence's first step.  name -> count; all must be 0.
+    layer: the layer the backward stopped at (kernel's layer): the dgi / dgh planes are that layer's, and its input planes
+    are checked against x, the layer's dropped input dropped(Y[l-1], factor), when the layer owns them (x None: it reads
+    the Y planes of layer l-1 and has none).  With h0 (got["dh0"]) the scratch's dh_{-1} must equal the caller's
+    dh0[l*D + d] bit for bit.
     masks: the host restatement of the recurrent-dropout masks [L, D, B, H] (rd_masks).  Then the masks in the stash must
     equal them, RDS[l] must be split_bf16 of fp32(m * Y) (at fp32 the float32 product itself; only these two at fp32), and
     the Y planes exist only for a layer below the top whose next layer reads them (to_planes_kernel): not where that layer
@@ -562,10 +609,13 @@ def plane_checks(got, s, prec, x, masks=None, lens=None, drop=False):
     for l, y in enumerate(got["ys"]):
         if masks is None or (l + 1 < s["L"] and not drop):
             out[f"Y_PLANES[l{l}]"] = cmp(ws["YP"][l], _split_bits(y.astype(np.float32), prec))
-    xw = np.zeros(ws["XP"][0].shape, np.float32)
-    xw[..., :F] = x
-    hi, lo = _split_bits(xw, prec)
-    out["IN_PLANES[l0]"] = cmp(ws["XP"], (hi, lo))
+    if x is not None:
+        xw = np.zeros(ws["XP"][0].shape, np.float32)
+        xw[..., :x.shape[2]] = x
+        hi, lo = _split_bits(xw, prec)
+        out[f"IN_PLANES[l{layer}]"] = cmp(ws["XP"], (hi, lo))
+    if got["dh0"] is not None:
+        out[f"DHC=dh0[l{layer}]"] = bad(ws["DHC"].astype(np.float64), got["dh0"][layer * D:(layer + 1) * D])
     padded = None if lens is None else np.arange(T)[None, :] >= np.asarray(lens)[:, None]
     want = [p.copy() if p is not None else None for p in _split_bits(ws["DGI"], prec)]
     if padded is not None:

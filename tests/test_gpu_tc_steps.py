@@ -12,8 +12,9 @@ gru_driver recomputes in float64, from exactly those bits:
   gemm_step every backward GEMM of layer 0 and of the head from the kernel's operand planes (gemm_steps): dW_ih, dW_hh
             with its h0 term, the bias column sums, dx, dcat and the top layer's dY;
 plus y_step, logits_step and w_step of the forward, as in the sibling file.  The planes themselves must equal split_bf16
-of their fp32 sources bit for bit.  Upper layers' dgi / dgh are not kept by the scratch (each layer reuses it): they keep
-only the free-running check of test_gpu_rounding_model.py.
+of their fp32 sources bit for bit.  The scratch keeps only the last layer the backward ran (each layer reuses it), so
+this file checks layer 0; test_gpu_layer_steps.py stops the backward at each upper layer (bigru_plan_set_backward_stop)
+and checks that layer's steps and GEMMs the same way.
 
 configs[1] runs at full size (B512 T128 F64 H256 L2 D2) without the free-running oracle: its forward steps are sampled by
 batch tile (the first, second and last 16-row tile, every step; configs[4]'s T = 1024 shape the first tile), its backward
